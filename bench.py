@@ -1,7 +1,7 @@
 #!/usr/bin/env python3
-"""bench.py — the discovery-scan benchmark (contract: see the task statement / DESIGN.md §Measurement).
+"""bench.py — the discovery-scan benchmark (see DESIGN.md §5).
 
-  python bench.py [--gpus N --steps K --warmup W] [--impl reference] [--records R]
+  python bench.py [--gpus N --steps K --warmup W] [--impl reference] [--records R] [--dump-outputs DIR]
 
 One "step" = one pass of the hot path over one batch of synthetic input:
   parse the full utils/pci.ids image (1,536,458 B) into the name table  +  classify / compact /
@@ -16,6 +16,9 @@ value   records/s with inputs resident in HBM (CUDA events on the launching stre
         between steps, max over ranks)
 e2e     the same metric through the reference-facing C-ABI calls (kvg_pciids_load + kvg_scan_pci)
         with PINNED HOST buffers in and host results out, copies inside the timed region
+
+--dump-outputs DIR writes the result of the last timed step (the arrays a caller of the scan receives) as
+DIR/<name>.npy in float64, so that two builds can be compared output for output on the same seeded inputs.
 """
 import argparse
 import gzip
@@ -43,11 +46,7 @@ def load_pciids() -> bytes:
 
 
 def peaks():
-    try:
-        with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
-            return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3)"
 
 
 class ClockSampler:
@@ -146,6 +145,33 @@ def _check_ordering(members, field, keys, off, perm, what):
         raise AssertionError("parity: %s ordering differs from a stable sort" % what)
 
 
+DUMP_BYTES = 64 << 20
+
+
+def _pci_result_arrays(res, prefix=""):
+    """name -> 1-D array of what a caller of the PCI scan receives in `res` (kvgpu.PciResult)."""
+    out = {prefix + "survivors_" + f: res.survivors[f] for f in res.survivors.dtype.names}
+    for f in ("dev_keys", "dev_off", "dev_perm", "dev_name_slot", "grp_keys", "grp_off", "grp_perm"):
+        out[prefix + f] = getattr(res, f)
+    out[prefix + "name_pool"] = np.frombuffer(res.name_pool, dtype=np.uint8)
+    return out
+
+
+def dump_outputs(path, arrays, budget=DUMP_BYTES):
+    """Write every array as <path>/<name>.npy in float64 (exact for the u32 values of the scan).  Above `budget` bytes
+    in all, an array longer than its equal share of the budget is replaced by the elements at a fixed, seeded sample
+    of positions (ascending; the same positions for every array of that length)."""
+    os.makedirs(path, exist_ok=True)
+    head = 256 * len(arrays)   # .npy headers
+    cap = (budget - head) // 8 // max(1, len(arrays))
+    over = sum(np.asarray(a).size for a in arrays.values()) * 8 + head > budget
+    for name, a in arrays.items():
+        a = np.asarray(a).reshape(-1)
+        if over and a.size > cap:
+            a = a[np.sort(np.random.default_rng(0).choice(a.size, cap, replace=False))]
+        np.save(os.path.join(path, name + ".npy"), a.astype(np.float64))
+
+
 def check_parity(ctx, sharded, rank, world, n, ids, gbits, text, O):
     """Exact check of THIS run's output before anything is timed.  N = 1: the fetched result of kvg_dev_scan_pci;
     N > 1: this rank's part of the sharded scan — its shard's survivors, and ALL members of the device ids /
@@ -242,6 +268,9 @@ def main():
                     help="records for the HBM-bound roofline leg (N=1 only; 0 disables)")
     ap.add_argument("--big-files", type=int, default=256,
                     help="pci.ids images for the HBM-bound parse roofline leg (0 disables)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the result of the last timed step as DIR/<name>.npy (float64, at most 64 MB; "
+                         "N > 1: one rank<r>_ prefix per rank)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else args.warmup
 
@@ -344,6 +373,18 @@ def main():
     launches = ctx.launch_count - launches0 - args.steps  # minus the flush fills
     dev_ms = sum(a.elapsed_time(b) for a, b in evs)
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs:   # the last timed step's result, fetched after the timing
+        info0 = ctx.pciids_info()
+        out = {"pciids_info": np.array([info0[k] for k in ("vendor_off", "section_end", "n_entries", "n_lines")])}
+        if sharded is None:
+            out.update(_pci_result_arrays(ctx.dev_scan_pci_fetch()))
+        else:
+            res = sharded.fetch()
+            out.update({"local_" + f: res.local[f] for f in res.local.dtype.names})
+            out.update(_pci_result_arrays(res.dev, "dev_part_"))
+            out.update(_pci_result_arrays(res.grp, "grp_part_"))
+            out = {"rank%d_%s" % (rank, k): v for k, v in out.items()}
+        dump_outputs(args.dump_outputs, out, DUMP_BYTES // world)
     if world > 1:
         t = torch.tensor([dev_ms], dtype=torch.float64, device="cuda")
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
@@ -393,22 +434,9 @@ def main():
     def roof(name, nbytes, ms, launches_per_step=1):
         ach = nbytes / (ms * 1e-3) / 1e9 if ms else 0.0
         return {"kernel": name, "bound": "hbm", "achieved": ach, "peak": hbm_peak, "unit": "GB/s",
-                "frac": ach / hbm_peak, "traffic": None, "algorithmic_bytes": nbytes,
+                "frac": ach / hbm_peak, "algorithmic_bytes": nbytes,
                 "avg_launch_ms": ms / launches_per_step, "peak_source": peak_src}
-    # DRAM traffic per launch from the committed ncu --set full captures (never measured here: a
-    # number taken under a profiler is not a bench number, and ncu is not run by bench.py)
-    try:
-        ncu_traffic = json.load(open(os.path.join(ROOT, "profiles", "r02_ncu_traffic.json")))
-    except (OSError, ValueError):
-        ncu_traffic = {}
-
-    def traffic_for(key):
-        t = ncu_traffic.get(key)
-        return t["bytes_per_launch"] if t else None
     roofline = roof(dominant, algo[dominant], ksum[dominant], nl[dominant])
-    if n == 1_000_000:
-        roofline["traffic"] = traffic_for(dominant + "@config2")
-        roofline["traffic_note"] = "per launch, from profiles/r02_ncu_traffic.json (ncu --set full capture of the same kernel and size)"
     roofline["share_of_step"] = ksum[dominant] / step_ms
     roofline["note"] = ("dominant kernel FAMILY of the step at this config (all its launches; per-kernel event timing "
                         "adds ~5 us per launch, so shares are indicative); at 1 M records every kernel is "
@@ -470,7 +498,6 @@ def main():
                   "whole_scan_contract": {"bytes": 16 * nb + 24 * Sb,
                                           "GBps": (16 * nb + 24 * Sb) / (whole_ms * 1e-3) / 1e9,
                                           "frac": (16 * nb + 24 * Sb) / (whole_ms * 1e-3) / 1e9 / hbm_peak}})
-        r["traffic"] = traffic_for("classify_compact@%d" % nb)
         roofline_big["classify_compact"] = r
         del big
     if world == 1 and args.big_files:
@@ -499,7 +526,6 @@ def main():
                                         "frac": nf * len(text) / (fam_ms * 1e-3) / 1e9 / hbm_peak,
                                         "what": "k_pciids_scan + k_pciids_resolve_finalize (the lines of the NVIDIA "
                                                 "block are recorded by the resolve pass)"}})
-        r["traffic"] = traffic_for("pciids_parse@%d" % nf)
         roofline_big["pciids_parse"] = r
         c2.close()
         del bigt
@@ -756,7 +782,7 @@ def main():
                        "exchange": None if world == 1 else sharded.mode,
                        "records_per_gpu": n, "survivors": S, "device_ids": KD, "iommu_groups": G,
                        "iommu_group_order": "bijective scramble of i>>1 (group_bits=%d)" % gbits,
-                       "l2": "flushed between timed steps (192 MiB fill, outside the event bracket)",
+                       "l2": "flushed between timed steps (128 MiB fill, outside the event bracket)",
                        "wall_s_timed_loop_incl_flush": t_wall},
             "pciids_parse_GBps": len(text) / (kavg.get("pciids_parse", 0) * 1e-3) / 1e9 if kavg.get("pciids_parse") else None,
             "parity": parity,

@@ -1,5 +1,5 @@
 /*
- * kvgpu.h — C-ABI of libkvgpu.so: the B200 (sm_100a) discovery-and-classification scan
+ * kvgpu.h — C-ABI of libkvgpu.so: the H100 (sm_90a) discovery-and-classification scan
  * that replaces the CPU scan of NVIDIA/kubevirt-gpu-device-plugin.
  *
  * The reference has NO FFI on this path today (it is pure Go).  The seam a maintainer binds is

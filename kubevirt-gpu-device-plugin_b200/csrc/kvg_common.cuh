@@ -1,4 +1,4 @@
-// kvg_common.cuh — device-side building blocks shared by every kernel of libkvgpu.so (sm_100a).
+// kvg_common.cuh — device-side building blocks shared by every kernel of libkvgpu.so (sm_90a).
 //
 //   * streaming global loads/stores (ld.global.nc.L1::no_allocate / st.global.L1::no_allocate)
 //   * mbarrier + 1-D TMA bulk copy (cp.async.bulk ... mbarrier::complete_tx::bytes -> SASS UBLKCP)

@@ -13,15 +13,15 @@
 //   k_order_final      latency-bound sizes: ONE launch, chained scan of the per-tile head counts
 //   k_order_heads<0/1> bandwidth-bound sizes: count -> k_tile_offsets -> emit (no CTA ever waits for another)
 //
-// Measured dead end (round 2, kept here so nobody repeats it): accumulating the histograms with global
-// REDs from the producers (one per survivor from the classify / pack kernel for pass 0, one per element
-// from the scatter for the next pass) removes the histogram launches but costs more than they do — +13 us
-// in the 1 M-record classify, +35 us in its pass-0 scatter (hot rows), +64 us in the 16.7 M-record pack.
+// Measured dead end (kept here so nobody repeats it): accumulating the histograms with global REDs from the
+// producers (one per survivor from the classify / pack kernel for pass 0, one per element from the scatter for
+// the next pass) removes the histogram launches but costs more than they do — in the 1 M-record classify, in
+// its pass-0 scatter (hot rows) and in the 16.7 M-record pack.
 //
-// Second measured dead end (round 2): the whole step as ONE persistent launch (the same device functions in a
-// grid that fits the GPU, 3 grid barriers per pass + 1 for the heads).  Correct (GPU suite green) but 7 us SLOWER
-// at 1 M records (0.121 vs 0.114 ms per step): seven barriers over ~440 CTAs cost more than the nine launch
-// boundaries they replace once those launches overlap through programmatic dependent launch.
+// Second measured dead end: the whole step as ONE persistent launch (the same device functions in a grid that
+// fits the GPU, 3 grid barriers per pass + 1 for the heads).  Correct (GPU suite green) but SLOWER at 1 M
+// records: seven grid barriers cost more than the nine launch boundaries they replace once those launches
+// overlap through programmatic dependent launch.
 //
 // Digit width is decided ON THE DEVICE from the largest key of the ordering: the fewest passes of at most
 // `max_bits` bits, the key bits split evenly between them (19-bit keys: 2 passes of 10 bits; 16-bit keys:

@@ -107,9 +107,9 @@ __global__ void __launch_bounds__(KVG_BLOCK) k_compact(Op op, uint64_t* tile_sta
 // of them, dispatched in blockIdx order by the hardware.  Many resident CTAs per SM hide the
 // count -> look-back -> write-out latency chain of each other; predecessors were dispatched
 // earlier, so the classic decoupled look-back usually finds an inclusive prefix close by.
-// (Measured alternative, round 2: every tile publishes its count and sums ALL earlier counts itself, a thread
-// per earlier tile — no chain, but 8 dependent L2 round trips per thread for the last tiles: 20.1 vs 14.9 us,
-// config-2 step 0.108 vs 0.097 ms.  The chained scan stays.)
+// (Measured alternative: every tile publishes its count and sums ALL earlier counts itself, a thread per
+// earlier tile — no chain, but several dependent L2 round trips per thread for the last tiles; it was slower
+// at 1 M records.  The chained scan stays.)
 // ------------------------------------------------------------------------------------------------
 template <class Op, int THREADS, int ROWS>
 __global__ void __launch_bounds__(THREADS) k_classify_oneshot(Op op, uint64_t* tile_state, uint32_t epoch) {
@@ -631,9 +631,9 @@ __global__ void k_fill32(uint32_t* __restrict__ p, size_t n, uint32_t v) {
 //                      survivor once, no waiting on other CTAs: this is the HBM-roofline kernel.
 //   k_tile_offsets     exclusive scan of the tile counts (one CTA; n_tiles is ~N/1024)
 //   k_pack_survivors   dense, order-preserving copy scratch -> survivors using the known offsets
-// A single-pass look-back compaction (k_classify_oneshot / _tma / _ws, kept for A/B measurements,
-// KVG_CLASSIFY=oneshot|tma|ws) moves fewer bytes but spends ~2/3 of each CTA's lifetime waiting
-// for its base offset; measured on B200 it is ~1.7x slower end to end than this split form.
+// The single-pass look-back compaction (k_classify_oneshot, used below 2 M records) moves fewer bytes,
+// but at sizes that are bandwidth-bound each of its CTAs spends most of its lifetime waiting for its
+// base offset, which makes it slower end to end than this split form there.
 // ------------------------------------------------------------------------------------------------
 template <class Op, int THREADS, int ROWS>
 __global__ void __launch_bounds__(THREADS) k_classify_ragged(Op op, uint32_t* __restrict__ tile_count,

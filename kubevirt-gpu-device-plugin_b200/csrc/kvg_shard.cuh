@@ -17,8 +17,8 @@
 //                   every survivor is stored at its final position of region `me` in its owner's window
 //                   (match.any ranks: stable), once per ordering; the last CTA to finish publishes the
 //                   region counts and a release flag (st.release.sys) in every peer's control block
-//                   (round 2 first had count / scan / send as three launches: two reads of the list and
-//                   ~15 us of launch gaps more)
+//                   (count / scan / send as three launches cost two more reads of the list and two more
+//                   launch gaps)
 //   k_shard_gather  waits for the P flags of the step (ld.acquire.sys), concatenates the P regions of each
 //                   ordering — source-rank order == Walk order — into the dense OWNED list the orderings
 //                   read, reduces the largest owned keys (radix plan), and the last CTA acknowledges the
@@ -222,10 +222,10 @@ __global__ void __launch_bounds__(KVG_BLOCK) k_shard_send(ShardArgs A, ShardPeer
 // CW4 = uint4 loads per tile row: 4 * CW4 >= 1 + 2P.
 constexpr uint32_t CS_COUNT_BITS = 11;
 #ifndef KVG_CS_MINB_WIDE
-#define KVG_CS_MINB_WIDE 7  // the same for P >= 4 (more counters: more registers in the prefix loop)
+#define KVG_CS_MINB_WIDE 7  // P >= 4 (more counters: more registers in the prefix loop); 8 would cap it at 64 registers
 #endif
 #ifndef KVG_CS_MINB
-#define KVG_CS_MINB 7  // CTAs per SM asked of the P <= 3 instantiation: 7 x 148 >= the 977 tiles of a 1 M-record shard (one wave)
+#define KVG_CS_MINB 8  // CTAs per SM asked of the P <= 3 instantiation: 8 x 132 SMs >= the 977 tiles of a 1 M-record shard (one wave)
 #endif
 template <class Op, int THREADS, int ROWS, int CW4>
 __global__ void __launch_bounds__(THREADS, CW4 <= 2 ? KVG_CS_MINB : KVG_CS_MINB_WIDE) k_classify_send(Op op, ShardArgs A, ShardPeers peers, const ShardCtrl* mine,
@@ -357,7 +357,7 @@ __global__ void __launch_bounds__(THREADS, CW4 <= 2 ? KVG_CS_MINB : KVG_CS_MINB_
       }
     }
     // totals of all earlier tiles: a thread per earlier tile, CW4 independent 16-byte loads each (fetching 2 or 4
-    // earlier tiles per round instead of one was measured: 0.131 / 0.133 vs 0.131 ms per scan — no gain)
+    // earlier tiles per round instead of one was measured: no gain)
     uint32_t acc[CW];
 #pragma unroll
     for (uint32_t c = 0; c < CW; c++) acc[c] = 0;
@@ -502,7 +502,7 @@ __global__ void __launch_bounds__(KVG_BLOCK) k_shard_gather(ShardArgs A, GatherA
   // blockIdx.y = ordering; regions in source order == Walk order.  The P regions are walked as ONE index space
   // (a record's region = the last one that starts at or before it), four records of a thread in flight per
   // round: region by region and one record at a time, a 1 M-record shard was 13 rounds of a dependent
-  // load -> store (20 us for 16 MB on one GPU), and 8 regions at P = 8 were 8 rounds even when each was short.
+  // load -> store, and 8 regions at P = 8 were 8 rounds even when each was short.
   const uint32_t o = blockIdx.y;
   uint32_t mx = 0;
   {

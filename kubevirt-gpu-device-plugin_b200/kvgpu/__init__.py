@@ -1,6 +1,6 @@
-"""kvgpu — B200-native discovery-and-classification scan for the KubeVirt GPU device plugin.
+"""kvgpu — H100-native discovery-and-classification scan for the KubeVirt GPU device plugin.
 
-The compute lives in libkvgpu.so (hand-written sm_100a CUDA, C-ABI in include/kvgpu.h); this
+The compute lives in libkvgpu.so (hand-written sm_90a CUDA, C-ABI in include/kvgpu.h); this
 package is the host-side mirror of the reference's plugin interface for that path.
 """
 from ._lib import (KVG_NO_NAME, MDEV_REC, MDEV_SURV, PCI_REC, PCI_SURV, KvgError, declared_symbols,

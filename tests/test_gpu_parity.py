@@ -1,6 +1,6 @@
 """GPU parity: the CUDA path (through the C-ABI of libkvgpu.so) against the CPU oracle, bit for bit.
 
-Every test here needs a B200 (`-m gpu`).  The oracle is only ever the checker.
+Every test here needs an H100 (`-m gpu`).  The oracle is only ever the checker.
 """
 import hashlib
 import os

@@ -1,4 +1,4 @@
-"""Register -> ListAndWatch -> Allocate replayed on the real scan (libkvgpu.so on a B200):
+"""Register -> ListAndWatch -> Allocate replayed on the real scan (libkvgpu.so on an H100):
 DiscoveryScan over a sysfs-shaped tree (BASELINE.json config 1), the plugin servers of kvgpu.serve,
 the Allocate-time re-validation as one batched pass of the classification kernel, the health feed
 through the K6 delta kernel — checked against the oracle's view of the same tree."""

@@ -1,10 +1,10 @@
 #!/usr/bin/env python3
 """profiles/<tag>_sass_tma.txt: what the built libkvgpu.so contains, per kernel — the SASS mnemonics that prove the
-sm_100a features the design relies on (UBLKCP = TMA bulk copy, SYNCS = mbarrier, REDUX = warp reduction,
+sm_90a features the design relies on (UBLKCP = TMA bulk copy, SYNCS = mbarrier, REDUX = warp reduction,
 MATCH = match.any, REDG / ATOMG = fire-and-forget / returning global atomics, ACQBULK/griddepcontrol = programmatic
-dependent launch), with registers and shared memory.   python tools/sass_report.py r02"""
+dependent launch), with registers and shared memory.   python tools/sass_report.py <tag>"""
 import collections, os, re, subprocess, sys
-tag = sys.argv[1] if len(sys.argv) > 1 else "r02"
+tag = sys.argv[1] if len(sys.argv) > 1 else "h100"
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 lib = os.path.join(ROOT, "kubevirt-gpu-device-plugin_b200", "libkvgpu.so")
 sass = subprocess.run(["cuobjdump", "-sass", lib], capture_output=True, text=True).stdout
@@ -36,6 +36,7 @@ def demangle(names):
     out = subprocess.run(["c++filt"], input="\n".join(names), capture_output=True, text=True).stdout.splitlines()
     return dict(zip(names, out))
 dm = demangle([r[0] for r in rows])
+os.makedirs(os.path.join(ROOT, "profiles"), exist_ok=True)
 out = os.path.join(ROOT, "profiles", "%s_sass_tma.txt" % tag)
 with open(out, "w") as f:
     f.write("# cuobjdump -sass / -res-usage of kubevirt-gpu-device-plugin_b200/libkvgpu.so  (arch: %s)\n" % ", ".join(arch))

@@ -21,7 +21,7 @@ ctx.set_kernel_timing(False)
 ms = {k: sum(v) / len(v) for k, v in acc.items()}
 gb = nf * len(text) / 1e9
 print("256 images:", {k: round(v * 1e3, 1) for k, v in ms.items()},
-      "scan GB/s %.0f (%.1f%%)  scan+resolve GB/s %.0f" % (gb / (ms["pciids_parse"] * 1e-3), 100 * gb / (ms["pciids_parse"] * 1e-3) / 6567.4,
+      "scan GB/s %.0f (%.1f%%)  scan+resolve GB/s %.0f" % (gb / (ms["pciids_parse"] * 1e-3), 100 * gb / (ms["pciids_parse"] * 1e-3) / B.peaks()[0],
                                                           gb / ((ms["pciids_parse"] + ms["pciids_resolve"]) * 1e-3)))
 # single image
 acc = {}
