@@ -284,7 +284,10 @@ int kvg_scan_pci(kvg_ctx *ctx, const kvg_pci_rec *recs, size_t n, kvg_pci_result
 int kvg_scan_mdev(kvg_ctx *ctx, const kvg_mdev_rec *recs, size_t n, const kvg_type_dict *types,
                   kvg_mdev_result **res);
 /* Classify `recs`, diff against the alive-set of the previous call on this context (first call:
- * against "nothing alive").  n must stay constant between calls; kvg_health_reset() re-arms. */
+ * against "nothing alive").  A call with a different n re-arms the same way, as does
+ * kvg_health_reset(); n = 0 returns an empty delta.  Pinned (cudaHostAlloc / registered) `recs` of
+ * at most 32,768 records are read in place by TMA bulk copies and must be 16-byte aligned; this is
+ * not checked.  Pageable memory is staged and has no alignment requirement. */
 int kvg_health_rescan(kvg_ctx *ctx, const kvg_pci_rec *recs, size_t n, kvg_health_delta **delta);
 int kvg_health_reset(kvg_ctx *ctx);
 

@@ -321,12 +321,13 @@ __global__ void __launch_bounds__(KVG_BLOCK) k_lookup_general(const uint8_t* __r
     if (ok) atomicMin(&match_off[kidx], b);
   }
 }
-// one thread per key: sanitise the remainder of the matched line into out[k*cap ...]
+// one thread per key: sanitise the remainder of the matched line into out[k*cap ...], or, with out_off, into
+// out[out_off[k] .. out_off[k+1]); out_len[k] is the name's full length either way
 __global__ void k_sanitise_matches(const uint8_t* __restrict__ text, uint32_t len,
                                    const uint32_t* __restrict__ key_off,
                                    const uint32_t* __restrict__ match_off, uint32_t n_keys,
                                    uint8_t* __restrict__ out, uint32_t cap,
-                                   uint32_t* __restrict__ out_len) {
+                                   uint32_t* __restrict__ out_len, const uint64_t* __restrict__ out_off) {
   pdl_enter();
   uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= n_keys) return;
@@ -339,7 +340,9 @@ __global__ void k_sanitise_matches(const uint8_t* __restrict__ text, uint32_t le
   uint32_t e = s;
   while (e < len && text[e] != '\n') e++;
   if (e > s && text[e - 1] == '\r') e--;  // ScanLines dropCR (TrimSpace would drop it anyway)
-  out_len[k] = d_sanitise_name(text + s, e - s, out + (size_t)k * cap, cap);
+  const size_t o = out_off ? out_off[k] : (size_t)k * cap;
+  const uint32_t c = out_off ? (uint32_t)(out_off[k + 1] - out_off[k]) : cap;
+  out_len[k] = d_sanitise_name(text + s, e - s, out + o, c);
 }
 
 }  // namespace kvg

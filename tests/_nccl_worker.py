@@ -1,6 +1,10 @@
 """Worker for the multi-GPU parity test: rank r scans its shard on GPU r (PCI records, then mdev records);
 the union of the ranks' parts — every rank holds the keys it owns, with ALL their members — must equal the
-oracle on the unsharded snapshot, byte for byte, for several back-to-back steps (window reuse, acks)."""
+oracle on the unsharded snapshot, byte for byte, for several back-to-back steps (window reuse, acks).
+
+Arguments: n [mode [m_total [table]]]; table "long-names" scans against util.long_name_pciids() with the
+type names of util.long_name_types() (vGPU resource names of up to 60,000 bytes) instead of the shipped
+pci.ids and the synthetic type names."""
 import hashlib
 import os
 import sys
@@ -23,10 +27,11 @@ def main():
     n = int(sys.argv[1])
     mode = sys.argv[2] if len(sys.argv) > 2 else "p2p"
     m_total = int(sys.argv[3]) if len(sys.argv) > 3 else max(n // 8, 3)
+    long_names = len(sys.argv) > 4 and sys.argv[4] == "long-names"
     rank, world, local_rank = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"]), int(os.environ["LOCAL_RANK"])
     torch.cuda.set_device(local_rank)
     dist.init_process_group("nccl", device_id=torch.device("cuda", local_rank))
-    text = util.pciids_text()
+    text = util.long_name_pciids() if long_names else util.pciids_text()
     ids = O.nv_ids(text)
     ctx = kvgpu.Context(local_rank)
     ctx.pciids_load(text)
@@ -62,7 +67,7 @@ def main():
     torch.cuda.synchronize()
     ctx.dev_gen_pci(buf.data_ptr(), lo, hi - lo, ids, 17)
     ctx.dev_gen_mdev(mbuf.data_ptr(), mlo, mhi - mlo)
-    types = O.gen_type_names(256)
+    types = util.long_name_types() if long_names else O.gen_type_names(256)
     want_m = O.Maps()
     want_m.create_iommu_device_map_flat(O.gen_pci(0, n, ids, 17))
     want_m.create_vgpu_id_map_flat(O.gen_mdev(0, m_total), types)

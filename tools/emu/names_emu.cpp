@@ -139,7 +139,7 @@ int emu_get_device_names(const uint8_t* text, uint32_t len, const uint8_t* keys,
     if (sec)
       emu_launch(k_lookup_general, dim3(4, 1), KVG_BLOCK, text, len, (const uint32_t*)sec_lines.data(),
                  (const uint32_t*)(sec_lines.data() + sec_cap), key, (const uint32_t*)off2, &match);
-    emu_launch(k_sanitise_matches, dim3(1), 64, text, len, (const uint32_t*)off2, (const uint32_t*)&match, 1u, out, name_cap, &n);
+    emu_launch(k_sanitise_matches, dim3(1), 64, text, len, (const uint32_t*)off2, (const uint32_t*)&match, 1u, out, name_cap, &n, (const uint64_t*)nullptr);
     if (n > name_cap) return 2;
     names_len[k] = n;
   }
