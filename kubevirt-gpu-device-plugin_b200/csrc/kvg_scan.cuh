@@ -35,118 +35,67 @@ struct ScanCtrl {
 };
 
 // ------------------------------------------------------------------------------------------------
-// generic stable compaction
-//   Op::Item                        what a thread holds per input element
-//   uint32_t count()                number of input items (may read device memory)
-//   Item load(uint32_t i, bool ok)  ok == false -> any value that fails pred
+// The tile front-end of every classify kernel.  A warp owns 32 x ROWS consecutive records of the tile
+// (THREADS x ROWS records); `classify` issues every load before the first ballot, votes Op::pred per row and
+// calls Op::prepare for the survivors, whose dependent loads then overlap what the kernel does next.  `emit`
+// hands each of the lane's survivors to f(pos, item, i, aux), numbered in record order from the warp's offset.
+//   Op::Item                          what a thread holds per record
+//   uint32_t n                        number of records
+//   Item load(uint32_t i, bool ok)    ok == false -> any value that fails pred
 //   bool pred(const Item&, i)
-//   void emit(uint32_t pos, const Item&, i)
-//   void warp_epilogue(...)         optional per-warp reduction hook (called once per tile)
-//   void finish(uint32_t total)     called by one thread of the last tile
-// ------------------------------------------------------------------------------------------------
-template <class Op>
-__global__ void __launch_bounds__(KVG_BLOCK) k_compact(Op op, uint64_t* tile_state, uint32_t epoch) {
-  pdl_enter();
-  __shared__ uint32_t s_base;
-  __shared__ uint32_t s_wtot[KVG_WARPS], s_woff[KVG_WARPS];
-  op.begin();
-  const uint32_t n = op.count();
-  const uint32_t n_tiles = (n + C_TILE - 1) / C_TILE;
-  const uint32_t lane = lane_id(), warp = warp_id();
-  if (n_tiles == 0) {
-    if (blockIdx.x == 0 && threadIdx.x == 0) op.finish(0);
-    return;
-  }
-  // Persistent, co-resident grid; tile = blockIdx + k*gridDim.  A look-back predecessor is owned by
-  // a resident CTA that reaches it no later than this CTA reaches its own tile (no ticket needed).
-  for (uint32_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-    const uint32_t base = tile * C_TILE + warp * C_WARP_ITEMS;
-    typename Op::Item item[C_ROWS];
-#pragma unroll
-    for (uint32_t k = 0; k < C_ROWS; k++) {
-      uint32_t i = base + k * 32 + lane;
-      item[k] = op.load(i, i < n);
-    }
-    uint32_t bal[C_ROWS], aux[C_ROWS];
-    uint32_t wtot = 0;
-#pragma unroll
-    for (uint32_t k = 0; k < C_ROWS; k++) {
-      uint32_t i = base + k * 32 + lane;
-      bool p = i < n && op.pred(item[k], i);
-      bal[k] = __ballot_sync(KVG_FULL, p);
-      wtot += __popc(bal[k]);
-      aux[k] = p ? op.prepare(item[k]) : 0u;  // dependent loads overlap the look-back below
-    }
-    if (lane == 0) s_wtot[warp] = wtot;
-    __syncthreads();
-    if (warp == 0) {
-      uint32_t w = lane < KVG_WARPS ? s_wtot[lane] : 0;
-      uint32_t wi = warp_incl_sum(w);
-      if (lane < KVG_WARPS) s_woff[lane] = wi - w;
-      uint32_t tile_total = __shfl_sync(KVG_FULL, wi, KVG_WARPS - 1);
-      uint32_t excl = lookback_sum(tile_state, tile, tile_total, epoch);
-      if (lane == 0) {
-        s_base = excl;
-        if (tile == n_tiles - 1) op.finish(excl + tile_total);
-      }
-    }
-    __syncthreads();
-    uint32_t off = s_base + s_woff[warp];
-#pragma unroll
-    for (uint32_t k = 0; k < C_ROWS; k++) {
-      uint32_t i = base + k * 32 + lane;
-      if ((bal[k] >> lane) & 1u) op.emit(off + __popc(bal[k] & lanemask_lt()), item[k], i, aux[k]);
-      off += __popc(bal[k]);
-    }
-    op.tile_epilogue();
-  }
-}
-
-// ------------------------------------------------------------------------------------------------
-// K3/K5, one-tile-per-CTA form: small CTAs (THREADS x ROWS records kept in registers), thousands
-// of them, dispatched in blockIdx order by the hardware.  Many resident CTAs per SM hide the
-// count -> look-back -> write-out latency chain of each other; predecessors were dispatched
-// earlier, so the classic decoupled look-back usually finds an inclusive prefix close by.
-// (Measured alternative: every tile publishes its count and sums ALL earlier counts itself, a thread per
-// earlier tile — no chain, but several dependent L2 round trips per thread for the last tiles; it was slower
-// at 1 M records.  The chained scan stays.)
+//   uint32_t prepare(const Item&)     per-survivor value handed to emit (name slot, canonical type)
 // ------------------------------------------------------------------------------------------------
 template <class Op, int THREADS, int ROWS>
-__global__ void __launch_bounds__(THREADS) k_classify_oneshot(Op op, uint64_t* tile_state, uint32_t epoch) {
-  pdl_enter();
-  constexpr uint32_t TILE = THREADS * ROWS;
-  constexpr uint32_t NW = THREADS / 32;
-  constexpr uint32_t WARP_ITEMS = 32 * ROWS;
-  __shared__ uint32_t s_wtot[NW], s_woff[NW];
-  __shared__ uint32_t s_base;
-  op.begin();
-  const uint32_t n = op.count();
-  const uint32_t n_tiles = (n + TILE - 1) / TILE;
-  const uint32_t lane = lane_id(), warp = threadIdx.x >> 5;
-  const uint32_t tile = blockIdx.x;
-  if (n_tiles == 0) {
-    if (tile == 0 && threadIdx.x == 0) op.finish(0);
-    return;
-  }
-  if (tile >= n_tiles) return;
-  const uint32_t base = tile * TILE + warp * WARP_ITEMS;
+struct ClassifyTile {
+  static constexpr uint32_t TILE = THREADS * ROWS;
+  static constexpr uint32_t NW = THREADS / 32;
+  static constexpr uint32_t WARP_ITEMS = 32 * ROWS;
   typename Op::Item item[ROWS];
-#pragma unroll
-  for (int k = 0; k < ROWS; k++) {
-    uint32_t i = base + k * 32 + lane;
-    item[k] = op.load(i, i < n);
-  }
   uint32_t bal[ROWS], aux[ROWS];
-  uint32_t wtot = 0;
+  uint32_t base;  // the warp's first record
+  uint32_t wtot;  // the warp's survivors
+
+  __device__ __forceinline__ void classify(Op& op, uint32_t tile) {
+    const uint32_t lane = lane_id(), n = op.n;
+    base = tile * TILE + (threadIdx.x >> 5) * WARP_ITEMS;
 #pragma unroll
-  for (int k = 0; k < ROWS; k++) {
-    uint32_t i = base + k * 32 + lane;
-    bool p = i < n && op.pred(item[k], i);
-    bal[k] = __ballot_sync(KVG_FULL, p);
-    wtot += __popc(bal[k]);
-    aux[k] = p ? op.prepare(item[k]) : 0u;
+    for (int k = 0; k < ROWS; k++) {
+      const uint32_t i = base + k * 32 + lane;
+      item[k] = op.load(i, i < n);
+    }
+    wtot = 0;
+#pragma unroll
+    for (int k = 0; k < ROWS; k++) {
+      const uint32_t i = base + k * 32 + lane;
+      const bool p = i < n && op.pred(item[k], i);
+      bal[k] = __ballot_sync(KVG_FULL, p);
+      wtot += __popc(bal[k]);
+      aux[k] = p ? op.prepare(item[k]) : 0u;
+    }
   }
-  if (lane == 0) s_wtot[warp] = wtot;
+  template <class F>
+  __device__ __forceinline__ void emit(uint32_t off, F&& f) const {
+    const uint32_t lane = lane_id();
+#pragma unroll
+    for (int k = 0; k < ROWS; k++) {
+      if ((bal[k] >> lane) & 1u) f(off + __popc(bal[k] & lanemask_lt()), item[k], base + k * 32 + lane, aux[k]);
+      off += __popc(bal[k]);
+    }
+  }
+};
+
+// One tile of the look-back compaction: classify it, place it behind all earlier tiles (decoupled look-back on
+// the tile counts), write its survivors.  Besides the front-end, Op provides emit(pos, item, i, aux),
+// tile_epilogue() (once per warp after its survivors) and finish(total) (one thread of the last tile).
+// s_wtot / s_woff: a word per warp of shared memory.
+template <class Op, int THREADS, int ROWS>
+__device__ __forceinline__ void lookback_tile(Op& op, uint32_t tile, uint32_t n_tiles, uint64_t* tile_state, uint32_t epoch,
+                                              uint32_t* s_wtot, uint32_t* s_woff, uint32_t& s_base) {
+  constexpr uint32_t NW = THREADS / 32;
+  const uint32_t lane = lane_id(), warp = threadIdx.x >> 5;
+  ClassifyTile<Op, THREADS, ROWS> ct;
+  ct.classify(op, tile);
+  if (lane == 0) s_wtot[warp] = ct.wtot;
   __syncthreads();
   if (warp == 0) {
     uint32_t w = lane < NW ? s_wtot[lane] : 0;
@@ -160,14 +109,51 @@ __global__ void __launch_bounds__(THREADS) k_classify_oneshot(Op op, uint64_t* t
     }
   }
   __syncthreads();
-  uint32_t off = s_base + s_woff[warp];
-#pragma unroll
-  for (int k = 0; k < ROWS; k++) {
-    uint32_t i = base + k * 32 + lane;
-    if ((bal[k] >> lane) & 1u) op.emit(off + __popc(bal[k] & lanemask_lt()), item[k], i, aux[k]);
-    off += __popc(bal[k]);
-  }
+  ct.emit(s_base + s_woff[warp], [&](uint32_t pos, const typename Op::Item& r, uint32_t i, uint32_t a) { op.emit(pos, r, i, a); });
   op.tile_epilogue();
+}
+
+// ------------------------------------------------------------------------------------------------
+// K3 at latency-bound sizes: small CTAs (THREADS x ROWS records kept in registers), thousands
+// of them, dispatched in blockIdx order by the hardware.  Many resident CTAs per SM hide the
+// count -> look-back -> write-out latency chain of each other; predecessors were dispatched
+// earlier, so the classic decoupled look-back usually finds an inclusive prefix close by.
+// (Measured alternative: every tile publishes its count and sums ALL earlier counts itself, a thread per
+// earlier tile — no chain, but several dependent L2 round trips per thread for the last tiles; it was slower
+// at 1 M records.  The chained scan stays.)
+// ------------------------------------------------------------------------------------------------
+template <class Op, int THREADS, int ROWS>
+__global__ void __launch_bounds__(THREADS) k_classify_oneshot(Op op, uint64_t* tile_state, uint32_t epoch) {
+  pdl_enter();
+  constexpr uint32_t TILE = THREADS * ROWS;
+  __shared__ uint32_t s_wtot[THREADS / 32], s_woff[THREADS / 32];
+  __shared__ uint32_t s_base;
+  const uint32_t n_tiles = (op.n + TILE - 1) / TILE;
+  const uint32_t tile = blockIdx.x;
+  if (n_tiles == 0) {
+    if (tile == 0 && threadIdx.x == 0) op.finish(0);
+    return;
+  }
+  if (tile >= n_tiles) return;
+  lookback_tile<Op, THREADS, ROWS>(op, tile, n_tiles, tile_state, epoch, s_wtot, s_woff, s_base);
+}
+
+// K6: the same compaction on a persistent, co-resident grid of 2048-record tiles; tile = blockIdx + k*gridDim.
+// A look-back predecessor is owned by a resident CTA that reaches it no later than this CTA reaches its own
+// tile (no ticket needed).  One CTA per tile (k_classify_oneshot<HealthOp, KVG_BLOCK, C_ROWS>) measured about
+// 5 % slower at 4 Mi records (39.5 against 37.7 us, H100 SXM with a 400 W power limit).
+template <class Op>
+__global__ void __launch_bounds__(KVG_BLOCK) k_compact(Op op, uint64_t* tile_state, uint32_t epoch) {
+  pdl_enter();
+  __shared__ uint32_t s_wtot[KVG_WARPS], s_woff[KVG_WARPS];
+  __shared__ uint32_t s_base;
+  const uint32_t n_tiles = (op.n + C_TILE - 1) / C_TILE;
+  if (n_tiles == 0) {
+    if (blockIdx.x == 0 && threadIdx.x == 0) op.finish(0);
+    return;
+  }
+  for (uint32_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x)
+    lookback_tile<Op, KVG_BLOCK, C_ROWS>(op, tile, n_tiles, tile_state, epoch, s_wtot, s_woff, s_base);
 }
 
 // ---- K3: PCI classify ---------------------------------------------------------------------------
@@ -180,29 +166,59 @@ __device__ __forceinline__ bool pci_record_alive(const uint4& r) {
   static_assert((KVG_PF_VENDOR_ERR | KVG_PF_DRIVER_ERR | KVG_PF_IOMMU_ERR | KVG_PF_DEVICE_ERR) == 0xf, "flags");
   return (r.y & 0xffffu) == 0x10deu && ((r.w & 0x0fffu) - 1u) < 2u;
 }
-struct PciClassifyOp {
+// What the PCI and mdev classify operators share: a survivor goes out as Self::UNITS 16-byte streaming stores of
+// Self::make, and the largest Self::keys of the survivors a thread wrote bound the radix passes of the two
+// orderings: keys().x -> ScanCtrl::max_devkey (ordering 0), keys().y -> max_group (ordering 1).
+template <class Self>
+struct SurvivorOp {
+  uint4* out;
+  ScanCtrl* ctrl;
+  uint32_t local_max_x = 0, local_max_y = 0;  // per-thread running maxima of keys() (registers)
+
+  template <class Item>
+  __device__ __forceinline__ void emit(uint32_t pos, const Item& r, uint32_t i, uint32_t aux) {
+    constexpr int U = Self::UNITS;
+    const Self& self = static_cast<const Self&>(*this);
+    uint4 s[U];
+    self.make(r, i, aux, s);
+#pragma unroll
+    for (int u = 0; u < U; u++) st_stream(out + (size_t)pos * U + u, s[u]);
+    const uint2 k = self.keys(r, aux);
+    local_max_x = max(local_max_x, k.x);
+    local_max_y = max(local_max_y, k.y);
+  }
+  __device__ __forceinline__ void tile_epilogue() {
+    uint32_t g = warp_max(local_max_y), d = warp_max(local_max_x);
+    if (lane_id() == 0) {
+      if (g) atomicMax(&ctrl->max_group, g);
+      if (d) atomicMax(&ctrl->max_devkey, d);
+    }
+    local_max_x = 0;
+    local_max_y = 0;
+  }
+  __device__ __forceinline__ void finish(uint32_t total) { ctrl->n_surv = total; }
+  // the thread's maxima as k_tile_offsets reads a tile_max slot: {group, dev}
+  __device__ __forceinline__ uint2 take_maxima() {
+    uint2 m = make_uint2(local_max_y, local_max_x);
+    local_max_x = local_max_y = 0;
+    return m;
+  }
+};
+
+struct PciClassifyOp : SurvivorOp<PciClassifyOp> {
   using Item = uint4;
-  static constexpr uint32_t REC_BYTES = 16;
+  static constexpr int UNITS = 1;  // 16-byte units per survivor
   const uint4* recs;
   uint32_t n;
-  kvg_pci_surv* out;
-  ScanCtrl* ctrl;
-  const uint32_t* nv_index;                 // device id -> name pool slot (K1's k_pciids_names)
-  uint32_t local_max_group, local_max_dev;  // per-thread running maxima (registers)
+  const uint32_t* nv_index;  // device id -> name pool slot (K1's k_pciids_names)
 
-  __device__ __forceinline__ void begin() {}
-  // the name join: one load per survivor from the flattened table of vendor 10de
-  // (nv_index == NULL: the parse is still running on its own stream; the final ordering kernel joins the names)
-  __device__ __forceinline__ uint32_t prepare(const Item& r) const { return nv_index ? __ldg(&nv_index[r.y >> 16]) : P_NONE; }
-  __device__ __forceinline__ uint32_t count() const { return n; }
   __device__ __forceinline__ Item load(uint32_t i, bool ok) const {
     return ok ? ld_stream(recs + i) : make_uint4(0, 0, 0, 0xff00u);
   }
-  // record = {addr, vendor | device<<16, iommu_group, driver | flags<<8 | numa<<16}
-  // device_plugin.go:203-238: any of vendor/driver/iommu/device read errors drops the entry,
-  // vendor must be "10de" (:209), driver in supportedVfioDrivers (:217, :75-78)
   __device__ __forceinline__ bool pred(const Item& r, uint32_t) const { return pci_record_alive(r); }
-  static constexpr int UNITS = 1;  // 16-byte units per survivor
+  // the name join: one load per survivor from the flattened table of vendor 10de
+  // (nv_index == NULL: the parse is still running on its own stream; the final ordering kernel joins the names)
+  __device__ __forceinline__ uint32_t prepare(const Item& r) const { return nv_index ? __ldg(&nv_index[r.y >> 16]) : P_NONE; }
   // the survivor record (kvgpu.h kvg_pci_surv)
   __device__ __forceinline__ void make(const Item& r, uint32_t, uint32_t name_slot, uint4* s) const {
     uint32_t device = r.y >> 16;
@@ -216,28 +232,6 @@ struct PciClassifyOp {
   }
   // keys of the two group-by maps: {device id (deviceMap), iommu group (iommuMap)}
   __device__ __forceinline__ uint2 keys(const Item& r, uint32_t) const { return make_uint2(r.y >> 16, r.z); }
-  __device__ __forceinline__ void emit(uint32_t pos, const Item& r, uint32_t i, uint32_t name_slot) {
-    uint4 s[1];
-    make(r, i, name_slot, s);
-    st_stream(reinterpret_cast<uint4*>(out) + pos, s[0]);
-    local_max_group = max(local_max_group, r.z);
-    local_max_dev = max(local_max_dev, r.y >> 16);
-  }
-  __device__ __forceinline__ void tile_epilogue() {
-    uint32_t g = warp_max(local_max_group), d = warp_max(local_max_dev);
-    if (lane_id() == 0) {
-      if (g) atomicMax(&ctrl->max_group, g);
-      if (d) atomicMax(&ctrl->max_devkey, d);
-    }
-    local_max_group = 0;
-    local_max_dev = 0;
-  }
-  __device__ __forceinline__ void finish(uint32_t total) { ctrl->n_surv = total; }
-  __device__ __forceinline__ uint2 take_maxima() {
-    uint2 m = make_uint2(local_max_group, local_max_dev);
-    local_max_group = local_max_dev = 0;
-    return m;
-  }
 };
 // the deferred name join of a dense PCI survivor list no ordering walks (the rank's own shard of a sharded scan):
 // runs on the side stream behind the parse, beside the exchange and the orderings
@@ -255,20 +249,14 @@ __global__ void __launch_bounds__(KVG_BLOCK) k_join_names(uint4* __restrict__ re
 struct MdevItem {
   uint4 lo, hi;
 };
-struct MdevClassifyOp {
+struct MdevClassifyOp : SurvivorOp<MdevClassifyOp> {
   using Item = MdevItem;
-  static constexpr uint32_t REC_BYTES = 32;
+  static constexpr int UNITS = 2;  // 16-byte units per survivor
   const uint4* recs;  // 2 x uint4 per record
   uint32_t n;
-  uint4* out;
-  ScanCtrl* ctrl;
   const uint16_t* type_canon;  // [n_types] canonical id per raw dictionary entry
   uint32_t n_types;
-  uint32_t local_max_parent, local_max_type;
 
-  __device__ __forceinline__ void begin() {}
-  __device__ __forceinline__ uint32_t prepare(const Item& r) const { return type_canon[r.hi.y & 0xffffu]; }
-  __device__ __forceinline__ uint32_t count() const { return n; }
   __device__ __forceinline__ Item load(uint32_t i, bool ok) const {
     Item it;
     if (ok) {
@@ -286,7 +274,7 @@ struct MdevClassifyOp {
     uint32_t type_idx = r.hi.y & 0xffffu;
     return (flags & (KVG_MF_TYPE_ERR | KVG_MF_PARENT_ERR)) == 0 && type_idx < n_types;
   }
-  static constexpr int UNITS = 2;  // 16-byte units per survivor
+  __device__ __forceinline__ uint32_t prepare(const Item& r) const { return type_canon[r.hi.y & 0xffffu]; }
   // the survivor record (kvgpu.h kvg_mdev_surv)
   __device__ __forceinline__ void make(const Item& r, uint32_t i, uint32_t canon, uint4* s) const {
     uint32_t flags = (r.hi.y >> 16) & 0xffu;
@@ -300,29 +288,6 @@ struct MdevClassifyOp {
   }
   // keys of the two group-by maps: {canonical type (vGpuMap), parent GPU (gpuVgpuMap)}
   __device__ __forceinline__ uint2 keys(const Item& r, uint32_t canon) const { return make_uint2(canon, r.hi.x); }
-  __device__ __forceinline__ void emit(uint32_t pos, const Item& r, uint32_t i, uint32_t canon) {
-    uint4 s[2];
-    make(r, i, canon, s);
-    st_stream(out + 2 * (size_t)pos, s[0]);
-    st_stream(out + 2 * (size_t)pos + 1, s[1]);
-    local_max_parent = max(local_max_parent, r.hi.x);
-    local_max_type = max(local_max_type, canon);
-  }
-  __device__ __forceinline__ void tile_epilogue() {
-    uint32_t g = warp_max(local_max_parent), d = warp_max(local_max_type);
-    if (lane_id() == 0) {
-      if (g) atomicMax(&ctrl->max_group, g);
-      if (d) atomicMax(&ctrl->max_devkey, d);
-    }
-    local_max_parent = 0;
-    local_max_type = 0;
-  }
-  __device__ __forceinline__ void finish(uint32_t total) { ctrl->n_surv = total; }
-  __device__ __forceinline__ uint2 take_maxima() {
-    uint2 m = make_uint2(local_max_parent, local_max_type);
-    local_max_parent = local_max_type = 0;
-    return m;
-  }
 };
 
 // ---- K6: health diff ----------------------------------------------------------------------------
@@ -334,9 +299,7 @@ struct HealthOp {
   uint32_t* changed;
   ScanCtrl* ctrl;
   uint32_t local_alive;
-  __device__ __forceinline__ void begin() {}
   __device__ __forceinline__ uint32_t prepare(const Item&) const { return 0; }
-  __device__ __forceinline__ uint32_t count() const { return n; }
   __device__ __forceinline__ Item load(uint32_t i, bool ok) const {
     if (!ok) return make_uint4(0, 0, 0, 0);
     uint4 r = ld_stream(recs + i);
@@ -639,35 +602,17 @@ template <class Op, int THREADS, int ROWS>
 __global__ void __launch_bounds__(THREADS) k_classify_ragged(Op op, uint32_t* __restrict__ tile_count,
                                                              uint2* __restrict__ tile_max) {
   pdl_enter();
-  constexpr uint32_t TILE = THREADS * ROWS;
-  constexpr uint32_t NW = THREADS / 32;
-  constexpr uint32_t WARP_ITEMS = 32 * ROWS;
+  using Tile = ClassifyTile<Op, THREADS, ROWS>;
+  constexpr uint32_t NW = Tile::NW;
   __shared__ uint32_t s_wtot[NW];
   __shared__ uint2 s_wmax[NW];
-  op.begin();
-  const uint32_t n = op.count();
   const uint32_t lane = lane_id(), warp = threadIdx.x >> 5;
   const uint32_t tile = blockIdx.x;
-  const uint32_t base = tile * TILE + warp * WARP_ITEMS;
-  typename Op::Item item[ROWS];
-#pragma unroll
-  for (int k = 0; k < ROWS; k++) {
-    uint32_t i = base + k * 32 + lane;
-    item[k] = op.load(i, i < n);
-  }
-  uint32_t bal[ROWS], aux[ROWS];
-  uint32_t wtot = 0;
-#pragma unroll
-  for (int k = 0; k < ROWS; k++) {
-    uint32_t i = base + k * 32 + lane;
-    bool p = i < n && op.pred(item[k], i);
-    bal[k] = __ballot_sync(KVG_FULL, p);
-    wtot += __popc(bal[k]);
-    aux[k] = p ? op.prepare(item[k]) : 0u;
-  }
-  if (lane == 0) s_wtot[warp] = wtot;
+  Tile ct;
+  ct.classify(op, tile);
+  if (lane == 0) s_wtot[warp] = ct.wtot;
   __syncthreads();
-  uint32_t off = tile * TILE;  // tile-local base: survivors of a tile stay contiguous and ordered
+  uint32_t off = tile * Tile::TILE;  // tile-local base: survivors of a tile stay contiguous and ordered
 #pragma unroll
   for (uint32_t w = 0; w < NW; w++) {
     uint32_t c = s_wtot[w];
@@ -679,12 +624,7 @@ __global__ void __launch_bounds__(THREADS) k_classify_ragged(Op op, uint32_t* __
       tile_count[tile] = tot;
     }
   }
-#pragma unroll
-  for (int k = 0; k < ROWS; k++) {
-    uint32_t i = base + k * 32 + lane;
-    if ((bal[k] >> lane) & 1u) op.emit(off + __popc(bal[k] & lanemask_lt()), item[k], i, aux[k]);
-    off += __popc(bal[k]);
-  }
+  ct.emit(off, [&](uint32_t pos, const typename Op::Item& r, uint32_t i, uint32_t a) { op.emit(pos, r, i, a); });
   // largest keys of the tile (they bound the radix pass counts): per-tile slot, no global atomics
   uint2 m = op.take_maxima();
   m.x = warp_max(m.x);

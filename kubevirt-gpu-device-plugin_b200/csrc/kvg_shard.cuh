@@ -114,6 +114,42 @@ __device__ __forceinline__ uint32_t shard_owner(uint32_t key, const ShardArgs& A
 __device__ __forceinline__ size_t shard_region(const ShardArgs& A, uint32_t o, uint32_t s, int U) {
   return (((size_t)A.parity * 2 + o) * A.n_src + s) * A.region_cap * (size_t)U;
 }
+// store a record (U units) at position `at` of my region of ordering o in owner q's window
+template <int U>
+__device__ __forceinline__ void shard_store(const ShardPeers& peers, const ShardArgs& A, uint32_t q, uint32_t o, uint32_t at,
+                                            const uint4* rec) {
+  uint4* dst = peers.win[q] + shard_region(A, o, A.src, U) + (size_t)at * U;
+#pragma unroll
+  for (int u = 0; u < U; u++) dst[u] = rec[u];  // NVLink store (or local)
+}
+
+// The window parity of this step is rewritten: every owner must have consumed the step that used it two steps
+// ago.  Thread q < P waits for owner q's acknowledgement; after SH_SPIN_LIMIT clocks it raises *err and goes on.
+__device__ __forceinline__ void shard_wait_acks(const ShardArgs& A, const ShardCtrl* mine, uint32_t* err) {
+  const uint32_t q = threadIdx.x;
+  if (q >= A.P || A.step <= 2) return;
+  const long long t0 = clock64();
+  while (ld_acquire_sys(&mine->ack[q]) < A.step - 2) {
+    if (clock64() - t0 > SH_SPIN_LIMIT) {
+      atomicExch(err, 1u);
+      break;
+    }
+  }
+}
+
+// Stable rank of the lane's survivor among the survivors of its warp that go to owner q in ordering o (called by
+// the whole warp, one row at a time; q == SH_ALL: no survivor in this lane): the warp's earlier rows counted in
+// wcnt[o][q], plus the lanes before it in this row.  One lane per owner then advances wcnt[o][q].
+__device__ __forceinline__ uint32_t shard_warp_rank(uint32_t (*wcnt)[SH_MAX_RANKS], uint32_t o, uint32_t q) {
+  const uint32_t same = __match_any_sync(KVG_FULL, q);
+  const uint32_t before = __popc(same & lanemask_lt());
+  const uint32_t prior = q != SH_ALL ? wcnt[o][q] : 0;
+  const uint32_t rank = prior + before;
+  __syncwarp();
+  if (q != SH_ALL && before == 0) wcnt[o][q] = prior + __popc(same);
+  __syncwarp();
+  return rank;
+}
 
 // One launch: count, chained scan, send.  A CTA owns a 2048-survivor tile.  Ranks inside a warp come from
 // match.any (one instruction per row and ordering whatever P is); the 2P per-tile counts are combined over the
@@ -131,16 +167,7 @@ __global__ void __launch_bounds__(KVG_BLOCK) k_shard_send(ShardArgs A, ShardPeer
   const uint32_t lane = lane_id(), warp = warp_id();
   const uint32_t active = max(Tu, 1u);  // CTAs that take part (tile 0 also stands for the empty list)
   if (tile >= active) return;
-  // the window parity is rewritten: every owner must have consumed the step that used it two steps ago
-  if (threadIdx.x < A.P && A.step > 2 && A.only == SH_ALL) {
-    const long long t0 = clock64();
-    while (ld_acquire_sys(&mine->ack[threadIdx.x]) < A.step - 2) {
-      if (clock64() - t0 > SH_SPIN_LIMIT) {
-        atomicExch(err, 1u);
-        break;
-      }
-    }
-  }
+  if (A.only == SH_ALL) shard_wait_acks(A, mine, err);
   if (tile < Tu) {
     const uint32_t base = tile * C_TILE + warp * C_WARP_ITEMS;
     uint4 rec[C_ROWS][U];
@@ -165,16 +192,7 @@ __global__ void __launch_bounds__(KVG_BLOCK) k_shard_send(ShardArgs A, ShardPeer
 #pragma unroll
     for (uint32_t k = 0; k < C_ROWS; k++) {
 #pragma unroll
-      for (uint32_t o = 0; o < 2; o++) {
-        const uint32_t q = o ? q1[k] : q0[k];
-        const uint32_t same = __match_any_sync(KVG_FULL, q);
-        const uint32_t before = __popc(same & lanemask_lt());
-        const uint32_t prior = q != SH_ALL ? s_wcnt[warp][o][q] : 0;
-        pos[k][o] = prior + before;
-        __syncwarp();
-        if (q != SH_ALL && before == 0) s_wcnt[warp][o][q] = prior + __popc(same);  // one lane per owner advances
-        __syncwarp();
-      }
+      for (uint32_t o = 0; o < 2; o++) pos[k][o] = shard_warp_rank(s_wcnt[warp], o, o ? q1[k] : q0[k]);
     }
     __syncthreads();
     // warp c: counter c = (ordering, owner) — prefix over the warps in place, tile aggregate, chained scan
@@ -197,10 +215,7 @@ __global__ void __launch_bounds__(KVG_BLOCK) k_shard_send(ShardArgs A, ShardPeer
       for (uint32_t o = 0; o < 2; o++) {
         const uint32_t q = o ? q1[k] : q0[k];
         if (q != SH_ALL && (A.only == SH_ALL || q == A.only)) {
-          const uint32_t at = s_base[o][q] + s_wcnt[warp][o][q] + pos[k][o];
-          uint4* dst = peers.win[q] + shard_region(A, o, A.src, U) + (size_t)at * U;
-#pragma unroll
-          for (int u = 0; u < U; u++) dst[u] = rec[k][u];  // NVLink store (or local)
+          shard_store<U>(peers, A, q, o, s_base[o][q] + s_wcnt[warp][o][q] + pos[k][o], rec[k]);
         }
       }
     }
@@ -234,10 +249,9 @@ __global__ void __launch_bounds__(THREADS, CW4 <= 2 ? KVG_CS_MINB : KVG_CS_MINB_
   constexpr int U = Op::UNITS;
   constexpr uint32_t TILE = THREADS * ROWS;
   constexpr uint32_t NW = THREADS / 32;
-  constexpr uint32_t WARP_ITEMS = 32 * ROWS;
   constexpr uint32_t CW = 4 * CW4;
   static_assert(TILE < (1u << CS_COUNT_BITS), "a tile count fits the count field");
-  static_assert(ROWS <= 8 && WARP_ITEMS <= 256, "warp-local positions are packed in bytes");
+  static_assert(ROWS <= 8, "warp-local positions (< 32 x ROWS) are packed in bytes");
   __shared__ uint32_t s_wcnt[NW][2][SH_MAX_RANKS];  // per warp: survivors of every (ordering, owner) -> prefix over the warps
   __shared__ uint32_t s_wtot[NW], s_woff[NW];
   __shared__ uint32_t s_agg[CW], s_excl[CW];
@@ -248,46 +262,20 @@ __global__ void __launch_bounds__(THREADS, CW4 <= 2 ? KVG_CS_MINB : KVG_CS_MINB_
   __shared__ uint4 s_rec[TILE * U];
   __shared__ uint32_t s_meta[TILE];  // warp | position among the warp's survivors of the same (ordering, owner): 2 + 8 + 8 bits
   static_assert(NW <= 4, "the warp index has two bits in s_meta");
-  op.begin();
-  const uint32_t n = op.count();
-  const uint32_t n_tiles = (n + TILE - 1) / TILE;
+  const uint32_t n_tiles = (op.n + TILE - 1) / TILE;
   const uint32_t active = max(n_tiles, 1u);  // tile 0 also stands for the empty shard
   const uint32_t tile = blockIdx.x;
   if (tile >= active) return;
   const uint32_t lane = lane_id(), warp = threadIdx.x >> 5, tid = threadIdx.x;
   const uint32_t C = 1 + 2 * A.P;  // counters in use: [0] survivors, [1 + o*P + q] survivors of ordering o owned by q
   const uint32_t ep = epoch << CS_COUNT_BITS;
-  // the window parity is rewritten: every owner must have consumed the step that used it two steps ago
-  if (tid < A.P && A.step > 2) {
-    const long long t0 = clock64();
-    while (ld_acquire_sys(&mine->ack[tid]) < A.step - 2) {
-      if (clock64() - t0 > SH_SPIN_LIMIT) {
-        atomicExch(err, 1u);
-        break;
-      }
-    }
-  }
+  shard_wait_acks(A, mine, err);
   if (n_tiles == 0) {
     if (tid == 0) op.finish(0);
     if (tid < 2 * A.P) A.totals[tid] = 0;
   } else {
-    const uint32_t base = tile * TILE + warp * WARP_ITEMS;
-    typename Op::Item item[ROWS];
-#pragma unroll
-    for (int k = 0; k < ROWS; k++) {
-      const uint32_t i = base + k * 32 + lane;
-      item[k] = op.load(i, i < n);
-    }
-    uint32_t bal[ROWS], aux[ROWS];
-    uint32_t wtot = 0;
-#pragma unroll
-    for (int k = 0; k < ROWS; k++) {
-      const uint32_t i = base + k * 32 + lane;
-      const bool p = i < n && op.pred(item[k], i);
-      bal[k] = __ballot_sync(KVG_FULL, p);
-      wtot += __popc(bal[k]);
-      aux[k] = p ? op.prepare(item[k]) : 0u;
-    }
+    ClassifyTile<Op, THREADS, ROWS> ct;
+    ct.classify(op, tile);
     static_assert(2 * SH_MAX_RANKS == 32, "one lane per counter");
     (&s_wcnt[warp][0][0])[lane] = 0;
     __syncwarp();
@@ -295,43 +283,26 @@ __global__ void __launch_bounds__(THREADS, CW4 <= 2 ? KVG_CS_MINB : KVG_CS_MINB_
     uint32_t pos0[2] = {0, 0}, pos1[2] = {0, 0};
 #pragma unroll
     for (int k = 0; k < ROWS; k++) {
-      const bool p = (bal[k] >> lane) & 1u;
-      const uint2 key = op.keys(item[k], aux[k]);
-#pragma unroll
-      for (uint32_t o = 0; o < 2; o++) {
-        const uint32_t q = p ? shard_owner(o ? key.y : key.x, A) : SH_ALL;
-        const uint32_t same = __match_any_sync(KVG_FULL, q);
-        const uint32_t before = __popc(same & lanemask_lt());
-        const uint32_t prior = p ? s_wcnt[warp][o][q] : 0;
-        const uint32_t at = prior + before;  // < 256
-        if (o == 0)
-          pos0[k >> 2] |= at << (8 * (k & 3));
-        else
-          pos1[k >> 2] |= at << (8 * (k & 3));
-        __syncwarp();
-        if (p && before == 0) s_wcnt[warp][o][q] = prior + __popc(same);  // one lane per owner advances
-        __syncwarp();
-      }
+      const bool p = (ct.bal[k] >> lane) & 1u;
+      const uint2 key = op.keys(ct.item[k], ct.aux[k]);
+      pos0[k >> 2] |= shard_warp_rank(s_wcnt[warp], 0, p ? shard_owner(key.x, A) : SH_ALL) << (8 * (k & 3));  // < 256
+      pos1[k >> 2] |= shard_warp_rank(s_wcnt[warp], 1, p ? shard_owner(key.y, A) : SH_ALL) << (8 * (k & 3));
     }
-    if (lane == 0) s_wtot[warp] = wtot;
+    if (lane == 0) s_wtot[warp] = ct.wtot;
     __syncthreads();
     {
       uint32_t l = 0;
 #pragma unroll
       for (uint32_t w = 0; w < NW; w++)
         if (w < warp) l += s_wtot[w];
+      ct.emit(l, [&](uint32_t my, const typename Op::Item& r, uint32_t i, uint32_t a) {
+        uint4 rec[U];
+        op.make(r, i, a, rec);
 #pragma unroll
-      for (int k = 0; k < ROWS; k++) {
-        if ((bal[k] >> lane) & 1u) {
-          const uint32_t my = l + __popc(bal[k] & lanemask_lt());
-          uint4 rec[U];
-          op.make(item[k], base + k * 32 + lane, aux[k], rec);
-#pragma unroll
-          for (int u = 0; u < U; u++) s_rec[my * U + u] = rec[u];
-          s_meta[my] = warp | (((pos0[k >> 2] >> (8 * (k & 3))) & 0xffu) << 2) | (((pos1[k >> 2] >> (8 * (k & 3))) & 0xffu) << 10);
-        }
-        l += __popc(bal[k]);
-      }
+        for (int u = 0; u < U; u++) s_rec[my * U + u] = rec[u];
+        const uint32_t k = (i - ct.base) / 32;  // the record's row
+        s_meta[my] = warp | (((pos0[k >> 2] >> (8 * (k & 3))) & 0xffu) << 2) | (((pos1[k >> 2] >> (8 * (k & 3))) & 0xffu) << 10);
+      });
     }
     // counts of the tile -> published words; the warps' counts become prefixes over the warps in place
     if (warp == 0) {
@@ -413,7 +384,6 @@ __global__ void __launch_bounds__(THREADS, CW4 <= 2 ? KVG_CS_MINB : KVG_CS_MINB_
     {
       const uint32_t tile_total = s_agg[0];
       const size_t out0 = s_excl[0];
-      uint4* out = reinterpret_cast<uint4*>(op.out);
       uint32_t mx0 = 0, mx1 = 0;
       for (uint32_t l = tid; l < tile_total; l += THREADS) {
         uint4 rec[U];
@@ -421,17 +391,14 @@ __global__ void __launch_bounds__(THREADS, CW4 <= 2 ? KVG_CS_MINB : KVG_CS_MINB_
         for (int u = 0; u < U; u++) rec[u] = s_rec[l * U + u];
         const uint32_t meta = s_meta[l];
 #pragma unroll
-        for (int u = 0; u < U; u++) st_stream(out + (out0 + l) * U + u, rec[u]);
+        for (int u = 0; u < U; u++) st_stream(op.out + (out0 + l) * U + u, rec[u]);
         const uint2 key = shard_keys<U>(rec);
         mx0 = max(mx0, key.x);
         mx1 = max(mx1, key.y);
 #pragma unroll
         for (uint32_t o = 0; o < 2; o++) {
           const uint32_t q = shard_owner(o ? key.y : key.x, A);
-          const uint32_t at = s_excl[1 + o * A.P + q] + s_wcnt[meta & 3u][o][q] + ((meta >> (2 + 8 * o)) & 0xffu);
-          uint4* dst = peers.win[q] + shard_region(A, o, A.src, U) + (size_t)at * U;
-#pragma unroll
-          for (int u = 0; u < U; u++) dst[u] = rec[u];  // NVLink store (or local)
+          shard_store<U>(peers, A, q, o, s_excl[1 + o * A.P + q] + s_wcnt[meta & 3u][o][q] + ((meta >> (2 + 8 * o)) & 0xffu), rec);
         }
       }
       // largest keys of the shard (the radix plans): ordering 0 -> max_devkey, ordering 1 -> max_group

@@ -33,14 +33,12 @@ int emu_classify_pci(const uint4* recs, uint32_t n, const uint32_t* nv_index, in
   op.n = n;
   op.ctrl = &ctrl;
   op.nv_index = nv_index;
-  op.local_max_group = 0;
-  op.local_max_dev = 0;
   const uint32_t epoch = 7;
   if (variant == 1) {
-    op.out = (kvg_pci_surv*)surv_out;
+    op.out = surv_out;
     emu_launch(k_classify_oneshot<PciClassifyOp, T, R>, dim3((unsigned)(tiles ? tiles : 1)), T, op, state.data(), epoch);
   } else if (tiles) {
-    op.out = (kvg_pci_surv*)ragged.data();
+    op.out = ragged.data();
     emu_launch(k_classify_ragged<PciClassifyOp, T, R>, dim3((unsigned)tiles), T, op, tile_count.data(), tile_max.data());
     TileOffsetsArgs2 tt;
     tt.o[0] = {tile_count.data(), tile_max.data(), nullptr, (uint32_t)tiles, tile_off.data(), &ctrl.n_surv, state.data()};
@@ -112,8 +110,6 @@ int emu_scan_mdev(const uint4* recs, uint32_t n, const uint8_t* raw, const uint3
   op.ctrl = &ctrl;
   op.type_canon = canon;
   op.n_types = n_types;
-  op.local_max_parent = 0;
-  op.local_max_type = 0;
   if (tiles) {
     emu_launch(k_classify_ragged<MdevClassifyOp, T, R>, dim3((unsigned)tiles), T, op, tile_count.data(), tile_max.data());
     TileOffsetsArgs2 tt;

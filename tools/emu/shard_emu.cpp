@@ -145,11 +145,9 @@ static int run_fused(const uint4* const* recs, const uint32_t* n, uint32_t P, ui
       PciClassifyOp op;
       op.recs = recs[r];
       op.n = n[r];
-      op.out = (kvg_pci_surv*)(surv_out + (size_t)r * cap);
+      op.out = surv_out + (size_t)r * cap;
       op.ctrl = &sc[r];
       op.nv_index = nv_index;
-      op.local_max_group = 0;
-      op.local_max_dev = 0;
       emu_launch(k_classify_send<PciClassifyOp, TH, ROWS, CW4>, dim3((unsigned)tiles), TH, op, args(r, step), peers,
                  (const ShardCtrl*)&ctrl[r], &err, words[r].data(), 40u + step);
       n_surv_out[r] = sc[r].n_surv;
