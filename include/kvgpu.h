@@ -14,6 +14,7 @@
  *                                            (+ readVgpuIDFromFileFunc label rule :334-344, join :152-155)
  *   kvg_health_rescan                     <- health flips fed to ListAndWatch
  *                                            generic_device_plugin.go:325-342, :611-690
+ *   kvg_scan_pci_delta                    <- (no reference equivalent: the reference never re-scans)
  *   kvg_comm_*, kvg_scan_pci_sharded      <- (no reference equivalent; BASELINE.json config 4)
  *
  * Plain C: pointers + sizes only, no C++ types, no exceptions cross this boundary.
@@ -238,6 +239,39 @@ typedef struct kvg_health_delta {
   const uint32_t *changed; /* [n_changed] (record index << 1) | now_alive, ascending index */
 } kvg_health_delta;
 
+/* ---- re-scan delta (K7): what changed since the previous kvg_scan_pci_delta ------------------ */
+enum {
+  KVG_CH_ADDED = 1u << 0,   /* survives now, did not before                    */
+  KVG_CH_REMOVED = 1u << 1, /* survived before, does not now                    */
+  KVG_CH_GROUP = 1u << 2,   /* survives on both sides with another iommu group  */
+  KVG_CH_DEVICE = 1u << 3,  /* ... another device id                            */
+  KVG_CH_NUMA = 1u << 4     /* ... another clamped NUMA node                    */
+};
+
+typedef struct kvg_pci_change { /* 32 bytes; one per address whose survivor differs */
+  uint32_t addr;
+  uint32_t what;                  /* KVG_CH_* */
+  uint32_t prev_group, now_group; /* 0 on the absent side */
+  uint16_t prev_device, now_device;
+  uint16_t prev_numa, now_numa;   /* clamped, as in kvg_pci_surv */
+  uint32_t now_index;  /* index into this result's survivors, or 0xffffffff (removed) */
+  uint32_t prev_index; /* index into the previous delta scan's survivors, or 0xffffffff (added) */
+} kvg_pci_change;
+
+typedef struct kvg_pci_delta {
+  uint64_t n_prev;    /* survivors of the previous result (0: first call / after reset) */
+  uint64_t n_changes;
+  const kvg_pci_change *changes; /* [n_changes] ascending addr */
+  uint32_t n_dev_dirty;
+  const uint32_t *dev_dirty; /* indices into res->dev_keys, ascending */
+  uint32_t n_dev_gone;
+  const uint16_t *dev_gone;  /* device ids of the previous result absent now, ascending */
+  uint32_t n_grp_dirty;
+  const uint32_t *grp_dirty; /* indices into res->grp_keys, ascending */
+  uint32_t n_grp_gone;
+  const uint32_t *grp_gone;  /* groups of the previous result absent now, ascending */
+} kvg_pci_delta;
+
 /* ---- context -------------------------------------------------------------------------------- */
 typedef struct kvg_ctx kvg_ctx;
 
@@ -290,6 +324,35 @@ int kvg_scan_mdev(kvg_ctx *ctx, const kvg_mdev_rec *recs, size_t n, const kvg_ty
  * not checked.  Pageable memory is staged and has no alignment requirement. */
 int kvg_health_rescan(kvg_ctx *ctx, const kvg_pci_rec *recs, size_t n, kvg_health_delta **delta);
 int kvg_health_reset(kvg_ctx *ctx);
+
+/* Scan `recs` and diff the result against the previous one, keyed by survivor address.
+ *
+ * *res is byte for byte what kvg_scan_pci(ctx, recs, n, ...) returns for the same input, at every size (single
+ * copy, pipelined, split classify and final steps).  *res and *delta are both freed with kvg_result_free.
+ *
+ * "Previous" is the result of the last SUCCESSFUL kvg_scan_pci_delta on this context since kvg_ctx_create or
+ * kvg_scan_pci_delta_reset; before any such call it is empty, so every survivor is KVG_CH_ADDED, every key is dirty
+ * and nothing is gone.  The library keeps its own copy of it: kvg_scan_pci, kvg_dev_scan_pci*, the mdev scans,
+ * kvg_health_rescan, the sharded scans and kvg_pciids_load in between leave it unchanged.
+ *
+ * changes: an address has an entry iff it survives on exactly one side, or on both with a different iommu group,
+ * device id or clamped NUMA node.  The name slot is not compared (a pci.ids reload is the caller's own event).
+ * dev_dirty / grp_dirty: key k of deviceMap (iommuMap) is dirty iff the sequence of (addr, numa) of its members, in
+ * Walk order, differs between the two results; keys that are new are dirty.  So a group-only change dirties
+ * iommuMap keys and no deviceMap key, a device-only change deviceMap keys and no group, a NUMA change the key of
+ * the device and the key of the group.  dev_gone / grp_gone: keys present before and absent now.
+ *
+ * Precondition: survivor addresses ascend strictly, and a handle means the same device in both snapshots.
+ * Numeric (packed-BDF) snapshots satisfy both.  Strict ascent is checked on the device: if it fails the call
+ * returns KVG_EINVAL (text in kvg_last_error), hands out no objects, and the previous result stays as it was.
+ * Index-mode handles ascend but are not stable across snapshots: such calls are accepted, and the delta is then
+ * relative to the handles only (a device that moved in the Walk shows as changed or as removed + added).
+ *
+ * Cost beyond kvg_scan_pci on the same input: two kernel launches and one synchronisation. */
+int kvg_scan_pci_delta(kvg_ctx *ctx, const kvg_pci_rec *recs, size_t n, kvg_pci_result **res,
+                       kvg_pci_delta **delta);
+/* forget the previous result: the next kvg_scan_pci_delta reports everything as added */
+int kvg_scan_pci_delta_reset(kvg_ctx *ctx);
 
 /* ---- device-resident entry points (inputs already in HBM; used by bench.py "value") -------- */
 

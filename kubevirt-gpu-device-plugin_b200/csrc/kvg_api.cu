@@ -31,6 +31,7 @@
 #include "kvg_scan.cuh"
 #include "kvg_order.cuh"
 #include "kvg_shard.cuh"
+#include "kvg_delta.cuh"
 
 using namespace kvg;
 
@@ -39,6 +40,7 @@ using namespace kvg;
 #include "api/kvg_api_pciids.inc"
 #include "api/kvg_api_scan.inc"
 #include "api/kvg_api_health.inc"
+#include "api/kvg_api_delta.inc"
 #include "api/kvg_api_mdev.inc"
 #include "api/kvg_api_util.inc"
 #include "api/kvg_api_shard.inc"

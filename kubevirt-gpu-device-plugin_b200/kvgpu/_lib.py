@@ -32,7 +32,12 @@ MDEV_REC = np.dtype([("uuid", "u1", (16,)), ("parent", "<u4"), ("type_idx", "<u2
                      ("pad0", "u1"), ("parent_numa", "<i2"), ("pad1", "u1", (6,))])
 MDEV_SURV = np.dtype([("uuid", "u1", (16,)), ("parent", "<u4"), ("type_key", "<u2"),
                       ("numa", "<u2"), ("src", "<u4"), ("pad", "<u4")])
-assert PCI_REC.itemsize == 16 and PCI_SURV.itemsize == 16
+PCI_CHANGE = np.dtype([("addr", "<u4"), ("what", "<u4"), ("prev_group", "<u4"), ("now_group", "<u4"),
+                       ("prev_device", "<u2"), ("now_device", "<u2"), ("prev_numa", "<u2"), ("now_numa", "<u2"),
+                       ("now_index", "<u4"), ("prev_index", "<u4")])
+CH_ADDED, CH_REMOVED, CH_GROUP, CH_DEVICE, CH_NUMA = 1, 2, 4, 8, 16
+NO_INDEX = 0xFFFFFFFF
+assert PCI_REC.itemsize == 16 and PCI_SURV.itemsize == 16 and PCI_CHANGE.itemsize == 32
 assert MDEV_REC.itemsize == 32 and MDEV_SURV.itemsize == 32
 
 
@@ -98,6 +103,14 @@ class HealthDeltaC(C.Structure):
                 ("changed", C.c_void_p)]
 
 
+class PciDeltaC(C.Structure):
+    _fields_ = [("n_prev", C.c_uint64), ("n_changes", C.c_uint64), ("changes", C.c_void_p),
+                ("n_dev_dirty", C.c_uint32), ("dev_dirty", C.c_void_p),
+                ("n_dev_gone", C.c_uint32), ("dev_gone", C.c_void_p),
+                ("n_grp_dirty", C.c_uint32), ("grp_dirty", C.c_void_p),
+                ("n_grp_gone", C.c_uint32), ("grp_gone", C.c_void_p)]
+
+
 def declared_symbols() -> list[str]:
     """Every function name include/kvgpu.h declares (used by the export test)."""
     src = open(HEADER_PATH).read()
@@ -135,6 +148,8 @@ def load() -> C.CDLL:
         "kvg_scan_mdev": (C.c_int, [vp, vp, sz, P(TypeDict), P(P(MdevResultC))]),
         "kvg_health_rescan": (C.c_int, [vp, vp, sz, P(P(HealthDeltaC))]),
         "kvg_health_reset": (C.c_int, [vp]),
+        "kvg_scan_pci_delta": (C.c_int, [vp, vp, sz, P(P(PciResultC)), P(P(PciDeltaC))]),
+        "kvg_scan_pci_delta_reset": (C.c_int, [vp]),
         "kvg_text_pad": (sz, [sz]),
         "kvg_dev_pciids_parse": (C.c_int, [vp, vp, sz, sz, u32]),
         "kvg_dev_scan_pci": (C.c_int, [vp, vp, sz]),

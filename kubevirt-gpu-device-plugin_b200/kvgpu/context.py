@@ -71,6 +71,17 @@ class HealthDelta:
     changed: np.ndarray         # (index << 1) | now_alive
 
 
+@dataclass
+class PciDelta:
+    """What changed since the previous scan_pci_delta (include/kvgpu.h kvg_pci_delta)."""
+    n_prev: int
+    changes: np.ndarray         # PCI_CHANGE, ascending addr
+    dev_dirty: np.ndarray       # u32 indices into the result's dev_keys, ascending
+    dev_gone: np.ndarray        # u16 device ids absent now, ascending
+    grp_dirty: np.ndarray       # u32 indices into the result's grp_keys, ascending
+    grp_gone: np.ndarray        # u32 groups absent now, ascending
+
+
 class _LockedLib:
     """A kvg_ctx is single-threaded (include/kvgpu.h).  gRPC handler threads, the health feed and the
     Allocate re-validation all share one Context (kvgpu/serve.py), so every C call on it is serialised."""
@@ -245,6 +256,25 @@ class Context:
 
     def health_reset(self):
         self._ck(self._lib.kvg_health_reset(self._h))
+
+    def scan_pci_delta(self, recs: np.ndarray):
+        """scan_pci plus the keyed diff against the previous scan_pci_delta on this context -> (PciResult, PciDelta).
+        Meaningful for numeric (packed-BDF) snapshots; with index-mode handles it is relative to the handles."""
+        recs = np.ascontiguousarray(recs, dtype=L.PCI_REC)
+        res = C.POINTER(L.PciResultC)()
+        dl = C.POINTER(L.PciDeltaC)()
+        self._ck(self._lib.kvg_scan_pci_delta(self._h, recs.ctypes.data, len(recs), C.byref(res), C.byref(dl)))
+        d = dl.contents
+        delta = PciDelta(int(d.n_prev), L._arr(d.changes, int(d.n_changes), L.PCI_CHANGE),
+                         L._arr(d.dev_dirty, int(d.n_dev_dirty), np.uint32),
+                         L._arr(d.dev_gone, int(d.n_dev_gone), np.uint16),
+                         L._arr(d.grp_dirty, int(d.n_grp_dirty), np.uint32),
+                         L._arr(d.grp_gone, int(d.n_grp_gone), np.uint32))
+        self._lib.kvg_result_free(dl)
+        return self._take_pci(res), delta
+
+    def scan_pci_delta_reset(self):
+        self._ck(self._lib.kvg_scan_pci_delta_reset(self._h))
 
     # -- device-resident entry points (raw device pointers, e.g. torch tensor.data_ptr()) ----
     def text_pad(self, n: int) -> int:

@@ -372,6 +372,69 @@ def pci_maps_from_result(res: PciResult, snap: PciSnapshot | None = None, maps: 
     return m
 
 
+@dataclass
+class PciMapsTouched:
+    """The deviceMap / iommuMap keys apply_pci_delta rewrote (dirty: present now, new ones included) or removed."""
+    dev_dirty: list
+    dev_gone: list
+    grp_dirty: list
+    grp_gone: list
+
+
+def _fully_numeric(snap: PciSnapshot | None) -> bool:
+    return snap is None or (snap.packed_addr and snap.group_names is None and snap.device_names is None)
+
+
+def _rebuild_pci_maps(maps: Maps, res: PciResult, snap, name_of) -> PciMapsTouched:
+    """pci_maps_from_result into `maps`, reporting every key of the new maps and every key that went."""
+    before_dev, before_grp = set(maps.deviceMap), set(maps.iommuMap)
+    pci_maps_from_result(res, snap, maps, name_of=name_of)
+    return PciMapsTouched(list(maps.deviceMap), sorted(before_dev - set(maps.deviceMap)),
+                          list(maps.iommuMap), sorted(before_grp - set(maps.iommuMap)))
+
+
+def apply_pci_delta(maps: Maps, res: PciResult, delta, snap: PciSnapshot | None = None,
+                    prev_snap: PciSnapshot | None = None, name_of=None) -> PciMapsTouched:
+    """Patch deviceMap, iommuMap and bdfToIommuMap of `maps` (built from the previous delta scan's result) into
+    what pci_maps_from_result(res) builds, touching only dirty or gone keys and changed addresses.  A snapshot
+    that is not fully numeric (index-mode addresses, groups or device strings) has no stable handles: the maps are
+    then rebuilt and every key is reported."""
+    if not (_fully_numeric(snap) and _fully_numeric(prev_snap)):
+        return _rebuild_pci_maps(maps, res, snap, name_of)
+    s = res.survivors
+
+    def members(perm, off, k):
+        idx = perm[off[k]:off[k + 1]]
+        return [NvidiaGpuDevice(format_bdf(int(s["addr"][i])), int(s["numa"][i])) for i in idx]
+
+    t = PciMapsTouched([], [], [], [])
+    for k in delta.dev_dirty:
+        key = "%04x" % int(res.dev_keys[k])
+        maps.deviceMap[key] = members(res.dev_perm, res.dev_off, k)
+        maps.deviceNames[key] = res.name_at(int(res.dev_name_slot[k]))
+        t.dev_dirty.append(key)
+    for d in delta.dev_gone:
+        key = "%04x" % int(d)
+        maps.deviceMap.pop(key, None)
+        maps.deviceNames.pop(key, None)
+        t.dev_gone.append(key)
+    for k in delta.grp_dirty:
+        key = str(int(res.grp_keys[k]))
+        maps.iommuMap[key] = members(res.grp_perm, res.grp_off, k)
+        t.grp_dirty.append(key)
+    for g in delta.grp_gone:
+        key = str(int(g))
+        maps.iommuMap.pop(key, None)
+        t.grp_gone.append(key)
+    for c in delta.changes:
+        addr = format_bdf(int(c["addr"]))
+        if c["what"] & L.CH_REMOVED:
+            maps.bdfToIommuMap.pop(addr, None)
+        else:
+            maps.bdfToIommuMap[addr] = str(int(c["now_group"]))
+    return t
+
+
 def mdev_maps_from_result(res: MdevResult, snap: MdevSnapshot | None = None, maps: Maps | None = None) -> Maps:
     m = maps or Maps()
     m.vGpuMap, m.gpuVgpuMap = {}, {}  # :256-257
@@ -445,6 +508,7 @@ class DiscoveryScan:
         self.ctx = Context(device)
         self.maps = Maps()
         self._loaded_path = None
+        self._prev_pci_snap = None   # snapshot of the last rescan_iommu_device_map
 
     def close(self):
         self.ctx.close()
@@ -469,6 +533,17 @@ class DiscoveryScan:
             raise
         res = self.ctx.scan_pci(snap.recs)
         return pci_maps_from_result(res, snap, self.maps, name_of=self.ctx.name_lookup)
+
+    def rescan_iommu_device_map(self) -> PciMapsTouched:
+        """Re-walk the tree and bring deviceMap / iommuMap / bdfToIommuMap up to date through the re-scan delta.
+        The first call has no previous delta scan to diff against: it rebuilds the maps and reports every key."""
+        self._ensure_table()
+        snap = snapshot_pci_tree(self.basePath)
+        res, delta = self.ctx.scan_pci_delta(snap.recs)
+        prev, self._prev_pci_snap = self._prev_pci_snap, snap
+        if prev is None:
+            return _rebuild_pci_maps(self.maps, res, snap, self.ctx.name_lookup)
+        return apply_pci_delta(self.maps, res, delta, snap, prev, name_of=self.ctx.name_lookup)
 
     def create_vgpu_id_map(self) -> Maps:
         self._ensure_table()

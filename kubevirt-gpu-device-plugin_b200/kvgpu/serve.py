@@ -15,7 +15,8 @@ Allocate" is testable end to end in an image without a Go toolchain.
 
 Nothing here computes on the CPU what the scan computes on the GPU: the maps come from
 plugin.DiscoveryScan (libkvgpu.so); the re-validation's classification goes through
-Context.scan_pci (K3); the health feed through Context.health_rescan (K6).
+Context.scan_pci (K3); the health feed through Context.health_rescan (K6); the hot-plug feed through
+Context.scan_pci_delta (K7).
 """
 from __future__ import annotations
 
@@ -31,7 +32,7 @@ import numpy as np
 from . import _lib as L
 from . import dpapi
 from .plugin import (DEVICE_NAMESPACE, GPU_PREFIX, VGPU_PREFIX, Maps, PluginSpec, ReferencePanic, _read_id,
-                     _read_link, _read_vgpu_raw)
+                     _read_link, _read_vgpu_raw, _rebuild_pci_maps, apply_pci_delta, plugin_specs_from_maps)
 
 VFIO_DEVICE_PATH = "/dev/vfio"      # generic_device_plugin.go:54
 IOMMU_DEVICE_PATH = "/dev/iommu"    # :55
@@ -251,7 +252,8 @@ class _PluginBase:
         self.socket_path = os.path.join(socket_dir, "kubevirt-%s.sock" % device_name)
         self.kubelet_socket = kubelet_socket or os.path.join(socket_dir, "kubelet.sock")
         self.server = None
-        self._events = queue.Queue()     # ("healthy" | "unhealthy", device id): the two Go channels
+        self._events = queue.Queue()     # ("healthy" | "unhealthy", device id): the two Go channels;
+                                         # ("devices", None): the device list changed (PciRescanFeed)
         self._stop = threading.Event()
         self._term = threading.Event()
         self._lock = threading.Lock()
@@ -262,6 +264,16 @@ class _PluginBase:
 
     def unhealthy(self, dev_id: str):
         self._events.put(("unhealthy", dev_id))
+
+    def set_devices(self, devs: list):
+        """A new device list (a re-scan changed this key): devices that stay keep their current health, and
+        ListAndWatch re-sends the whole list."""
+        with self._lock:
+            health = {d.ID: d.health for d in self.devs}
+            for d in devs:
+                d.health = health.get(d.ID, d.health)
+            self.devs = list(devs)
+        self._events.put(("devices", None))
 
     def resource_name(self) -> str:
         return "%s/%s" % (DEVICE_NAMESPACE, self.device_name)
@@ -276,7 +288,8 @@ class _PluginBase:
         return dpapi.PreStartContainerResponse()
 
     def ListAndWatch(self, request, context):
-        """:312-349 — send the list once, then the whole list again after every health flip."""
+        """:312-349 — send the list once, then the whole list again after every health flip and after every
+        set_devices."""
         yield dpapi.ListAndWatchResponse(devices=self.devs)
         while not (self._stop.is_set() or self._term.is_set()):
             if context is not None and not context.is_active():
@@ -287,9 +300,10 @@ class _PluginBase:
                 continue
             with self._lock:
                 for dev in self.devs:
-                    if dev.ID == dev_id:
+                    if kind != "devices" and dev.ID == dev_id:
                         dev.health = dpapi.HEALTHY if kind == "healthy" else dpapi.UNHEALTHY
-            yield dpapi.ListAndWatchResponse(devices=self.devs)
+                devs = list(self.devs)
+            yield dpapi.ListAndWatchResponse(devices=devs)
 
     # -- lifecycle
     def _handlers(self):
@@ -534,6 +548,62 @@ class HealthRescanFeed:
                     sent += 1
         self._primed = True
         return sent
+
+    def start(self):
+        def loop():
+            while not self._stop.is_set():
+                self.tick()
+                time.sleep(self.period_s)
+        self._thread = threading.Thread(target=loop, daemon=True)
+        self._thread.start()
+
+    def stop(self):
+        self._stop.set()
+        if self._thread:
+            self._thread.join(2.0)
+
+
+# ------------------------------------------------------------------------------------------------
+# hot-plug feed driven by the K7 re-scan delta
+# ------------------------------------------------------------------------------------------------
+class PciRescanFeed:
+    """Periodic re-snapshot -> Context.scan_pci_delta (K7) -> the shared maps and the set of passthrough plugins.
+
+    `snapshot()` returns a PciSnapshot, `scan_delta(recs)` is Context.scan_pci_delta, `plugins` maps deviceMap keys
+    to running plugins and `make_plugin(spec)` builds one for a new key.  Each tick patches `maps` in place (Allocate
+    reads iommuMap / bdfToIommuMap from it, so it sees a moved device at once), gives every plugin whose key is
+    dirty its new device list, starts and registers a plugin for every new key, and stops the plugin of every key
+    that went.  The first tick has no previous snapshot: it rebuilds the maps and treats every key as dirty."""
+
+    def __init__(self, scan_delta, snapshot, maps: Maps, plugins: dict, make_plugin, period_s: float = 0.01):
+        self.scan_delta, self.snapshot, self.maps = scan_delta, snapshot, maps
+        self.plugins, self.make_plugin, self.period_s = plugins, make_plugin, period_s
+        self._prev_snap = None
+        self._stop = threading.Event()
+        self._thread = None
+
+    def tick(self):
+        snap = self.snapshot()
+        res, delta = self.scan_delta(snap.recs)
+        if self._prev_snap is None:
+            touched = _rebuild_pci_maps(self.maps, res, snap, None)
+        else:
+            touched = apply_pci_delta(self.maps, res, delta, snap, self._prev_snap)
+        self._prev_snap = snap
+        dirty = Maps(deviceMap={k: self.maps.deviceMap[k] for k in touched.dev_dirty}, deviceNames=self.maps.deviceNames)
+        for spec in plugin_specs_from_maps(dirty):
+            plugin = self.plugins.get(spec.key)
+            if plugin is None:
+                plugin = self.make_plugin(spec)
+                plugin.start()
+                self.plugins[spec.key] = plugin
+            else:
+                plugin.set_devices(devices_from_spec(spec))
+        for key in touched.dev_gone:
+            plugin = self.plugins.pop(key, None)
+            if plugin is not None:
+                plugin.stop()
+        return touched
 
     def start(self):
         def loop():
