@@ -6,17 +6,21 @@
 //   * epoch-tagged decoupled look-back (single-pass chained scan) used by the stable compactions
 //     and by the vendor-context carry of the pci.ids parser
 #pragma once
-#include <cuda_runtime.h>
 #include <stdint.h>
 
 #define KVG_BLOCK 256
 #define KVG_WARPS (KVG_BLOCK / 32)
 #define KVG_FULL 0xffffffffu
 
+// ---- the hardware layer -------------------------------------------------------------------------
+// The inline PTX of the library lives in this one block.  The CPU emulator (tools/emu/warp_emu.h) defines
+// KVG_HOST_EMU and supplies the same functions; everything outside the block, and every kernel header, is
+// compiled from the same text for the GPU and for the emulator.
+#ifndef KVG_HOST_EMU
+#include <cuda_runtime.h>
+
 namespace kvg {
 
-__device__ __forceinline__ uint32_t lane_id() { return threadIdx.x & 31; }
-__device__ __forceinline__ uint32_t warp_id() { return threadIdx.x >> 5; }
 __device__ __forceinline__ uint32_t lanemask_lt() {
   uint32_t m;
   asm("mov.u32 %0, %%lanemask_lt;" : "=r"(m));
@@ -105,13 +109,13 @@ __device__ __forceinline__ void tma_load_1d(void* smem_dst, const void* gmem_src
       : "memory");
 }
 
-// named barriers (id 1..15; id 0 is __syncthreads): producer/consumer hand-off inside a CTA
-__device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {
-  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
-}
-__device__ __forceinline__ void named_bar_arrive(uint32_t id, uint32_t nthreads) {
-  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
-}
+}  // namespace kvg
+#endif  // KVG_HOST_EMU
+
+namespace kvg {
+
+__device__ __forceinline__ uint32_t lane_id() { return threadIdx.x & 31; }
+__device__ __forceinline__ uint32_t warp_id() { return threadIdx.x >> 5; }
 
 // ---- scans --------------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t warp_incl_sum(uint32_t v) {

@@ -29,9 +29,7 @@
 // nothing about it crosses the host; a pass above the largest key returns immediately and the ping-pong
 // parity tells consumers which buffer is final.
 #pragma once
-#ifndef KVG_HOST_EMU  // tools/emu/ compiles this file for the CPU on top of warp_emu.h instead
 #include "kvg_common.cuh"
-#endif
 
 namespace kvg {
 

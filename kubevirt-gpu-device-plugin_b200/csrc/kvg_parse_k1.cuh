@@ -35,9 +35,7 @@
 // path of the single-image parse: chains of dependent L2 atomics in the one span that holds the NVIDIA
 // header).
 #pragma once
-#ifndef KVG_HOST_EMU
 #include "kvg_parse.cuh"
-#endif
 
 namespace kvg {
 

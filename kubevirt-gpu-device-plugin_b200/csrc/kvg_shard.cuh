@@ -30,10 +30,8 @@
 // allgatherv) and the SAME kernels run in local mode on the gathered list: one source, only the records
 // this rank owns are kept.
 #pragma once
-#ifndef KVG_HOST_EMU
 #include "kvg_common.cuh"
 #include "kvg_order.cuh"
-#endif
 
 namespace kvg {
 

@@ -1,9 +1,8 @@
 #!/usr/bin/env python3
-"""Build the CPU twins of the CUDA kernels (tools/emu/_build/lib*_emu.so): kernel source is compiled
-verbatim on top of warp_emu.h; the helpers it needs are cut out of csrc/*.cuh at build time, so nothing is
-transcribed by hand."""
+"""Build the CPU twins of the CUDA kernels (tools/emu/_build/lib*_emu.so): each harness <name>_emu.cpp includes
+warp_emu.h and then the kernel headers of csrc/ whole, so the emulator compiles the same text nvcc compiles."""
+import glob
 import os
-import re
 import subprocess
 import sys
 
@@ -12,216 +11,46 @@ ROOT = os.path.dirname(os.path.dirname(HERE))
 CSRC = os.path.join(ROOT, "kubevirt-gpu-device-plugin_b200", "csrc")
 OUT = os.path.join(HERE, "_build")
 
-def func_body(src: str, name: str) -> str:
-    m = re.search(r"^__device__ __forceinline__ [\w ]+\b%s\(" % name, src, re.M)
-    assert m, name
-    i = src.index("{", m.end())
-    depth, j = 0, i
-    while True:
-        depth += {"{": 1, "}": -1}.get(src[j], 0)
-        j += 1
-        if depth == 0:
-            break
-    return src[m.start():j] + "\n"
 
-
-def cut_order(common: str, scan: str = "") -> str:
-    """What csrc/kvg_order.cuh (compiled whole, verbatim) needs from kvg_common.cuh: the warp / block scans
-    and the chained-scan words of the final kernel."""
-    out = ["// GENERATED by tools/emu/build.py from csrc/kvg_common.cuh — do not edit\n"]
-    out.append(func_body(common, "warp_incl_sum"))
-    out.append(func_body(common, "block_excl_sum"))
-    out.append(re.search(r"^enum : uint32_t \{ LB_INVALID.*$", common, re.M).group(0) + "\n")
-    out.append(re.search(r"^constexpr int LB_WIDE = [^;]+;.*$", common, re.M).group(0) + "\n")
-    for f in ("lb_pack", "lb_status", "lookback_sum"):
-        out.append(func_body(common, f))
-    return "".join(out)
-
-
-def definition(src: str, head_regex: str) -> str:
-    """A struct / function / kernel definition located by the regex of its head line(s); a preceding
-    `template <...>` line is included; the body is matched brace by brace (a struct keeps its `;`)."""
-    m = re.search(head_regex, src, re.M)
-    assert m, head_regex
-    start = m.start()
-    prev = src.rfind("\n", 0, start - 1) + 1
-    if src[prev:start].startswith("template <"):
-        start = prev
-    i = src.index("{", m.end() - 1)
-    depth, j = 0, i
-    while True:
-        depth += {"{": 1, "}": -1}.get(src[j], 0)
-        j += 1
-        if depth == 0:
-            break
-    if src[j:j + 1] == ";":
-        j += 1
-    return src[start:j] + "\n"
-
-
-def cut_classify(common: str, parse: str, scan: str) -> str:
-    """The classification pipeline of csrc/kvg_scan.cuh, verbatim: ScanCtrl, the tile front-end, the PCI
-    predicate and operator, k_classify_oneshot, k_classify_ragged, k_tile_offsets, k_pack_survivors (with the
-    pass-0 histograms of kvg_order.cuh, which the harness includes whole), the health diff, the mdev dictionary."""
-    out = ["// GENERATED by tools/emu/build.py — do not edit\n"]
-    out.append(re.search(r"^constexpr \w+ P_NONE = [^;]+;.*$", parse, re.M).group(0) + "\n")
-    out.append(definition(scan, r"^struct ScanCtrl \{"))
-    out.append(definition(scan, r"^struct ClassifyTile \{"))
-    out.append(definition(scan, r"^__device__ __forceinline__ void lookback_tile\("))
-    out.append(definition(scan, r"^__global__ void __launch_bounds__\(THREADS\) k_classify_oneshot\("))
-    out.append(func_body(scan, "pci_record_alive"))
-    out.append(definition(scan, r"^struct SurvivorOp \{"))
-    out.append(definition(scan, r"^struct PciClassifyOp : SurvivorOp<PciClassifyOp> \{"))
-    out.append(definition(scan, r"^__global__ void __launch_bounds__\(THREADS\) k_classify_ragged\("))
-    out.append(definition(scan, r"^struct TileOffsetsArgs \{"))
-    out.append(definition(scan, r"^struct TileOffsetsArgs2 \{"))
-    out.append(definition(scan, r"^__global__ void __launch_bounds__\(KVG_BLOCK\) k_tile_offsets\("))
-    out.append(definition(scan, r"^__global__ void __launch_bounds__\(128\) k_pack_survivors\("))
-    # K6: the health diff is the persistent look-back compaction with HealthOp
-    out.append(definition(scan, r"^__global__ void __launch_bounds__\(KVG_BLOCK\) k_compact\("))
-    out.append(definition(scan, r"^struct HealthOp \{"))
-    for c in ("HEALTH_SMALL_THREADS", "HEALTH_SMALL_ROWS", "HEALTH_SMALL_MAX", "HEALTH_STAGE_ROWS", "HEALTH_SMALL_SMEM"):
-        out.append(re.search(r"^constexpr \w+ %s = [^;]+;.*$" % c, scan, re.M).group(0) + "\n")
-    out.append(definition(scan, r"^__global__ void __launch_bounds__\(HEALTH_SMALL_THREADS\) k_health_small\("))
-    # K5: mdev records and the type dictionary (label rule + merge of equal labels)
-    out.append(func_body(parse, "d_re2_space"))
-    out.append(definition(scan, r"^struct MdevItem \{"))
-    out.append(definition(scan, r"^struct MdevClassifyOp : SurvivorOp<MdevClassifyOp> \{"))
-    out.append(definition(scan, r"^__global__ void k_mdev_labels\("))
-    out.append(definition(scan, r"^__global__ void k_mdev_canon\("))
-    return "".join(out)
-
-
-def _compile(lib: str, cpp: str):
+def build(name: str, force: bool = False) -> str:
+    """lib<name>_emu.so from <name>_emu.cpp; rebuilt when older than any header it may include (every
+    csrc/*.cuh, as the Makefile's HDRS rule does), the emulator, the harness or this script."""
+    os.makedirs(OUT, exist_ok=True)
+    lib = os.path.join(OUT, "lib%s_emu.so" % name)
+    cpp = os.path.join(HERE, "%s_emu.cpp" % name)
+    srcs = glob.glob(os.path.join(CSRC, "*.cuh")) + [
+        os.path.join(ROOT, "include", "kvgpu.h"), os.path.join(HERE, "warp_emu.h"), cpp, __file__]
+    if not force and os.path.exists(lib) and all(os.path.getmtime(lib) >= os.path.getmtime(s) for s in srcs):
+        return lib
     cmd = ["g++", "-std=c++20", "-O1", "-g", "-fPIC", "-shared", "-Wall", "-Wno-unused-function",
-           "-Wno-unknown-pragmas", "-I", OUT, "-I", HERE, "-I", os.path.join(ROOT, "include"), cpp, "-o", lib]
+           "-Wno-unknown-pragmas", "-I", HERE, cpp, "-o", lib]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode:
         sys.stderr.write(r.stderr)
         raise RuntimeError("emulation build failed")
-
-
-def _stale(lib: str, srcs: list) -> bool:
-    return not os.path.exists(lib) or any(os.path.getmtime(lib) < os.path.getmtime(s) for s in srcs)
+    return lib
 
 
 def build_radix(force: bool = False) -> str:
-    """libradix_emu.so: K4 (csrc/kvg_order.cuh, verbatim) on the CPU."""
-    os.makedirs(OUT, exist_ok=True)
-    lib = os.path.join(OUT, "libradix_emu.so")
-    srcs = [os.path.join(CSRC, "kvg_common.cuh"), os.path.join(CSRC, "kvg_order.cuh"), os.path.join(CSRC, "kvg_scan.cuh"),
-            os.path.join(HERE, "warp_emu.h"), os.path.join(HERE, "radix_emu.cpp"), __file__]
-    if not force and not _stale(lib, srcs):
-        return lib
-    with open(os.path.join(OUT, "emu_order.inc"), "w") as f:
-        f.write(cut_order(open(srcs[0]).read()))
-    scan = open(os.path.join(CSRC, "kvg_scan.cuh")).read()
-    with open(os.path.join(OUT, "emu_offsets.inc"), "w") as f:   # the chained scan of per-tile counts (k_order_heads path)
-        f.write("// GENERATED by tools/emu/build.py from csrc/kvg_scan.cuh — do not edit\n" +
-                definition(scan, r"^struct ScanCtrl \{") + definition(scan, r"^struct TileOffsetsArgs \{") +
-                definition(scan, r"^struct TileOffsetsArgs2 \{") +
-                definition(scan, r"^__global__ void __launch_bounds__\(KVG_BLOCK\) k_tile_offsets\("))
-    _compile(lib, os.path.join(HERE, "radix_emu.cpp"))
-    return lib
+    return build("radix", force)
 
 
 def build_shard(force: bool = False) -> str:
-    """libshard_emu.so: the exchange step of the sharded scan (csrc/kvg_shard.cuh, verbatim) on the CPU."""
-    os.makedirs(OUT, exist_ok=True)
-    lib = os.path.join(OUT, "libshard_emu.so")
-    srcs = [os.path.join(CSRC, "kvg_common.cuh"), os.path.join(CSRC, "kvg_order.cuh"), os.path.join(CSRC, "kvg_shard.cuh"),
-            os.path.join(HERE, "warp_emu.h"), os.path.join(HERE, "shard_emu.cpp"), __file__,
-            os.path.join(CSRC, "kvg_parse.cuh"), os.path.join(CSRC, "kvg_scan.cuh")]
-    if not force and not _stale(lib, srcs):
-        return lib
-    with open(os.path.join(OUT, "emu_order.inc"), "w") as f:
-        f.write(cut_order(open(srcs[0]).read()))
-    with open(os.path.join(OUT, "emu_classify.inc"), "w") as f:  # the classify operators of k_classify_send
-        f.write(cut_classify(open(srcs[0]).read(), open(srcs[6]).read(), open(srcs[7]).read()))
-    _compile(lib, os.path.join(HERE, "shard_emu.cpp"))
-    return lib
-
-
-def cut_names(parse: str) -> str:
-    """Everything of csrc/kvg_parse.cuh behind the parse itself, verbatim: the name transform, k_nv_index,
-    k_pciids_sanitise_lines, k_probe_keys, k_section_lines, k_lookup_general, k_sanitise_matches."""
-    a = parse.index("__device__ __forceinline__ bool d_ascii_space(")
-    b = parse.rindex("}  // namespace kvg")
-    return "// GENERATED by tools/emu/build.py from csrc/kvg_parse.cuh — do not edit\n" + parse[a:b]
-
-
-def cut_parse_all(common: str, parse: str) -> str:
-    """csrc/kvg_parse.cuh from its first constant to the end of its namespace, verbatim (k_pciids_parse with
-    its TMA ring, k_pciids_finalize, the name transform, every lookup kernel), preceded by the look-back word
-    helpers of kvg_common.cuh.  The one patch: dynamic shared memory becomes a static buffer."""
-    out = ["// GENERATED by tools/emu/build.py from csrc/kvg_common.cuh + csrc/kvg_parse.cuh — do not edit\n"]
-    out.append(re.search(r"^enum : uint32_t \{ LB_INVALID.*$", common, re.M).group(0) + "\n")
-    for f in ("lb_pack", "lb_status", "warp_incl_sum"):
-        out.append(func_body(common, f))
-    body = parse[parse.index("constexpr uint32_t P_TILE"):parse.rindex("}  // namespace kvg")]
-    out.append(body)
-    return "".join(out)
-
-
-def build_names(force: bool = False) -> str:
-    os.makedirs(OUT, exist_ok=True)
-    lib = os.path.join(OUT, "libnames_emu.so")
-    srcs = [os.path.join(CSRC, "kvg_parse.cuh"), os.path.join(CSRC, "kvg_parse_k1.cuh"),
-            os.path.join(HERE, "warp_emu.h"), os.path.join(HERE, "names_emu.cpp"), __file__]
-    if not force and not _stale(lib, srcs):
-        return lib
-    src = open(srcs[0]).read()
-    with open(os.path.join(OUT, "emu_parse_all.inc"), "w") as f:
-        f.write(cut_parse_all(open(os.path.join(CSRC, "kvg_common.cuh")).read(), src))
-    _compile(lib, os.path.join(HERE, "names_emu.cpp"))
-    return lib
+    return build("shard", force)
 
 
 def build_classify(force: bool = False) -> str:
-    os.makedirs(OUT, exist_ok=True)
-    lib = os.path.join(OUT, "libclassify_emu.so")
-    srcs = [os.path.join(CSRC, "kvg_common.cuh"), os.path.join(CSRC, "kvg_parse.cuh"), os.path.join(CSRC, "kvg_scan.cuh"),
-            os.path.join(CSRC, "kvg_order.cuh"), os.path.join(HERE, "warp_emu.h"), os.path.join(HERE, "classify_emu.cpp"), __file__]
-    if not force and not _stale(lib, srcs):
-        return lib
-    with open(os.path.join(OUT, "emu_order.inc"), "w") as f:
-        f.write(cut_order(open(srcs[0]).read()))
-    with open(os.path.join(OUT, "emu_classify.inc"), "w") as f:
-        f.write(cut_classify(open(srcs[0]).read(), open(srcs[1]).read(), open(srcs[2]).read()))
-    _compile(lib, os.path.join(HERE, "classify_emu.cpp"))
-    return lib
+    return build("classify", force)
 
 
-def cut_delta(scan: str, delta: str) -> str:
-    """K7 of csrc/kvg_delta.cuh from its first constant to the end of its namespace, verbatim, behind the pieces
-    of csrc/kvg_scan.cuh it runs on: ScanCtrl, the tile front-end and the look-back tile body."""
-    out = ["// GENERATED by tools/emu/build.py from csrc/kvg_scan.cuh + csrc/kvg_delta.cuh — do not edit\n"]
-    out.append(definition(scan, r"^struct ScanCtrl \{"))
-    out.append(definition(scan, r"^struct ClassifyTile \{"))
-    out.append(definition(scan, r"^__device__ __forceinline__ void lookback_tile\("))
-    out.append(delta[delta.index("constexpr int DELTA_THREADS"):delta.rindex("}  // namespace kvg")])
-    return "".join(out)
+def build_names(force: bool = False) -> str:
+    return build("names", force)
 
 
 def build_delta(force: bool = False) -> str:
-    """libdelta_emu.so: the re-scan delta (csrc/kvg_delta.cuh, verbatim) on the CPU."""
-    os.makedirs(OUT, exist_ok=True)
-    lib = os.path.join(OUT, "libdelta_emu.so")
-    srcs = [os.path.join(CSRC, "kvg_common.cuh"), os.path.join(CSRC, "kvg_scan.cuh"), os.path.join(CSRC, "kvg_delta.cuh"),
-            os.path.join(CSRC, "kvg_order.cuh"), os.path.join(HERE, "warp_emu.h"), os.path.join(HERE, "delta_emu.cpp"), __file__]
-    if not force and not _stale(lib, srcs):
-        return lib
-    with open(os.path.join(OUT, "emu_order.inc"), "w") as f:
-        f.write(cut_order(open(srcs[0]).read()))
-    with open(os.path.join(OUT, "emu_delta.inc"), "w") as f:
-        f.write(cut_delta(open(srcs[1]).read(), open(srcs[2]).read()))
-    _compile(lib, os.path.join(HERE, "delta_emu.cpp"))
-    return lib
+    return build("delta", force)
 
 
 if __name__ == "__main__":
-    print(build_radix(force=True))
-    print(build_shard(force=True))
-    print(build_classify(force=True))
-    print(build_names(force=True))
-    print(build_delta(force=True))
+    for name in ("radix", "shard", "classify", "names", "delta"):
+        print(build(name, force=True))

@@ -4,14 +4,7 @@
 // used below 2 M records (k_classify_oneshot).  Launch shapes are those of enqueue_classify (kvg_api.cu).
 #define KVG_HOST_EMU 1
 #include "warp_emu.h"
-#include "kvgpu.h"
-namespace kvg {
-#include "emu_order.inc"
-}
-#include "../../kubevirt-gpu-device-plugin_b200/csrc/kvg_order.cuh"   // tile constants
-namespace kvg {
-#include "emu_classify.inc"
-}
+#include "../../kubevirt-gpu-device-plugin_b200/csrc/kvg_scan.cuh"
 using namespace kvg;
 
 extern "C" {

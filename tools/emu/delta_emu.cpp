@@ -2,14 +2,7 @@
 // warp_emu.h: k_delta_merge then k_delta_lists, with the launch shapes of kvg_scan_pci_delta (kvg_api_delta.inc).
 #define KVG_HOST_EMU 1
 #include "warp_emu.h"
-#include "kvgpu.h"
-namespace kvg {
-#include "emu_order.inc"
-}
-#include "../../kubevirt-gpu-device-plugin_b200/csrc/kvg_order.cuh"   // tile constants
-namespace kvg {
-#include "emu_delta.inc"
-}
+#include "../../kubevirt-gpu-device-plugin_b200/csrc/kvg_delta.cuh"
 using namespace kvg;
 
 extern "C" {

@@ -6,9 +6,6 @@
 //   general path   k_section_lines -> k_lookup_general -> k_sanitise_matches   (every other key)
 #define KVG_HOST_EMU 1
 #include "warp_emu.h"
-namespace kvg {
-#include "emu_parse_all.inc"   // all of csrc/kvg_parse.cuh
-}
 #include "../../kubevirt-gpu-device-plugin_b200/csrc/kvg_parse_k1.cuh"
 using namespace kvg;
 

@@ -3,14 +3,7 @@
 // on top of warp_emu.h.  The launch sequence is the one of enqueue_orderings (kvg_api.cu).
 #define KVG_HOST_EMU 1
 #include "warp_emu.h"
-#include "kvgpu.h"
-namespace kvg {
-#include "emu_order.inc"
-}
-#include "../../kubevirt-gpu-device-plugin_b200/csrc/kvg_order.cuh"
-namespace kvg {
-#include "emu_offsets.inc"
-}
+#include "../../kubevirt-gpu-device-plugin_b200/csrc/kvg_scan.cuh"
 
 using namespace kvg;
 

@@ -4,14 +4,7 @@
 // kernels of a step run rank after rank (all sends, then all gathers — the order the flags allow).
 #define KVG_HOST_EMU 1
 #include "warp_emu.h"
-#include "kvgpu.h"
-namespace kvg {
-#include "emu_order.inc"
-}
-#include "../../kubevirt-gpu-device-plugin_b200/csrc/kvg_order.cuh"
-namespace kvg {
-#include "emu_classify.inc"
-}
+#include "../../kubevirt-gpu-device-plugin_b200/csrc/kvg_scan.cuh"
 #include "../../kubevirt-gpu-device-plugin_b200/csrc/kvg_shard.cuh"
 using namespace kvg;
 

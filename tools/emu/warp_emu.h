@@ -6,6 +6,10 @@
 // execute, leave the block with runnable-but-blocked fibers only, which the scheduler reports as a
 // deadlock (abort) — the CPU-side picture of a mis-synchronised kernel.
 //
+// A harness defines KVG_HOST_EMU, includes this file, then includes the kernel headers of csrc/ whole:
+// kvg_common.cuh skips its inline-PTX block, whose functions are defined here, and everything else is
+// compiled from the same text nvcc compiles.
+//
 // Test infrastructure only (tests/test_*_emu.py); never part of the product.
 #pragma once
 #include <cassert>
@@ -70,26 +74,12 @@ static inline void emu_yield() {
 #define __shared__ static
 #define __align__(n) __attribute__((aligned(n)))
 #define __restrict__ __restrict
-#define KVG_FULL 0xffffffffu
-constexpr uint32_t KVG_BLOCK = 256;
-constexpr uint32_t KVG_WARPS = KVG_BLOCK / 32;
 
-static inline uint32_t lane_id() { return threadIdx.x & 31u; }
-static inline uint32_t warp_id() { return threadIdx.x >> 5; }
-static inline void pdl_enter() {}
+static inline uint32_t emu_lane() { return threadIdx.x & 31u; }
+static inline uint32_t emu_warp() { return threadIdx.x >> 5; }
 static inline void __threadfence() {}
 static inline void __threadfence_system() {}
 static inline long long clock64() { return 0; }
-static inline uint4 ld_stream(const uint4* p) { return *p; }
-static inline void st_stream(uint4* p, const uint4& v) { *p = v; }
-static inline uint64_t ld_relaxed_u64(const uint64_t* p) { return __atomic_load_n(p, __ATOMIC_RELAXED); }
-static inline void st_relaxed_u64(uint64_t* p, uint64_t v) { __atomic_store_n(p, v, __ATOMIC_RELAXED); }
-static inline void st_relaxed_u32(uint32_t* p, uint32_t v) { __atomic_store_n(p, v, __ATOMIC_RELAXED); }
-static inline uint4 ld_volatile_v4(const uint4* p) {
-  const uint32_t* w = reinterpret_cast<const uint32_t*>(p);
-  return uint4{__atomic_load_n(w, __ATOMIC_RELAXED), __atomic_load_n(w + 1, __ATOMIC_RELAXED),
-               __atomic_load_n(w + 2, __ATOMIC_RELAXED), __atomic_load_n(w + 3, __ATOMIC_RELAXED)};
-}
 template <class T>
 static inline T __ldg(const T* p) { return *p; }
 static inline int __popc(uint32_t v) { return __builtin_popcount(v); }
@@ -122,8 +112,8 @@ static inline void __syncwarp() {
 }
 // every lane publishes, everybody reads, everybody leaves: two rendezvous per collective
 static inline uint64_t emu_exchange(uint64_t mine, uint32_t src_lane) {
-  uint64_t* slot = &emu_block->xchg[warp_id() * 32];
-  slot[lane_id()] = mine;
+  uint64_t* slot = &emu_block->xchg[emu_warp() * 32];
+  slot[emu_lane()] = mine;
   __syncwarp();
   uint64_t got = slot[src_lane & 31u];
   __syncwarp();
@@ -131,13 +121,13 @@ static inline uint64_t emu_exchange(uint64_t mine, uint32_t src_lane) {
 }
 static inline uint32_t __shfl_sync(uint32_t, uint32_t v, uint32_t src) { return (uint32_t)emu_exchange(v, src); }
 static inline uint32_t __shfl_up_sync(uint32_t, uint32_t v, uint32_t d) {
-  uint32_t l = lane_id();
+  uint32_t l = emu_lane();
   return (uint32_t)emu_exchange(v, l >= d ? l - d : l);
 }
-static inline uint32_t __shfl_xor_sync(uint32_t, uint32_t v, uint32_t m) { return (uint32_t)emu_exchange(v, lane_id() ^ m); }
+static inline uint32_t __shfl_xor_sync(uint32_t, uint32_t v, uint32_t m) { return (uint32_t)emu_exchange(v, emu_lane() ^ m); }
 static inline uint32_t __ballot_sync(uint32_t, bool p) {
-  uint64_t* slot = &emu_block->xchg[warp_id() * 32];
-  slot[lane_id()] = p ? 1 : 0;
+  uint64_t* slot = &emu_block->xchg[emu_warp() * 32];
+  slot[emu_lane()] = p ? 1 : 0;
   __syncwarp();
   uint32_t m = 0;
   for (uint32_t l = 0; l < 32; l++) m |= (uint32_t)(slot[l] & 1) << l;
@@ -146,54 +136,34 @@ static inline uint32_t __ballot_sync(uint32_t, bool p) {
 }
 static inline bool __any_sync(uint32_t mask, bool p) { return __ballot_sync(mask, p) != 0; }
 static inline uint32_t __match_any_sync(uint32_t, uint32_t v) {
-  uint64_t* slot = &emu_block->xchg[warp_id() * 32];
-  slot[lane_id()] = v;
+  uint64_t* slot = &emu_block->xchg[emu_warp() * 32];
+  slot[emu_lane()] = v;
   __syncwarp();
   uint32_t m = 0;
   for (uint32_t l = 0; l < 32; l++) m |= (uint32_t)(slot[l] == v) << l;
   __syncwarp();
   return m;
 }
-static inline uint32_t lanemask_lt() { return (1u << lane_id()) - 1u; }
 
-// mbarrier + TMA 1-D bulk copy (kvg_common.cuh) as used by the 4-stage text ring of k_pciids_parse: the
-// copy completes at issue time, the barrier word counts completed phases, a wait on parity p returns once
-// phase p has completed — the same observable protocol, minus the asynchrony
-// (barrier word here: low half = completed phases, high half = bytes still expected by the current phase;
-// one arriving thread per phase, which is how every kernel of this library uses its barriers)
-static inline void mbar_init(uint64_t* bar, uint32_t) { *bar = 0; }
-static inline void mbar_fence_init() {}
-static inline void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes) { *bar += (uint64_t)bytes << 32; }
-static inline void tma_load_1d(void* smem_dst, const void* gmem_src, uint32_t bytes, uint64_t* bar) {
-  memcpy(smem_dst, gmem_src, bytes);
-  assert((*bar >> 32) >= bytes && "bulk copy without a matching expect_tx");
-  *bar -= (uint64_t)bytes << 32;
-  if ((*bar >> 32) == 0) (*bar)++;  // the phase's last byte has landed
-  emu_block->progressed = true;
-}
-static inline void mbar_wait(uint64_t* bar, uint32_t parity) {
-  while (((*bar) & 1u) == parity) emu_yield();
-}
-
-// the reductions of kvg_common.cuh, on top of the emulated shuffles
-static inline uint32_t warp_sum(uint32_t v) {
-  for (uint32_t o = 16; o; o >>= 1) v += __shfl_xor_sync(KVG_FULL, v, o);
+// full-warp reductions (REDUX on the GPU), on top of the emulated shuffles
+static inline uint32_t __reduce_add_sync(uint32_t, uint32_t v) {
+  for (uint32_t o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
   return v;
 }
-static inline uint32_t warp_min(uint32_t v) {
-  for (uint32_t o = 16; o; o >>= 1) v = min(v, __shfl_xor_sync(KVG_FULL, v, o));
+static inline uint32_t __reduce_min_sync(uint32_t, uint32_t v) {
+  for (uint32_t o = 16; o; o >>= 1) v = min(v, __shfl_xor_sync(0xffffffffu, v, o));
   return v;
 }
-static inline uint32_t warp_max(uint32_t v) {
-  for (uint32_t o = 16; o; o >>= 1) v = max(v, __shfl_xor_sync(KVG_FULL, v, o));
+static inline uint32_t __reduce_max_sync(uint32_t, uint32_t v) {
+  for (uint32_t o = 16; o; o >>= 1) v = max(v, __shfl_xor_sync(0xffffffffu, v, o));
   return v;
 }
-static inline uint32_t warp_incl_max(uint32_t v) {
-  for (uint32_t o = 1; o < 32; o <<= 1) {
-    uint32_t t = __shfl_up_sync(KVG_FULL, v, o);
-    if (lane_id() >= o) v = max(v, t);
-  }
-  return v;
+// byte n of the result is byte (s >> 4n) & 7 of the eight bytes {y:x}
+static inline uint32_t __byte_perm(uint32_t x, uint32_t y, uint32_t s) {
+  const uint64_t v = ((uint64_t)y << 32) | x;
+  uint32_t r = 0;
+  for (int n = 0; n < 4; n++) r |= (uint32_t)((v >> (8 * ((s >> (4 * n)) & 7u))) & 0xffu) << (8 * n);
+  return r;
 }
 
 static inline uint32_t atomicAdd(uint32_t* p, uint32_t v) { return __atomic_fetch_add(p, v, __ATOMIC_SEQ_CST); }
@@ -219,6 +189,40 @@ static inline unsigned long long atomicMin(unsigned long long* p, unsigned long 
   while (v < old && !__atomic_compare_exchange_n(p, &old, v, false, __ATOMIC_SEQ_CST, __ATOMIC_SEQ_CST)) {
   }
   return old;
+}
+
+// ---- the hardware layer: what kvg_common.cuh defines in inline PTX under #ifndef KVG_HOST_EMU ----------
+static inline uint32_t lanemask_lt() { return (1u << emu_lane()) - 1u; }
+static inline void pdl_enter() {}
+static inline uint4 ld_stream(const uint4* p) { return *p; }
+static inline void st_stream(uint4* p, const uint4& v) { *p = v; }
+static inline uint64_t ld_relaxed_u64(const uint64_t* p) { return __atomic_load_n(p, __ATOMIC_RELAXED); }
+static inline void st_relaxed_u64(uint64_t* p, uint64_t v) { __atomic_store_n(p, v, __ATOMIC_RELAXED); }
+static inline void st_relaxed_u32(uint32_t* p, uint32_t v) { __atomic_store_n(p, v, __ATOMIC_RELAXED); }
+static inline uint4 ld_volatile_v4(const uint4* p) {
+  const uint32_t* w = reinterpret_cast<const uint32_t*>(p);
+  return uint4{__atomic_load_n(w, __ATOMIC_RELAXED), __atomic_load_n(w + 1, __ATOMIC_RELAXED),
+               __atomic_load_n(w + 2, __ATOMIC_RELAXED), __atomic_load_n(w + 3, __ATOMIC_RELAXED)};
+}
+
+// mbarrier + TMA 1-D bulk copy as used by the per-warp text ring of k_pciids_scan and the span re-reads of
+// k_pciids_resolve_finalize (kvg_parse_k1.cuh): the copy completes at issue time, the barrier word counts
+// completed phases, a wait on parity p returns once phase p has completed — the same observable protocol,
+// minus the asynchrony
+// (barrier word here: low half = completed phases, high half = bytes still expected by the current phase;
+// one arriving thread per phase, which is how every kernel of this library uses its barriers)
+static inline void mbar_init(uint64_t* bar, uint32_t) { *bar = 0; }
+static inline void mbar_fence_init() {}
+static inline void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes) { *bar += (uint64_t)bytes << 32; }
+static inline void tma_load_1d(void* smem_dst, const void* gmem_src, uint32_t bytes, uint64_t* bar) {
+  memcpy(smem_dst, gmem_src, bytes);
+  assert((*bar >> 32) >= bytes && "bulk copy without a matching expect_tx");
+  *bar -= (uint64_t)bytes << 32;
+  if ((*bar >> 32) == 0) (*bar)++;  // the phase's last byte has landed
+  emu_block->progressed = true;
+}
+static inline void mbar_wait(uint64_t* bar, uint32_t parity) {
+  while (((*bar) & 1u) == parity) emu_yield();
 }
 
 // kernel<<<grid, block>>>(args)
