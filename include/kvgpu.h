@@ -15,6 +15,7 @@
  *   kvg_health_rescan                     <- health flips fed to ListAndWatch
  *                                            generic_device_plugin.go:325-342, :611-690
  *   kvg_scan_pci_delta                    <- (no reference equivalent: the reference never re-scans)
+ *   kvg_scan_mdev_delta                   <- (no reference equivalent: createVgpuIDMap runs once)
  *   kvg_comm_*, kvg_scan_pci_sharded      <- (no reference equivalent; BASELINE.json config 4)
  *
  * Plain C: pointers + sizes only, no C++ types, no exceptions cross this boundary.
@@ -239,13 +240,15 @@ typedef struct kvg_health_delta {
   const uint32_t *changed; /* [n_changed] (record index << 1) | now_alive, ascending index */
 } kvg_health_delta;
 
-/* ---- re-scan delta (K7): what changed since the previous kvg_scan_pci_delta ------------------ */
+/* ---- re-scan delta (K7): what changed since the previous kvg_scan_pci_delta / kvg_scan_mdev_delta */
 enum {
   KVG_CH_ADDED = 1u << 0,   /* survives now, did not before                    */
   KVG_CH_REMOVED = 1u << 1, /* survived before, does not now                    */
-  KVG_CH_GROUP = 1u << 2,   /* survives on both sides with another iommu group  */
-  KVG_CH_DEVICE = 1u << 3,  /* ... another device id                            */
-  KVG_CH_NUMA = 1u << 4     /* ... another clamped NUMA node                    */
+  KVG_CH_GROUP = 1u << 2,   /* survives on both sides with another iommu group  (PCI)  */
+  KVG_CH_DEVICE = 1u << 3,  /* ... another device id                            (PCI)  */
+  KVG_CH_NUMA = 1u << 4,    /* ... another clamped NUMA node                    */
+  KVG_CH_TYPE = 1u << 5,    /* ... another sanitised type label                 (mdev) */
+  KVG_CH_PARENT = 1u << 6   /* ... another parent GPU handle                    (mdev) */
 };
 
 typedef struct kvg_pci_change { /* 32 bytes; one per address whose survivor differs */
@@ -271,6 +274,34 @@ typedef struct kvg_pci_delta {
   uint32_t n_grp_gone;
   const uint32_t *grp_gone;  /* groups of the previous result absent now, ascending */
 } kvg_pci_delta;
+
+typedef struct kvg_mdev_change { /* 48 bytes; one per UUID whose survivor differs */
+  uint8_t uuid[16];
+  uint32_t what;                    /* KVG_CH_ADDED / REMOVED / NUMA / TYPE / PARENT */
+  uint32_t prev_parent, now_parent; /* 0 on the absent side */
+  uint16_t prev_type, now_type;     /* canonical ids in the previous / this result's dictionary */
+  uint16_t prev_numa, now_numa;     /* clamped, as in kvg_mdev_surv */
+  uint32_t now_index;  /* index into this result's survivors, or 0xffffffff (removed) */
+  uint32_t prev_index; /* index into the previous delta scan's survivors, or 0xffffffff (added) */
+  uint32_t pad;
+} kvg_mdev_change;
+
+typedef struct kvg_mdev_delta {
+  uint64_t n_prev;    /* survivors of the previous result (0: first call / after reset) */
+  uint64_t n_changes;
+  const kvg_mdev_change *changes; /* [n_changes] ascending UUID (big-endian byte order) */
+  uint32_t n_type_dirty;
+  const uint32_t *type_dirty;     /* indices into res->type_keys, ascending */
+  /* vGpuMap keys of the previous result absent now, as labels, in ascending previous canonical id:
+     label g = type_gone_bytes[type_gone_off[g] .. type_gone_off[g+1]) */
+  uint32_t n_type_gone;
+  const uint32_t *type_gone_off;  /* [n_type_gone + 1] */
+  const uint8_t *type_gone_bytes;
+  uint32_t n_par_dirty;
+  const uint32_t *par_dirty;      /* indices into res->par_keys, ascending */
+  uint32_t n_par_gone;
+  const uint32_t *par_gone;       /* parent handles of the previous result absent now, ascending */
+} kvg_mdev_delta;
 
 /* ---- context -------------------------------------------------------------------------------- */
 typedef struct kvg_ctx kvg_ctx;
@@ -353,6 +384,42 @@ int kvg_scan_pci_delta(kvg_ctx *ctx, const kvg_pci_rec *recs, size_t n, kvg_pci_
                        kvg_pci_delta **delta);
 /* forget the previous result: the next kvg_scan_pci_delta reports everything as added */
 int kvg_scan_pci_delta_reset(kvg_ctx *ctx);
+
+/* Scan mdev `recs` with dictionary `types` and diff the result against the previous one, keyed by survivor UUID.
+ *
+ * *res is byte for byte what kvg_scan_mdev(ctx, recs, n, types, ...) returns for the same input, dictionary arrays
+ * included.  *res and *delta are both freed with kvg_result_free.
+ *
+ * "Previous" is the result of the last SUCCESSFUL kvg_scan_mdev_delta on this context since kvg_ctx_create or
+ * kvg_scan_mdev_delta_reset; before any such call it is empty, so every survivor is KVG_CH_ADDED, every key is dirty
+ * and nothing is gone.  The library keeps its own copy of it, survivors, keys and type labels, separate from the PCI
+ * delta's: kvg_scan_mdev, kvg_scan_pci, kvg_scan_pci_delta (and its reset), the kvg_dev_scan_* calls, the health
+ * calls, the sharded scans and kvg_pciids_load in between leave it unchanged, and this call leaves the PCI delta's
+ * previous result unchanged.
+ *
+ * Type identity across the two scans is the sanitised label, not the canonical id: each result numbers its own
+ * dictionary (first appearance in the Walk), so one new raw name can renumber every later one, and raw names that
+ * sanitise to one label are one key.
+ *
+ * changes: a UUID has an entry iff it survives on exactly one side, or on both with a different label
+ * (KVG_CH_TYPE), parent handle (KVG_CH_PARENT) or clamped NUMA node (KVG_CH_NUMA).  `src` and the resource-name join
+ * are not compared.  type_dirty: vGpuMap key (label) k is dirty iff the sequence of (uuid, numa) of its members, in
+ * Walk order, differs between the two results; keys that are new are dirty.  par_dirty: gpuVgpuMap key k is dirty
+ * iff its uuid sequence differs (its members carry no NUMA node, device_plugin.go:287-288).  So a NUMA-only change
+ * dirties a vGpuMap key and no gpuVgpuMap key, and a parent-only change gpuVgpuMap keys only.  type_gone (labels) /
+ * par_gone: keys present before and absent now; a label still in the dictionary without a survivor is gone.
+ *
+ * Precondition: survivor UUIDs ascend strictly (big-endian byte order), and a parent handle means the same GPU in
+ * both snapshots.  Canonical UUID names and packed-BDF parents satisfy both.  Strict ascent is checked on the device:
+ * if it fails the call returns KVG_EINVAL (text in kvg_last_error), hands out no objects, and the previous result
+ * stays as it was; so does every error of the scan itself, e.g. KVG_ERANGE for more than 65,535 types.  Index-mode
+ * UUIDs (Walk indices) and interned parents are accepted, but the delta is then relative to the handles only.
+ *
+ * Cost beyond kvg_scan_mdev on the same input: three kernel launches and one synchronisation. */
+int kvg_scan_mdev_delta(kvg_ctx *ctx, const kvg_mdev_rec *recs, size_t n, const kvg_type_dict *types,
+                        kvg_mdev_result **res, kvg_mdev_delta **delta);
+/* forget the previous result: the next kvg_scan_mdev_delta reports everything as added */
+int kvg_scan_mdev_delta_reset(kvg_ctx *ctx);
 
 /* ---- device-resident entry points (inputs already in HBM; used by bench.py "value") -------- */
 

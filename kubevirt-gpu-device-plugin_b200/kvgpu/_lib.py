@@ -35,10 +35,14 @@ MDEV_SURV = np.dtype([("uuid", "u1", (16,)), ("parent", "<u4"), ("type_key", "<u
 PCI_CHANGE = np.dtype([("addr", "<u4"), ("what", "<u4"), ("prev_group", "<u4"), ("now_group", "<u4"),
                        ("prev_device", "<u2"), ("now_device", "<u2"), ("prev_numa", "<u2"), ("now_numa", "<u2"),
                        ("now_index", "<u4"), ("prev_index", "<u4")])
+MDEV_CHANGE = np.dtype([("uuid", "u1", (16,)), ("what", "<u4"), ("prev_parent", "<u4"), ("now_parent", "<u4"),
+                        ("prev_type", "<u2"), ("now_type", "<u2"), ("prev_numa", "<u2"), ("now_numa", "<u2"),
+                        ("now_index", "<u4"), ("prev_index", "<u4"), ("pad", "<u4")])
 CH_ADDED, CH_REMOVED, CH_GROUP, CH_DEVICE, CH_NUMA = 1, 2, 4, 8, 16
+CH_TYPE, CH_PARENT = 32, 64
 NO_INDEX = 0xFFFFFFFF
 assert PCI_REC.itemsize == 16 and PCI_SURV.itemsize == 16 and PCI_CHANGE.itemsize == 32
-assert MDEV_REC.itemsize == 32 and MDEV_SURV.itemsize == 32
+assert MDEV_REC.itemsize == 32 and MDEV_SURV.itemsize == 32 and MDEV_CHANGE.itemsize == 48
 
 
 class KvgError(RuntimeError):
@@ -111,6 +115,14 @@ class PciDeltaC(C.Structure):
                 ("n_grp_gone", C.c_uint32), ("grp_gone", C.c_void_p)]
 
 
+class MdevDeltaC(C.Structure):
+    _fields_ = [("n_prev", C.c_uint64), ("n_changes", C.c_uint64), ("changes", C.c_void_p),
+                ("n_type_dirty", C.c_uint32), ("type_dirty", C.c_void_p),
+                ("n_type_gone", C.c_uint32), ("type_gone_off", C.c_void_p), ("type_gone_bytes", C.c_void_p),
+                ("n_par_dirty", C.c_uint32), ("par_dirty", C.c_void_p),
+                ("n_par_gone", C.c_uint32), ("par_gone", C.c_void_p)]
+
+
 def declared_symbols() -> list[str]:
     """Every function name include/kvgpu.h declares (used by the export test)."""
     src = open(HEADER_PATH).read()
@@ -150,6 +162,8 @@ def load() -> C.CDLL:
         "kvg_health_reset": (C.c_int, [vp]),
         "kvg_scan_pci_delta": (C.c_int, [vp, vp, sz, P(P(PciResultC)), P(P(PciDeltaC))]),
         "kvg_scan_pci_delta_reset": (C.c_int, [vp]),
+        "kvg_scan_mdev_delta": (C.c_int, [vp, vp, sz, P(TypeDict), P(P(MdevResultC)), P(P(MdevDeltaC))]),
+        "kvg_scan_mdev_delta_reset": (C.c_int, [vp]),
         "kvg_text_pad": (sz, [sz]),
         "kvg_dev_pciids_parse": (C.c_int, [vp, vp, sz, sz, u32]),
         "kvg_dev_scan_pci": (C.c_int, [vp, vp, sz]),

@@ -82,6 +82,17 @@ class PciDelta:
     grp_gone: np.ndarray        # u32 groups absent now, ascending
 
 
+@dataclass
+class MdevDelta:
+    """What changed since the previous scan_mdev_delta (include/kvgpu.h kvg_mdev_delta)."""
+    n_prev: int
+    changes: np.ndarray         # MDEV_CHANGE, ascending UUID
+    type_dirty: np.ndarray      # u32 indices into the result's type_keys, ascending
+    type_gone: list             # labels (bytes) of the vGpuMap keys absent now, ascending previous canonical id
+    par_dirty: np.ndarray       # u32 indices into the result's par_keys, ascending
+    par_gone: np.ndarray        # u32 parent handles absent now, ascending
+
+
 class _LockedLib:
     """A kvg_ctx is single-threaded (include/kvgpu.h).  gRPC handler threads, the health feed and the
     Allocate re-validation all share one Context (kvgpu/serve.py), so every C call on it is serialised."""
@@ -275,6 +286,32 @@ class Context:
 
     def scan_pci_delta_reset(self):
         self._ck(self._lib.kvg_scan_pci_delta_reset(self._h))
+
+    def scan_mdev_delta(self, recs: np.ndarray, raw_types: list):
+        """scan_mdev plus the keyed diff against the previous scan_mdev_delta on this context -> (MdevResult,
+        MdevDelta).  Types are compared by label.  Meaningful for canonical UUIDs and packed-BDF parents; with
+        index-mode handles it is relative to the handles."""
+        recs = np.ascontiguousarray(recs, dtype=L.MDEV_REC)
+        td, keep = self._type_dict(raw_types)
+        res = C.POINTER(L.MdevResultC)()
+        dl = C.POINTER(L.MdevDeltaC)()
+        self._ck(self._lib.kvg_scan_mdev_delta(self._h, recs.ctypes.data, len(recs), C.byref(td), C.byref(res),
+                                               C.byref(dl)))
+        del keep
+        d = dl.contents
+        ng = int(d.n_type_gone)
+        goff = L._arr(d.type_gone_off, ng + 1, np.uint32)
+        gbytes = C.string_at(d.type_gone_bytes, int(goff[-1])) if ng and goff[-1] else b""
+        delta = MdevDelta(int(d.n_prev), L._arr(d.changes, int(d.n_changes), L.MDEV_CHANGE),
+                          L._arr(d.type_dirty, int(d.n_type_dirty), np.uint32),
+                          [gbytes[goff[i]:goff[i + 1]] for i in range(ng)],
+                          L._arr(d.par_dirty, int(d.n_par_dirty), np.uint32),
+                          L._arr(d.par_gone, int(d.n_par_gone), np.uint32))
+        self._lib.kvg_result_free(dl)
+        return self._take_mdev(res), delta
+
+    def scan_mdev_delta_reset(self):
+        self._ck(self._lib.kvg_scan_mdev_delta_reset(self._h))
 
     # -- device-resident entry points (raw device pointers, e.g. torch tensor.data_ptr()) ----
     def text_pad(self, n: int) -> int:

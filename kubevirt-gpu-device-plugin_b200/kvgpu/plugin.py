@@ -459,6 +459,71 @@ def mdev_maps_from_result(res: MdevResult, snap: MdevSnapshot | None = None, map
     return m
 
 
+@dataclass
+class MdevMapsTouched:
+    """The vGpuMap / gpuVgpuMap keys apply_mdev_delta rewrote (dirty: present now, new ones included) or removed."""
+    type_dirty: list
+    type_gone: list
+    par_dirty: list
+    par_gone: list
+
+
+def _numeric_mdev(snap: MdevSnapshot | None) -> bool:
+    return snap is None or (snap.uuid_ok and snap.parent_names is None)
+
+
+def _rebuild_mdev_maps(maps: Maps, res: MdevResult, snap) -> MdevMapsTouched:
+    """mdev_maps_from_result into the dicts `maps` already holds (they are shared), reporting every key of the new
+    maps and every key that went."""
+    fresh = mdev_maps_from_result(res, snap)
+    type_gone = sorted(set(maps.vGpuMap) - set(fresh.vGpuMap))
+    par_gone = sorted(set(maps.gpuVgpuMap) - set(fresh.gpuVgpuMap))
+    for label in type_gone:
+        if label not in maps.deviceMap:
+            maps.deviceNames.pop(label, None)
+    maps.vGpuMap.clear()
+    maps.vGpuMap.update(fresh.vGpuMap)
+    maps.gpuVgpuMap.clear()
+    maps.gpuVgpuMap.update(fresh.gpuVgpuMap)
+    maps.deviceNames.update(fresh.deviceNames)
+    return MdevMapsTouched(list(fresh.vGpuMap), type_gone, list(fresh.gpuVgpuMap), par_gone)
+
+
+def apply_mdev_delta(maps: Maps, res: MdevResult, delta, snap: MdevSnapshot | None = None,
+                     prev_snap: MdevSnapshot | None = None) -> MdevMapsTouched:
+    """Patch vGpuMap, gpuVgpuMap and the label entries of deviceNames of `maps` (built from the previous delta scan's
+    result) IN PLACE into what mdev_maps_from_result(res) builds, touching only dirty or gone keys: whoever holds
+    maps.gpuVgpuMap (XidEventRouter) sees the new vGPUs.  A snapshot whose UUIDs are not canonical or whose parents are
+    not packed BDFs has no stable handles: the maps are then rebuilt (in place as well) and every key is reported."""
+    if not (_numeric_mdev(snap) and _numeric_mdev(prev_snap)):
+        return _rebuild_mdev_maps(maps, res, snap)
+    s = res.survivors
+    t = MdevMapsTouched([], [], [], [])
+    for k in delta.type_dirty:
+        c = int(res.type_keys[k])
+        label = res.labels[c].decode("latin-1")
+        idx = res.type_perm[res.type_off[k]:res.type_off[k + 1]]
+        maps.vGpuMap[label] = [NvidiaGpuDevice(format_uuid(s["uuid"][i]), int(s["numa"][i])) for i in idx]
+        maps.deviceNames[label] = res.type_names[c]
+        t.type_dirty.append(label)
+    for g in delta.type_gone:
+        label = g.decode("latin-1")
+        maps.vGpuMap.pop(label, None)
+        if label not in maps.deviceMap:
+            maps.deviceNames.pop(label, None)
+        t.type_gone.append(label)
+    for k in delta.par_dirty:
+        key = format_bdf(int(res.par_keys[k]))
+        idx = res.par_perm[res.par_off[k]:res.par_off[k + 1]]
+        maps.gpuVgpuMap[key] = [format_uuid(s["uuid"][i]) for i in idx]
+        t.par_dirty.append(key)
+    for p in delta.par_gone:
+        key = format_bdf(int(p))
+        maps.gpuVgpuMap.pop(key, None)
+        t.par_gone.append(key)
+    return t
+
+
 def canonical_dump(m: Maps) -> bytes:
     """Byte-identical to oracle kvo_dump for the same maps (SURVEY.md 8c)."""
     out = []
@@ -509,6 +574,7 @@ class DiscoveryScan:
         self.maps = Maps()
         self._loaded_path = None
         self._prev_pci_snap = None   # snapshot of the last rescan_iommu_device_map
+        self._prev_mdev_snap = None  # snapshot of the last rescan_vgpu_id_map
 
     def close(self):
         self.ctx.close()
@@ -550,6 +616,17 @@ class DiscoveryScan:
         snap = snapshot_mdev_tree(self.vGpuBasePath, self.basePath)
         res = self.ctx.scan_mdev(snap.recs, snap.raw_types)
         return mdev_maps_from_result(res, snap, self.maps)
+
+    def rescan_vgpu_id_map(self) -> MdevMapsTouched:
+        """Re-walk the mdev tree and bring vGpuMap / gpuVgpuMap up to date through the re-scan delta.  The first call
+        has no previous delta scan to diff against: it rebuilds the maps and reports every key."""
+        self._ensure_table()
+        snap = snapshot_mdev_tree(self.vGpuBasePath, self.basePath)
+        res, delta = self.ctx.scan_mdev_delta(snap.recs, snap.raw_types)
+        prev, self._prev_mdev_snap = self._prev_mdev_snap, snap
+        if prev is None:
+            return _rebuild_mdev_maps(self.maps, res, snap)
+        return apply_mdev_delta(self.maps, res, delta, snap, prev)
 
     def create_device_plugins(self) -> list:
         return plugin_specs_from_maps(self.maps)

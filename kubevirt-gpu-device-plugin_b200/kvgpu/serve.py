@@ -15,8 +15,8 @@ Allocate" is testable end to end in an image without a Go toolchain.
 
 Nothing here computes on the CPU what the scan computes on the GPU: the maps come from
 plugin.DiscoveryScan (libkvgpu.so); the re-validation's classification goes through
-Context.scan_pci (K3); the health feed through Context.health_rescan (K6); the hot-plug feed through
-Context.scan_pci_delta (K7).
+Context.scan_pci (K3); the health feed through Context.health_rescan (K6); the hot-plug feeds through
+Context.scan_pci_delta and Context.scan_mdev_delta (K7).
 """
 from __future__ import annotations
 
@@ -32,7 +32,8 @@ import numpy as np
 from . import _lib as L
 from . import dpapi
 from .plugin import (DEVICE_NAMESPACE, GPU_PREFIX, VGPU_PREFIX, Maps, PluginSpec, ReferencePanic, _read_id,
-                     _read_link, _read_vgpu_raw, _rebuild_pci_maps, apply_pci_delta, plugin_specs_from_maps)
+                     _read_link, _read_vgpu_raw, _rebuild_mdev_maps, _rebuild_pci_maps, apply_mdev_delta,
+                     apply_pci_delta, plugin_specs_from_maps)
 
 VFIO_DEVICE_PATH = "/dev/vfio"      # generic_device_plugin.go:54
 IOMMU_DEVICE_PATH = "/dev/iommu"    # :55
@@ -253,7 +254,7 @@ class _PluginBase:
         self.kubelet_socket = kubelet_socket or os.path.join(socket_dir, "kubelet.sock")
         self.server = None
         self._events = queue.Queue()     # ("healthy" | "unhealthy", device id): the two Go channels;
-                                         # ("devices", None): the device list changed (PciRescanFeed)
+                                         # ("devices", None): the device list changed (a re-scan feed)
         self._stop = threading.Event()
         self._term = threading.Event()
         self._lock = threading.Lock()
@@ -564,33 +565,21 @@ class HealthRescanFeed:
 
 
 # ------------------------------------------------------------------------------------------------
-# hot-plug feed driven by the K7 re-scan delta
+# hot-plug feeds driven by the K7 re-scan deltas
 # ------------------------------------------------------------------------------------------------
-class PciRescanFeed:
-    """Periodic re-snapshot -> Context.scan_pci_delta (K7) -> the shared maps and the set of passthrough plugins.
+class _RescanFeed:
+    """The loop and the plugin lifecycle both re-scan feeds share; a subclass supplies tick()."""
 
-    `snapshot()` returns a PciSnapshot, `scan_delta(recs)` is Context.scan_pci_delta, `plugins` maps deviceMap keys
-    to running plugins and `make_plugin(spec)` builds one for a new key.  Each tick patches `maps` in place (Allocate
-    reads iommuMap / bdfToIommuMap from it, so it sees a moved device at once), gives every plugin whose key is
-    dirty its new device list, starts and registers a plugin for every new key, and stops the plugin of every key
-    that went.  The first tick has no previous snapshot: it rebuilds the maps and treats every key as dirty."""
-
-    def __init__(self, scan_delta, snapshot, maps: Maps, plugins: dict, make_plugin, period_s: float = 0.01):
+    def __init__(self, scan_delta, snapshot, maps: Maps, plugins: dict, make_plugin, period_s: float):
         self.scan_delta, self.snapshot, self.maps = scan_delta, snapshot, maps
         self.plugins, self.make_plugin, self.period_s = plugins, make_plugin, period_s
         self._prev_snap = None
         self._stop = threading.Event()
         self._thread = None
 
-    def tick(self):
-        snap = self.snapshot()
-        res, delta = self.scan_delta(snap.recs)
-        if self._prev_snap is None:
-            touched = _rebuild_pci_maps(self.maps, res, snap, None)
-        else:
-            touched = apply_pci_delta(self.maps, res, delta, snap, self._prev_snap)
-        self._prev_snap = snap
-        dirty = Maps(deviceMap={k: self.maps.deviceMap[k] for k in touched.dev_dirty}, deviceNames=self.maps.deviceNames)
+    def _follow(self, dirty: Maps, gone: list):
+        """The plugins of the dirty keys (`dirty` holds their maps) get their new device list, or are started and
+        registered when the key is new; the plugins of the keys that went are stopped."""
         for spec in plugin_specs_from_maps(dirty):
             plugin = self.plugins.get(spec.key)
             if plugin is None:
@@ -599,11 +588,10 @@ class PciRescanFeed:
                 self.plugins[spec.key] = plugin
             else:
                 plugin.set_devices(devices_from_spec(spec))
-        for key in touched.dev_gone:
+        for key in gone:
             plugin = self.plugins.pop(key, None)
             if plugin is not None:
                 plugin.stop()
-        return touched
 
     def start(self):
         def loop():
@@ -617,6 +605,57 @@ class PciRescanFeed:
         self._stop.set()
         if self._thread:
             self._thread.join(2.0)
+
+
+class PciRescanFeed(_RescanFeed):
+    """Periodic re-snapshot -> Context.scan_pci_delta (K7) -> the shared maps and the set of passthrough plugins.
+
+    `snapshot()` returns a PciSnapshot, `scan_delta(recs)` is Context.scan_pci_delta, `plugins` maps deviceMap keys
+    to running plugins and `make_plugin(spec)` builds one for a new key.  Each tick patches `maps` in place (Allocate
+    reads iommuMap / bdfToIommuMap from it, so it sees a moved device at once), gives every plugin whose key is
+    dirty its new device list, starts and registers a plugin for every new key, and stops the plugin of every key
+    that went.  The first tick has no previous snapshot: it rebuilds the maps and treats every key as dirty."""
+
+    def __init__(self, scan_delta, snapshot, maps: Maps, plugins: dict, make_plugin, period_s: float = 0.01):
+        super().__init__(scan_delta, snapshot, maps, plugins, make_plugin, period_s)
+
+    def tick(self):
+        snap = self.snapshot()
+        res, delta = self.scan_delta(snap.recs)
+        if self._prev_snap is None:
+            touched = _rebuild_pci_maps(self.maps, res, snap, None)
+        else:
+            touched = apply_pci_delta(self.maps, res, delta, snap, self._prev_snap)
+        self._prev_snap = snap
+        self._follow(Maps(deviceMap={k: self.maps.deviceMap[k] for k in touched.dev_dirty},
+                          deviceNames=self.maps.deviceNames), touched.dev_gone)
+        return touched
+
+
+class MdevRescanFeed(_RescanFeed):
+    """Periodic re-snapshot -> Context.scan_mdev_delta (K7) -> the shared maps and the set of vGPU plugins.
+
+    `snapshot()` returns an MdevSnapshot, `scan_delta(recs, raw_types)` is Context.scan_mdev_delta, `plugins` maps
+    vGpuMap keys (labels) to running plugins and `make_plugin(spec)` builds a GenericVGpuDevicePlugin for a new label.
+    Each tick patches vGpuMap / gpuVgpuMap of `maps` in place (an XidEventRouter holding maps.gpuVgpuMap sees a new
+    vGPU at once), re-sends the device list of every plugin whose label is dirty (a NUMA move re-sends topology),
+    starts and registers a plugin for every new label, and stops the plugin of every label that went.  The first
+    tick has no previous snapshot: it rebuilds the maps and treats every key as dirty."""
+
+    def __init__(self, scan_delta, snapshot, maps: Maps, plugins: dict, make_plugin, period_s: float = 0.01):
+        super().__init__(scan_delta, snapshot, maps, plugins, make_plugin, period_s)
+
+    def tick(self):
+        snap = self.snapshot()
+        res, delta = self.scan_delta(snap.recs, snap.raw_types)
+        if self._prev_snap is None:
+            touched = _rebuild_mdev_maps(self.maps, res, snap)
+        else:
+            touched = apply_mdev_delta(self.maps, res, delta, snap, self._prev_snap)
+        self._prev_snap = snap
+        self._follow(Maps(vGpuMap={k: self.maps.vGpuMap[k] for k in touched.type_dirty},
+                          deviceNames=self.maps.deviceNames), touched.type_gone)
+        return touched
 
 
 # ------------------------------------------------------------------------------------------------
