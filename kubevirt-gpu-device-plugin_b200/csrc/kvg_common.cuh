@@ -5,6 +5,7 @@
 //   * warp / block scans
 //   * epoch-tagged decoupled look-back (single-pass chained scan) used by the stable compactions
 //     and by the vendor-context carry of the pci.ids parser
+//   * the tile front-end of every compaction (ClassifyTile) and its look-back tile body (lookback_tile)
 #pragma once
 #include <stdint.h>
 
@@ -167,12 +168,9 @@ __device__ __forceinline__ uint32_t lb_status(uint64_t w, uint32_t epoch) {
   return ((uint32_t)(w >> 34) == (epoch & 0x3fffffffu)) ? (uint32_t)((w >> 32) & 3) : LB_INVALID;
 }
 
-// Sum look-back, executed by one full warp.  Publishes this tile's aggregate, walks predecessors
-// and returns the exclusive prefix (valid in every lane); publishes the inclusive.
-// The walk reads LB_WIDE*32 predecessor states per step with INDEPENDENT loads: with ~1000 tiles
-// in flight the nearest inclusive prefix is typically hundreds of tiles back, and a 32-wide
-// window would turn that into a chain of ~15 dependent L2 round trips per tile.
-constexpr int LB_WIDE = 1;  // measured: 8-wide windows were slower (more polling traffic), 1 = classic
+// Sum look-back, executed by one full warp.  Publishes this tile's aggregate, walks the predecessors 32 at a time
+// (one state word per lane) and returns the exclusive prefix (valid in every lane); publishes the inclusive.
+// (Measured: windows of 8 x 32 predecessors per step, all loads independent, were slower — more polling traffic.)
 __device__ __forceinline__ uint32_t lookback_sum(uint64_t* state, uint32_t tile, uint32_t aggregate,
                                                  uint32_t epoch) {
   const uint32_t lane = lane_id();
@@ -182,34 +180,114 @@ __device__ __forceinline__ uint32_t lookback_sum(uint64_t* state, uint32_t tile,
   }
   if (lane == 0) st_relaxed_u64(&state[tile], lb_pack(epoch, LB_AGGREGATE, aggregate));
   uint32_t excl = 0;
-  int look = (int)tile - 1;
-  for (;;) {
-    uint64_t w[LB_WIDE];
-#pragma unroll
-    for (int k = 0; k < LB_WIDE; k++) {
-      int idx = look - (int)lane - 32 * k;
-      w[k] = idx >= 0 ? ld_relaxed_u64(&state[idx]) : lb_pack(epoch, LB_INCLUSIVE, 0);
-    }
-    bool done = false;
-#pragma unroll
-    for (int k = 0; k < LB_WIDE; k++) {
-      uint32_t st = lb_status(w[k], epoch);
-      uint32_t incl_mask = __ballot_sync(KVG_FULL, st == LB_INCLUSIVE);
-      uint32_t inv_mask = __ballot_sync(KVG_FULL, st == LB_INVALID);
-      uint32_t first = incl_mask ? (uint32_t)__ffs(incl_mask) - 1 : 32;
-      uint32_t need = first >= 31 ? KVG_FULL : ((2u << first) - 1);  // lanes 0..first
-      if (inv_mask & need) break;  // a needed predecessor is not published yet: reload from here
-      excl += warp_sum(lane <= first ? (uint32_t)w[k] : 0u);
-      if (first < 32) {
-        done = true;
-        break;
-      }
-      look -= 32;
-    }
-    if (done) break;
+  for (int look = (int)tile - 1;;) {
+    const int idx = look - (int)lane;
+    const uint64_t w = idx >= 0 ? ld_relaxed_u64(&state[idx]) : lb_pack(epoch, LB_INCLUSIVE, 0);
+    const uint32_t st = lb_status(w, epoch);
+    const uint32_t incl_mask = __ballot_sync(KVG_FULL, st == LB_INCLUSIVE);
+    const uint32_t inv_mask = __ballot_sync(KVG_FULL, st == LB_INVALID);
+    const uint32_t first = incl_mask ? (uint32_t)__ffs(incl_mask) - 1 : 32;
+    const uint32_t need = first >= 31 ? KVG_FULL : ((2u << first) - 1);  // lanes 0..first
+    if (inv_mask & need) continue;  // a needed predecessor is not published yet: reload the same window
+    excl += warp_sum(lane <= first ? (uint32_t)w : 0u);
+    if (first < 32) break;
+    look -= 32;
   }
   if (lane == 0) st_relaxed_u64(&state[tile], lb_pack(epoch, LB_INCLUSIVE, excl + aggregate));
   return excl;
+}
+
+// ------------------------------------------------------------------------------------------------
+// The tile front-end of every compaction (classify, health, the ordering heads, the delta lists).  A warp owns 32 x ROWS consecutive records of the tile
+// (THREADS x ROWS records); `classify` issues every load before the first ballot, votes Op::pred per row and
+// calls Op::prepare for the survivors, whose dependent loads then overlap what the kernel does next.  `emit`
+// hands each of the lane's survivors to f(pos, item, i, aux), numbered in record order from the warp's offset.
+//   Op::Item                          what a thread holds per record
+//   uint32_t n                        number of records
+//   Item load(uint32_t i, bool ok)    ok == false -> any value that fails pred
+//   bool pred(const Item&, i)
+//   uint32_t prepare(const Item&)     per-survivor value handed to emit (name slot, canonical type)
+// ------------------------------------------------------------------------------------------------
+template <class Op, int THREADS, int ROWS>
+struct ClassifyTile {
+  static constexpr uint32_t TILE = THREADS * ROWS;
+  static constexpr uint32_t NW = THREADS / 32;
+  static constexpr uint32_t WARP_ITEMS = 32 * ROWS;
+  typename Op::Item item[ROWS];
+  uint32_t bal[ROWS], aux[ROWS];
+  uint32_t base;  // the warp's first record
+  uint32_t wtot;  // the warp's survivors
+
+  __device__ __forceinline__ void classify(Op& op, uint32_t tile) {
+    const uint32_t lane = lane_id(), n = op.n;
+    base = tile * TILE + (threadIdx.x >> 5) * WARP_ITEMS;
+#pragma unroll
+    for (int k = 0; k < ROWS; k++) {
+      const uint32_t i = base + k * 32 + lane;
+      item[k] = op.load(i, i < n);
+    }
+    wtot = 0;
+#pragma unroll
+    for (int k = 0; k < ROWS; k++) {
+      const uint32_t i = base + k * 32 + lane;
+      const bool p = i < n && op.pred(item[k], i);
+      bal[k] = __ballot_sync(KVG_FULL, p);
+      wtot += __popc(bal[k]);
+      aux[k] = p ? op.prepare(item[k]) : 0u;
+    }
+  }
+  template <class F>
+  __device__ __forceinline__ void emit(uint32_t off, F&& f) const {
+    const uint32_t lane = lane_id();
+#pragma unroll
+    for (int k = 0; k < ROWS; k++) {
+      if ((bal[k] >> lane) & 1u) f(off + __popc(bal[k] & lanemask_lt()), item[k], base + k * 32 + lane, aux[k]);
+      off += __popc(bal[k]);
+    }
+  }
+};
+
+// One tile of the look-back compaction: classify it, place it behind all earlier tiles (decoupled look-back on
+// the tile counts), write its survivors.  Besides the front-end, Op provides emit(pos, item, i, aux),
+// tile_epilogue() (once per warp after its survivors) and finish(total) (one thread of the last tile).
+// s_wtot / s_woff: a word per warp of shared memory.
+template <class Op, int THREADS, int ROWS>
+__device__ __forceinline__ void lookback_tile(Op& op, uint32_t tile, uint32_t n_tiles, uint64_t* tile_state, uint32_t epoch,
+                                              uint32_t* s_wtot, uint32_t* s_woff, uint32_t& s_base) {
+  constexpr uint32_t NW = THREADS / 32;
+  const uint32_t lane = lane_id(), warp = threadIdx.x >> 5;
+  ClassifyTile<Op, THREADS, ROWS> ct;
+  ct.classify(op, tile);
+  if (lane == 0) s_wtot[warp] = ct.wtot;
+  __syncthreads();
+  if (warp == 0) {
+    uint32_t w = lane < NW ? s_wtot[lane] : 0;
+    uint32_t wi = warp_incl_sum(w);
+    if (lane < NW) s_woff[lane] = wi - w;
+    uint32_t tile_total = __shfl_sync(KVG_FULL, wi, NW - 1);
+    uint32_t excl = lookback_sum(tile_state, tile, tile_total, epoch);
+    if (lane == 0) {
+      s_base = excl;
+      if (tile == n_tiles - 1) op.finish(excl + tile_total);
+    }
+  }
+  __syncthreads();
+  ct.emit(s_base + s_woff[warp], [&](uint32_t pos, const typename Op::Item& r, uint32_t i, uint32_t a) { op.emit(pos, r, i, a); });
+  op.tile_epilogue();
+}
+
+// The whole look-back compaction of op.n records: tiles blockIdx.x, blockIdx.x + gridDim.x, ... (a grid of one CTA
+// per tile runs the loop once; a smaller grid must be co-resident, since a tile waits for every lower one).  An empty
+// list still finishes, with total 0.
+template <class Op, int THREADS, int ROWS>
+__device__ __forceinline__ void lookback_tiles(Op& op, uint64_t* tile_state, uint32_t epoch) {
+  constexpr uint32_t TILE = THREADS * ROWS;
+  __shared__ uint32_t s_wtot[THREADS / 32], s_woff[THREADS / 32];
+  __shared__ uint32_t s_base;
+  const uint32_t n_tiles = (op.n + TILE - 1) / TILE;
+  if (n_tiles == 0 && blockIdx.x == 0 && threadIdx.x == 0) op.finish(0);
+  for (uint32_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x)
+    lookback_tile<Op, THREADS, ROWS>(op, tile, n_tiles, tile_state, epoch, s_wtot, s_woff, s_base);
 }
 
 }  // namespace kvg

@@ -2,7 +2,7 @@
 //
 //   k_delta_merge<Tr>  merge path over the previous scan's survivors and the new ones (ascending key), one change
 //                      entry per key whose survivor differs, compacted in key order by the look-back tile body of
-//                      kvg_scan.cuh; every entry tags the keys of the two group-by maps whose member sequence it
+//                      kvg_common.cuh; every entry tags the keys of the two group-by maps whose member sequence it
 //                      changes.  Also checks that the new list ascends strictly.  Tr is the record trait:
 //                      PciDeltaRec (16-byte survivors keyed by address) or MdevDeltaRec (32-byte survivors keyed by
 //                      the 128-bit big-endian UUID).
@@ -329,7 +329,9 @@ struct DeltaListOp {
 struct DeltaListArgs {
   DeltaListOp o[4];  // dirty, gone of the first map (deviceMap / vGpuMap), then of the second
 };
-// grid (tiles of the longest list, 4); list y uses the look-back words tile_state[y * state_stride ..)
+// grid (tiles of the longest list, 4); list y uses the look-back words tile_state[y * state_stride ..).  One CTA per
+// tile, no tile loop: the loop of lookback_tiles measured 2 % slower here (10.35 against 10.1 us at 1 M records,
+// H100 SXM 80 GB with a 700 W power limit).
 __global__ void __launch_bounds__(KVG_BLOCK) k_delta_lists(DeltaListArgs args, uint64_t* tile_state, uint32_t state_stride,
                                                            uint32_t epoch) {
   pdl_enter();

@@ -486,21 +486,24 @@ __device__ __forceinline__ const uint2* ord_final_buf(const OrdFinalArgs& a) {
   const uint32_t np = radix_plan(*a.max_key, a.key_bits_max, 0, a.max_bits).npass;
   return ((np - 1) & 1) ? a.p1 : a.p0;
 }
-// one tile: load, write the permutation (unless `emit_only`), head ballots.  Returns the warp's head count.
-__device__ __forceinline__ uint32_t ord_tile_heads(const OrdFinalArgs& a, const uint2* pairs, uint32_t n,
-                                                   uint32_t base, uint32_t lane, bool write_perm,
-                                                   uint32_t (&bal)[C_ROWS], uint32_t (&key)[C_ROWS],
-                                                   uint32_t (&idx)[C_ROWS]) {
-  uint32_t wtot = 0;
-#pragma unroll
-  for (uint32_t k = 0; k < C_ROWS; k++) {
-    const uint32_t i = base + k * 32 + lane;
-    key[k] = idx[k] = 0;
-    uint32_t edge = 0;  // key of element i-1 when it lives in another row / tile (lane 0 only)
-    if (i < n) {
+// The segment heads of the sorted pairs as a ClassifyTile operator: element i is a head iff i == 0 or its key differs
+// from element i - 1's.  The previous key comes from the lane below, or for lane 0 (its predecessor lives in another
+// row or tile) from memory; it is taken in load, which every lane runs, so the shuffle is convergent.
+struct OrdHeadsOp {
+  struct Item {
+    uint32_t key, idx, prev;
+  };
+  OrdFinalArgs a;
+  const uint2* pairs;  // the sorted pairs (the final radix buffer)
+  uint32_t n;
+  bool write_perm;     // the launch that owns the permutation (and the deferred name join)
+
+  __device__ __forceinline__ Item load(uint32_t i, bool ok) const {
+    Item it = {0u, 0u, 0u};
+    if (ok) {
       const uint2 e = pairs[i];
-      key[k] = e.x;
-      idx[k] = e.y;
+      it.key = e.x;
+      it.idx = e.y;
       if (write_perm) {
         a.perm[i] = e.y;
         if (a.join == 1)
@@ -509,80 +512,45 @@ __device__ __forceinline__ uint32_t ord_tile_heads(const OrdFinalArgs& a, const 
           reinterpret_cast<uint32_t*>(a.join_recs + e.y)[3] =
               __ldg(&a.join_index[reinterpret_cast<const uint32_t*>(a.join_recs + e.y)[2] & 0xffffu]);
       }
-      if (lane == 0 && i) edge = pairs[i - 1].x;
     }
-    const uint32_t below = __shfl_up_sync(KVG_FULL, key[k], 1);
-    const bool head = i < n && (i == 0 || (lane ? below : edge) != key[k]);
-    bal[k] = __ballot_sync(KVG_FULL, head);
-    wtot += __popc(bal[k]);
+    it.prev = __shfl_up_sync(KVG_FULL, it.key, 1);
+    if (ok && lane_id() == 0 && i) it.prev = pairs[i - 1].x;  // overwrites the shuffled value: one register per row
+    return it;
   }
-  return wtot;
-}
-__device__ __forceinline__ void ord_emit_heads(const OrdFinalArgs& a, uint32_t off, uint32_t base, uint32_t lane,
-                                               const uint32_t (&bal)[C_ROWS], const uint32_t (&key)[C_ROWS],
-                                               const uint32_t (&idx)[C_ROWS]) {
-#pragma unroll
-  for (uint32_t k = 0; k < C_ROWS; k++) {
-    const uint32_t i = base + k * 32 + lane;
-    if ((bal[k] >> lane) & 1u) {
-      const uint32_t pos = off + __popc(bal[k] & lanemask_lt());
-      a.seg_key[pos] = key[k];
-      a.seg_off[pos] = i;
-      // all members of a device-id bucket share the name (same id): take the first member's slot
-      if (a.head_name)  // deferred join: straight from the table (the record's slot may be written by another thread)
-        a.head_name[pos] = a.join ? __ldg(&a.join_index[key[k] & 0xffffu]) : __ldg(&a.head_surv[idx[k]].w);
-    }
-    off += __popc(bal[k]);
+  __device__ __forceinline__ bool pred(const Item& it, uint32_t i) const { return i == 0 || it.prev != it.key; }
+  __device__ __forceinline__ uint32_t prepare(const Item&) const { return 0; }
+  __device__ __forceinline__ void emit(uint32_t pos, const Item& it, uint32_t i, uint32_t) const {
+    a.seg_key[pos] = it.key;
+    a.seg_off[pos] = i;
+    // all members of a device-id bucket share the name (same id): take the first member's slot
+    if (a.head_name)  // deferred join: straight from the table (the record's slot may be written by another thread)
+      a.head_name[pos] = a.join ? __ldg(&a.join_index[it.key & 0xffffu]) : __ldg(&a.head_surv[it.idx].w);
   }
+  __device__ __forceinline__ void tile_epilogue() {}
+  __device__ __forceinline__ void finish(uint32_t total) const {
+    *a.n_seg = total;
+    a.seg_off[total] = n;
+  }
+};
+// the operator of ordering blockIdx.y
+__device__ __forceinline__ OrdHeadsOp ord_heads_op(const OrdFinalArgs2& aa, bool write_perm) {
+  OrdHeadsOp op;
+  op.a = blockIdx.y ? aa.o[1] : aa.o[0];  // static indices: parameters stay in the constant bank
+  op.n = *op.a.n_ptr;
+  op.pairs = ord_final_buf(op.a);
+  op.write_perm = write_perm;
+  return op;
 }
 
 // latency-bound sizes: one launch; the per-tile head counts are combined by a chained scan (look-back).
 // Tile loop: the grid may be smaller than the tile count (the sharded scan sizes it for the EXPECTED length of
 // an owned list, not for its capacity) — it must then fit the GPU at once (a CTA waits for lower tiles, which
-// must be running or done: enqueue_orderings bounds the grid by the occupancy).
-__global__ void __launch_bounds__(KVG_BLOCK) k_order_final(OrdFinalArgs2 aa, uint32_t epoch) {
+// must be running or done: enqueue_orderings bounds the grid by the occupancy).  6 CTAs per SM: 40 registers, which
+// ptxas meets without spilling (left to itself it takes 48, i.e. 5 CTAs per SM and a smaller grid).
+__global__ void __launch_bounds__(KVG_BLOCK, 6) k_order_final(OrdFinalArgs2 aa, uint32_t epoch) {
   pdl_enter();
-  const OrdFinalArgs a = blockIdx.y ? aa.o[1] : aa.o[0];
-  const uint32_t n = *a.n_ptr;
-  const uint32_t T = (n + C_TILE - 1) / C_TILE;
-  if (n == 0) {
-    if (blockIdx.x == 0 && threadIdx.x == 0) {
-      a.seg_off[0] = 0;
-      *a.n_seg = 0;
-    }
-    return;
-  }
-  const uint2* pairs = ord_final_buf(a);
-  const uint32_t lane = lane_id(), warp = warp_id();
-  __shared__ uint32_t s_w[KVG_WARPS];
-  __shared__ uint32_t s_base;
-  for (uint32_t tile = blockIdx.x; tile < T; tile += gridDim.x) {
-    const uint32_t base = tile * C_TILE + warp * C_WARP_ITEMS;
-    uint32_t bal[C_ROWS], key[C_ROWS], idx[C_ROWS];
-    const uint32_t wtot = ord_tile_heads(a, pairs, n, base, lane, true, bal, key, idx);
-    if (lane == 0) s_w[warp] = wtot;
-    __syncthreads();
-    if (warp == 0) {
-      uint32_t t = 0;
-#pragma unroll
-      for (uint32_t w = 0; w < KVG_WARPS; w++) t += s_w[w];
-      const uint32_t excl = lookback_sum(a.state, tile, t, epoch);
-      if (lane == 0) {
-        s_base = excl;
-        if (tile == T - 1) {
-          *a.n_seg = excl + t;
-          a.seg_off[excl + t] = n;
-        }
-      }
-    }
-    __syncthreads();
-    uint32_t off = s_base;
-#pragma unroll
-    for (uint32_t w = 0; w < KVG_WARPS; w++)
-      if (w < warp) off += s_w[w];
-    ord_emit_heads(a, off, base, lane, bal, key, idx);
-    __syncthreads();  // s_w / s_base are rewritten by the next tile
-  }
+  OrdHeadsOp op = ord_heads_op(aa, true);
+  lookback_tiles<OrdHeadsOp, KVG_BLOCK, C_ROWS>(op, op.a.state, epoch);
 }
 
 // bandwidth-bound sizes: <false> writes the permutation and counts heads per tile, k_tile_offsets scans the
@@ -590,36 +558,31 @@ __global__ void __launch_bounds__(KVG_BLOCK) k_order_final(OrdFinalArgs2 aa, uin
 template <bool EMIT>
 __global__ void __launch_bounds__(KVG_BLOCK) k_order_heads(OrdFinalArgs2 aa) {
   pdl_enter();
-  const OrdFinalArgs a = blockIdx.y ? aa.o[1] : aa.o[0];
-  const uint32_t n = *a.n_ptr;
-  const uint32_t T = (n + C_TILE - 1) / C_TILE;
-  if (n == 0) {
-    if (EMIT && blockIdx.x == 0 && threadIdx.x == 0) a.seg_off[0] = 0;
-    return;
-  }
-  const uint2* pairs = ord_final_buf(a);
+  using Tile = ClassifyTile<OrdHeadsOp, KVG_BLOCK, C_ROWS>;
+  OrdHeadsOp op = ord_heads_op(aa, !EMIT);
+  const uint32_t T = (op.n + C_TILE - 1) / C_TILE;
   const uint32_t lane = lane_id(), warp = warp_id();
+  // n_seg came from k_tile_offsets; finishing ends the last segment (of an empty list too)
+  if (EMIT && blockIdx.x == 0 && threadIdx.x == 0) op.finish(*op.a.n_seg);
   __shared__ uint32_t s_w[KVG_WARPS];
   for (uint32_t tile = blockIdx.x; tile < T; tile += gridDim.x) {
-    const uint32_t base = tile * C_TILE + warp * C_WARP_ITEMS;
-    uint32_t bal[C_ROWS], key[C_ROWS], idx[C_ROWS];
-    const uint32_t wtot = ord_tile_heads(a, pairs, n, base, lane, !EMIT, bal, key, idx);
-    if (lane == 0) s_w[warp] = wtot;
+    Tile ct;
+    ct.classify(op, tile);
+    if (lane == 0) s_w[warp] = ct.wtot;
     __syncthreads();
     if (!EMIT) {
       if (threadIdx.x == 0) {
         uint32_t t = 0;
 #pragma unroll
         for (uint32_t w = 0; w < KVG_WARPS; w++) t += s_w[w];
-        a.tile_heads[tile] = t;
+        op.a.tile_heads[tile] = t;
       }
     } else {
-      uint32_t off = a.tile_off[tile];
+      uint32_t off = op.a.tile_off[tile];
 #pragma unroll
       for (uint32_t w = 0; w < KVG_WARPS; w++)
         if (w < warp) off += s_w[w];
-      ord_emit_heads(a, off, base, lane, bal, key, idx);
-      if (tile == T - 1 && threadIdx.x == 0) a.seg_off[*a.n_seg] = n;
+      ct.emit(off, [&](uint32_t pos, const OrdHeadsOp::Item& it, uint32_t i, uint32_t x) { op.emit(pos, it, i, x); });
     }
     __syncthreads();  // s_w is rewritten by the next tile
   }

@@ -3,10 +3,10 @@
 //   k_classify_ragged<Op>  K3/K5 at bandwidth-bound sizes: every CTA classifies one tile and writes its
 //                          survivors at a TILE-LOCAL base (no cross-tile dependency); k_tile_offsets scans
 //                          the tile counts, k_pack_survivors makes the list dense
-//   k_classify_oneshot<Op> K3 at latency-bound sizes: one launch, decoupled look-back on the tile counts
+//   k_compact<Op,T,R>      one launch, decoupled look-back on the tile counts: K3 at latency-bound sizes, K6
 //        PciClassifyOp       createIommuDeviceMap's filter (device_plugin.go:201-244) + name join
 //        MdevClassifyOp      createVgpuIDMap's filter (:268-289)
-//   k_compact<HealthOp>    K6: alive-set diff against the previous scan
+//        HealthOp            K6: alive-set diff against the previous scan
 //   k_mdev_labels / _canon K5: label rule (:341-342) + merge of equal labels
 //   k_gen_*                counter-based synthetic snapshots (twins of oracle/kvg_oracle.c kvo_gen_*)
 #pragma once
@@ -35,125 +35,22 @@ struct ScanCtrl {
 };
 
 // ------------------------------------------------------------------------------------------------
-// The tile front-end of every classify kernel.  A warp owns 32 x ROWS consecutive records of the tile
-// (THREADS x ROWS records); `classify` issues every load before the first ballot, votes Op::pred per row and
-// calls Op::prepare for the survivors, whose dependent loads then overlap what the kernel does next.  `emit`
-// hands each of the lane's survivors to f(pos, item, i, aux), numbered in record order from the warp's offset.
-//   Op::Item                          what a thread holds per record
-//   uint32_t n                        number of records
-//   Item load(uint32_t i, bool ok)    ok == false -> any value that fails pred
-//   bool pred(const Item&, i)
-//   uint32_t prepare(const Item&)     per-survivor value handed to emit (name slot, canonical type)
+// The one-launch look-back compaction (lookback_tiles), in two shapes:
+//   K3 at latency-bound sizes, k_compact<PciClassifyOp, 128, 8>: small CTAs (1024 records kept in registers), one
+//   per tile, thousands of them, dispatched in blockIdx order by the hardware.  Many resident CTAs per SM hide the
+//   count -> look-back -> write-out latency chain of each other; predecessors were dispatched earlier, so the
+//   classic decoupled look-back usually finds an inclusive prefix close by.  (Measured alternative: every tile
+//   publishes its count and sums ALL earlier counts itself, a thread per earlier tile — no chain, but several
+//   dependent L2 round trips per thread for the last tiles; it was slower at 1 M records.  The chained scan stays.)
+//   K6, k_compact<HealthOp, KVG_BLOCK, C_ROWS>: a persistent, co-resident grid of 2048-record tiles (compact_grid).
+//   A look-back predecessor is owned by a resident CTA that reaches it no later than this CTA reaches its own tile
+//   (no ticket needed).  One CTA per tile measured about 5 % slower at 4 Mi records (39.5 against 37.7 us, H100 SXM
+//   with a 400 W power limit).
 // ------------------------------------------------------------------------------------------------
 template <class Op, int THREADS, int ROWS>
-struct ClassifyTile {
-  static constexpr uint32_t TILE = THREADS * ROWS;
-  static constexpr uint32_t NW = THREADS / 32;
-  static constexpr uint32_t WARP_ITEMS = 32 * ROWS;
-  typename Op::Item item[ROWS];
-  uint32_t bal[ROWS], aux[ROWS];
-  uint32_t base;  // the warp's first record
-  uint32_t wtot;  // the warp's survivors
-
-  __device__ __forceinline__ void classify(Op& op, uint32_t tile) {
-    const uint32_t lane = lane_id(), n = op.n;
-    base = tile * TILE + (threadIdx.x >> 5) * WARP_ITEMS;
-#pragma unroll
-    for (int k = 0; k < ROWS; k++) {
-      const uint32_t i = base + k * 32 + lane;
-      item[k] = op.load(i, i < n);
-    }
-    wtot = 0;
-#pragma unroll
-    for (int k = 0; k < ROWS; k++) {
-      const uint32_t i = base + k * 32 + lane;
-      const bool p = i < n && op.pred(item[k], i);
-      bal[k] = __ballot_sync(KVG_FULL, p);
-      wtot += __popc(bal[k]);
-      aux[k] = p ? op.prepare(item[k]) : 0u;
-    }
-  }
-  template <class F>
-  __device__ __forceinline__ void emit(uint32_t off, F&& f) const {
-    const uint32_t lane = lane_id();
-#pragma unroll
-    for (int k = 0; k < ROWS; k++) {
-      if ((bal[k] >> lane) & 1u) f(off + __popc(bal[k] & lanemask_lt()), item[k], base + k * 32 + lane, aux[k]);
-      off += __popc(bal[k]);
-    }
-  }
-};
-
-// One tile of the look-back compaction: classify it, place it behind all earlier tiles (decoupled look-back on
-// the tile counts), write its survivors.  Besides the front-end, Op provides emit(pos, item, i, aux),
-// tile_epilogue() (once per warp after its survivors) and finish(total) (one thread of the last tile).
-// s_wtot / s_woff: a word per warp of shared memory.
-template <class Op, int THREADS, int ROWS>
-__device__ __forceinline__ void lookback_tile(Op& op, uint32_t tile, uint32_t n_tiles, uint64_t* tile_state, uint32_t epoch,
-                                              uint32_t* s_wtot, uint32_t* s_woff, uint32_t& s_base) {
-  constexpr uint32_t NW = THREADS / 32;
-  const uint32_t lane = lane_id(), warp = threadIdx.x >> 5;
-  ClassifyTile<Op, THREADS, ROWS> ct;
-  ct.classify(op, tile);
-  if (lane == 0) s_wtot[warp] = ct.wtot;
-  __syncthreads();
-  if (warp == 0) {
-    uint32_t w = lane < NW ? s_wtot[lane] : 0;
-    uint32_t wi = warp_incl_sum(w);
-    if (lane < NW) s_woff[lane] = wi - w;
-    uint32_t tile_total = __shfl_sync(KVG_FULL, wi, NW - 1);
-    uint32_t excl = lookback_sum(tile_state, tile, tile_total, epoch);
-    if (lane == 0) {
-      s_base = excl;
-      if (tile == n_tiles - 1) op.finish(excl + tile_total);
-    }
-  }
-  __syncthreads();
-  ct.emit(s_base + s_woff[warp], [&](uint32_t pos, const typename Op::Item& r, uint32_t i, uint32_t a) { op.emit(pos, r, i, a); });
-  op.tile_epilogue();
-}
-
-// ------------------------------------------------------------------------------------------------
-// K3 at latency-bound sizes: small CTAs (THREADS x ROWS records kept in registers), thousands
-// of them, dispatched in blockIdx order by the hardware.  Many resident CTAs per SM hide the
-// count -> look-back -> write-out latency chain of each other; predecessors were dispatched
-// earlier, so the classic decoupled look-back usually finds an inclusive prefix close by.
-// (Measured alternative: every tile publishes its count and sums ALL earlier counts itself, a thread per
-// earlier tile — no chain, but several dependent L2 round trips per thread for the last tiles; it was slower
-// at 1 M records.  The chained scan stays.)
-// ------------------------------------------------------------------------------------------------
-template <class Op, int THREADS, int ROWS>
-__global__ void __launch_bounds__(THREADS) k_classify_oneshot(Op op, uint64_t* tile_state, uint32_t epoch) {
+__global__ void __launch_bounds__(THREADS) k_compact(Op op, uint64_t* tile_state, uint32_t epoch) {
   pdl_enter();
-  constexpr uint32_t TILE = THREADS * ROWS;
-  __shared__ uint32_t s_wtot[THREADS / 32], s_woff[THREADS / 32];
-  __shared__ uint32_t s_base;
-  const uint32_t n_tiles = (op.n + TILE - 1) / TILE;
-  const uint32_t tile = blockIdx.x;
-  if (n_tiles == 0) {
-    if (tile == 0 && threadIdx.x == 0) op.finish(0);
-    return;
-  }
-  if (tile >= n_tiles) return;
-  lookback_tile<Op, THREADS, ROWS>(op, tile, n_tiles, tile_state, epoch, s_wtot, s_woff, s_base);
-}
-
-// K6: the same compaction on a persistent, co-resident grid of 2048-record tiles; tile = blockIdx + k*gridDim.
-// A look-back predecessor is owned by a resident CTA that reaches it no later than this CTA reaches its own
-// tile (no ticket needed).  One CTA per tile (k_classify_oneshot<HealthOp, KVG_BLOCK, C_ROWS>) measured about
-// 5 % slower at 4 Mi records (39.5 against 37.7 us, H100 SXM with a 400 W power limit).
-template <class Op>
-__global__ void __launch_bounds__(KVG_BLOCK) k_compact(Op op, uint64_t* tile_state, uint32_t epoch) {
-  pdl_enter();
-  __shared__ uint32_t s_wtot[KVG_WARPS], s_woff[KVG_WARPS];
-  __shared__ uint32_t s_base;
-  const uint32_t n_tiles = (op.n + C_TILE - 1) / C_TILE;
-  if (n_tiles == 0) {
-    if (blockIdx.x == 0 && threadIdx.x == 0) op.finish(0);
-    return;
-  }
-  for (uint32_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x)
-    lookback_tile<Op, KVG_BLOCK, C_ROWS>(op, tile, n_tiles, tile_state, epoch, s_wtot, s_woff, s_base);
+  lookback_tiles<Op, THREADS, ROWS>(op, tile_state, epoch);
 }
 
 // ---- K3: PCI classify ---------------------------------------------------------------------------
@@ -594,7 +491,7 @@ __global__ void k_fill32(uint32_t* __restrict__ p, size_t n, uint32_t v) {
 //                      survivor once, no waiting on other CTAs: this is the HBM-roofline kernel.
 //   k_tile_offsets     exclusive scan of the tile counts (one CTA; n_tiles is ~N/1024)
 //   k_pack_survivors   dense, order-preserving copy scratch -> survivors using the known offsets
-// The single-pass look-back compaction (k_classify_oneshot, used below 2 M records) moves fewer bytes,
+// The single-pass look-back compaction (k_compact, used below 2 M records) moves fewer bytes,
 // but at sizes that are bandwidth-bound each of its CTAs spends most of its lifetime waiting for its
 // base offset, which makes it slower end to end than this split form there.
 // ------------------------------------------------------------------------------------------------

@@ -251,7 +251,7 @@ __global__ void __launch_bounds__(THREADS, CW4 <= 2 ? KVG_CS_MINB : KVG_CS_MINB_
   static_assert(TILE < (1u << CS_COUNT_BITS), "a tile count fits the count field");
   static_assert(ROWS <= 8, "warp-local positions (< 32 x ROWS) are packed in bytes");
   __shared__ uint32_t s_wcnt[NW][2][SH_MAX_RANKS];  // per warp: survivors of every (ordering, owner) -> prefix over the warps
-  __shared__ uint32_t s_wtot[NW], s_woff[NW];
+  __shared__ uint32_t s_wtot[NW];
   __shared__ uint32_t s_agg[CW], s_excl[CW];
   __shared__ uint32_t s_part[NW][CW];
   // the tile's survivors, staged in tile order: the registers that held the records are free during the prefix
@@ -308,10 +308,7 @@ __global__ void __launch_bounds__(THREADS, CW4 <= 2 ? KVG_CS_MINB : KVG_CS_MINB_
         uint32_t agg = 0;
         if (c == 0) {
 #pragma unroll
-          for (uint32_t w = 0; w < NW; w++) {
-            s_woff[w] = agg;
-            agg += s_wtot[w];
-          }
+          for (uint32_t w = 0; w < NW; w++) agg += s_wtot[w];
         } else if (c < C) {
           const uint32_t o = (c - 1) / A.P, q = (c - 1) - o * A.P;
 #pragma unroll

@@ -1,5 +1,5 @@
 """K3, the record-classification pipeline (k_classify_ragged -> k_tile_offsets -> k_pack_survivors, and
-the one-launch k_classify_oneshot), executed on the CPU from its real kernel source under the warp
+the one-launch k_compact<PciClassifyOp, 128, 8>), executed on the CPU from its real kernel source under the warp
 emulator of tools/emu/: drop rules of device_plugin.go:203-238, NUMA clamp, name join through nv_index,
 Walk-order compaction across tiles, the device-side maxima that size the radix plan."""
 import ctypes as C
@@ -59,7 +59,7 @@ def test_classify_pipeline_matches_the_drop_rules(emu, variant):
 
 
 def test_health_diff_kernel_reports_transitions_in_record_order(emu):
-    """K6 = k_compact<HealthOp> (BASELINE.json config 5): the transition list of every tick, like
+    """K6 = k_compact<HealthOp, 256, 8> (BASELINE.json config 5): the transition list of every tick, like
     tests/test_gpu_parity.py::test_health_rescan_transitions, from kernel source."""
     emu.emu_health_rescan.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]
     ids = O.nv_ids(util.pciids_text())

@@ -1,7 +1,7 @@
 // classify_emu.cpp — the record-classification pipeline of csrc/kvg_scan.cuh compiled for the CPU from
 // its real source on top of warp_emu.h: the split form the large inputs and the pipelined host entry
 // point use (k_classify_ragged -> k_tile_offsets -> k_pack_survivors) and the one-launch look-back form
-// used below 2 M records (k_classify_oneshot).  Launch shapes are those of enqueue_classify (kvg_api.cu).
+// used below 2 M records (k_compact).  Launch shapes are those of enqueue_classify (kvg_api.cu).
 #define KVG_HOST_EMU 1
 #include "warp_emu.h"
 #include "../../kubevirt-gpu-device-plugin_b200/csrc/kvg_scan.cuh"
@@ -10,7 +10,7 @@ using namespace kvg;
 extern "C" {
 
 // recs: n x 16 B records; nv_index: 65536 name slots; surv_out: room for n survivors.
-// variant 0 = ragged / offsets / pack, 1 = oneshot.  ctrl_out: {n_surv, max_group, max_devkey}.
+// variant 0 = ragged / offsets / pack, 1 = one-launch look-back.  ctrl_out: {n_surv, max_group, max_devkey}.
 int emu_classify_pci(const uint4* recs, uint32_t n, const uint32_t* nv_index, int variant, uint4* surv_out,
                      uint32_t* ctrl_out) {
   constexpr int T = 128, R = 8;
@@ -29,7 +29,7 @@ int emu_classify_pci(const uint4* recs, uint32_t n, const uint32_t* nv_index, in
   const uint32_t epoch = 7;
   if (variant == 1) {
     op.out = surv_out;
-    emu_launch(k_classify_oneshot<PciClassifyOp, T, R>, dim3((unsigned)(tiles ? tiles : 1)), T, op, state.data(), epoch);
+    emu_launch(k_compact<PciClassifyOp, T, R>, dim3((unsigned)(tiles ? tiles : 1)), T, op, state.data(), epoch);
   } else if (tiles) {
     op.out = ragged.data();
     emu_launch(k_classify_ragged<PciClassifyOp, T, R>, dim3((unsigned)tiles), T, op, tile_count.data(), tile_max.data());
@@ -62,7 +62,7 @@ int emu_health_rescan(const uint4* recs, uint32_t n, uint8_t* alive_prev, uint32
   op.changed = changed_out;
   op.ctrl = &ctrl;
   op.local_alive = 0;
-  emu_launch(k_compact<HealthOp>, dim3((unsigned)(tiles ? tiles : 1)), KVG_BLOCK, op, state.data(), 11u);
+  emu_launch(k_compact<HealthOp, KVG_BLOCK, C_ROWS>, dim3((unsigned)(tiles ? tiles : 1)), KVG_BLOCK, op, state.data(), 11u);
   ctrl_out[0] = ctrl.n_changed;
   ctrl_out[1] = ctrl.n_alive;
   return 0;
