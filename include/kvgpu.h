@@ -17,6 +17,7 @@
  *   kvg_scan_pci_delta                    <- (no reference equivalent: the reference never re-scans)
  *   kvg_scan_mdev_delta                   <- (no reference equivalent: createVgpuIDMap runs once)
  *   kvg_comm_*, kvg_scan_pci_sharded      <- (no reference equivalent; BASELINE.json config 4)
+ *   kvg_dev_scan_pci_shard_fetch_delta    <- (no reference equivalent: the re-scan delta of the sharded scan)
  *
  * Plain C: pointers + sizes only, no C++ types, no exceptions cross this boundary.
  * Return value: 0 = KVG_OK, negative = error; text via kvg_last_error().
@@ -240,7 +241,8 @@ typedef struct kvg_health_delta {
   const uint32_t *changed; /* [n_changed] (record index << 1) | now_alive, ascending index */
 } kvg_health_delta;
 
-/* ---- re-scan delta (K7): what changed since the previous kvg_scan_pci_delta / kvg_scan_mdev_delta */
+/* ---- re-scan delta (K7): what changed since the previous kvg_scan_pci_delta / kvg_scan_mdev_delta
+ * (kvg_pci_delta also serves kvg_dev_scan_pci_shard_fetch_delta, where "survivors" are the local shard's) */
 enum {
   KVG_CH_ADDED = 1u << 0,   /* survives now, did not before                    */
   KVG_CH_REMOVED = 1u << 1, /* survived before, does not now                    */
@@ -484,6 +486,42 @@ int kvg_comm_p2p_enable(kvg_ctx *ctx, int on);
  * Collective: every rank of the communicator must call it, in the same order. */
 int kvg_dev_scan_pci_sharded(kvg_ctx *ctx, const void *d_recs, size_t n_local);
 int kvg_dev_scan_pci_shard_fetch(kvg_ctx *ctx, kvg_pci_shard_result **res);
+/* Fetch the last kvg_dev_scan_pci_sharded like kvg_dev_scan_pci_shard_fetch, and diff it against the previous
+ * successful call of this function on this context: this rank's share of the re-scan delta of the whole snapshot.
+ *
+ * *res is byte for byte what kvg_dev_scan_pci_shard_fetch returns for the same scan.  *res and *delta are both freed
+ * with kvg_result_free.  The call is NOT collective: it reads nothing from peers.
+ *
+ * "Previous" is the result of the last SUCCESSFUL call of this function on this context since kvg_ctx_create or
+ * kvg_dev_scan_pci_shard_delta_reset; before any such call it is empty, so every local survivor is KVG_CH_ADDED,
+ * every owned key is dirty and nothing is gone.  The library keeps its own copy of it (the local survivors, both
+ * owned member lists and both owned key lists), separate from the other deltas': kvg_dev_scan_pci_shard_fetch, the
+ * other scans, the other deltas and their resets, the health calls, kvg_pciids_load and the mdev sharded scan in
+ * between leave it unchanged, and this call leaves theirs unchanged.
+ *
+ * changes: the local shard's survivors (res->local), keyed by address and in ascending address order, diffed against
+ * the previous local list by the rules of kvg_scan_pci_delta.  now_index / prev_index index res->local / the previous
+ * local list, and n_prev is the previous local count.  An address that crossed a shard boundary between the two
+ * scans shows as KVG_CH_REMOVED on one rank and KVG_CH_ADDED on another; merging the ranks' changes in address order
+ * and fusing such pairs gives exactly the kvg_scan_pci_delta of the concatenated snapshot.
+ *
+ * dev_dirty / grp_dirty: indices into res->dev_keys / res->grp_keys, the keys this rank owns (key % nranks == rank),
+ * by the rule of kvg_scan_pci_delta: the (addr, numa) sequence of the key's members, in Walk order, changed.  The
+ * owner of a key does not change between scans and the owned member lists hold every member from every shard, so
+ * diffing them gives exactly this rank's share of the global lists, with no communication; a member that moved to a
+ * key another rank owns is removed here and added there.  dev_gone / grp_gone: owned keys present before and absent
+ * now.
+ *
+ * Precondition: survivor addresses ascend strictly in global Walk order (shards in rank order), and a handle means
+ * the same device in both snapshots.  The local list and both owned member lists are checked for strict ascent on the
+ * device: if that fails the call returns KVG_EINVAL (text in kvg_last_error), hands out no objects, and the previous
+ * result stays as it was; so does every error of the fetch itself (e.g. KVG_ENCCL when a peer timed out).
+ * KVG_EINVAL when the last scan on the context was not kvg_dev_scan_pci_sharded.
+ *
+ * Cost beyond kvg_dev_scan_pci_shard_fetch: two kernel launches and one synchronisation. */
+int kvg_dev_scan_pci_shard_fetch_delta(kvg_ctx *ctx, kvg_pci_shard_result **res, kvg_pci_delta **delta);
+/* forget the previous result: the next kvg_dev_scan_pci_shard_fetch_delta reports everything as added */
+int kvg_dev_scan_pci_shard_delta_reset(kvg_ctx *ctx);
 /* the same for mdev records (createVgpuIDMap): type / parent orderings of the owned members */
 int kvg_dev_scan_mdev_sharded(kvg_ctx *ctx, const void *d_recs, size_t n_local, const kvg_type_dict *types);
 int kvg_dev_scan_mdev_shard_fetch(kvg_ctx *ctx, kvg_mdev_shard_result **res);

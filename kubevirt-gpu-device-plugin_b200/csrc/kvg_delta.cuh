@@ -1,4 +1,5 @@
-// kvg_delta.cuh — K7: the keyed diff of two scans (kvg_scan_pci_delta, kvg_scan_mdev_delta).
+// kvg_delta.cuh — K7: the keyed diff of two scans (kvg_scan_pci_delta, kvg_scan_mdev_delta,
+// kvg_dev_scan_pci_shard_fetch_delta).
 //
 //   k_delta_merge<Tr>  merge path over the previous scan's survivors and the new ones (ascending key), one change
 //                      entry per key whose survivor differs, compacted in key order by the look-back tile body of
@@ -6,6 +7,8 @@
 //                      changes.  Also checks that the new list ascends strictly.  Tr is the record trait:
 //                      PciDeltaRec (16-byte survivors keyed by address) or MdevDeltaRec (32-byte survivors keyed by
 //                      the 128-bit big-endian UUID).
+//   k_delta_merge_shard  the same merge over a rank's three PCI lists, one per blockIdx.y: its local survivors
+//                      (change entries), the members of the device ids and of the groups it owns (key tags only)
 //   k_delta_lists      the four key lists (dirty / gone of both maps) from those tags: one look-back compaction per
 //                      list (blockIdx.y) through the same tile body
 //   k_mdev_delta_types the previous result's type keys in the new key space: same sanitised label, or none
@@ -100,6 +103,11 @@ struct PciDeltaRec {
     st_stream(out + 2 * (size_t)pos, make_uint4(hp ? p.x : q.x, what, p.y, q.y));
     st_stream(out + 2 * (size_t)pos + 1,
               make_uint4((p.z & 0xffffu) | (q.z << 16), (p.z >> 16) | (q.z & 0xffff0000u), b, a));
+    mark(what, hp, hn, p, q, dev, grp, tag);
+  }
+  // the keys alone (the sharded merge's owned lists tag keys and write no entry)
+  __device__ __forceinline__ static void mark(uint32_t what, bool hp, bool hn, const Rec& p, const Rec& q,
+                                              const DeltaKeys& dev, const DeltaKeys& grp, uint32_t tag) {
     if (what & (KVG_CH_ADDED | KVG_CH_REMOVED | KVG_CH_DEVICE | KVG_CH_NUMA))
       dev.mark(hn, q.z & 0xffffu, hp, p.z & 0xffffu, tag);
     if (what & (KVG_CH_ADDED | KVG_CH_REMOVED | KVG_CH_GROUP | KVG_CH_NUMA)) grp.mark(hn, q.y, hp, p.y, tag);
@@ -217,39 +225,33 @@ struct DeltaMergeOp {
   }
   __device__ __forceinline__ bool pred(const Item& it, uint32_t) const { return it.what != 0; }
   __device__ __forceinline__ uint32_t prepare(const Item&) const { return 0; }
-  // the change entry and the keys it dirties
-  __device__ __forceinline__ void emit(uint32_t pos, const Item& it, uint32_t i, uint32_t) const {
+  // the change at merged position i: ENTRY, its entry at `pos` and the keys it dirties; otherwise the keys alone
+  template <bool ENTRY>
+  __device__ __forceinline__ void apply(uint32_t pos, const Item& it, uint32_t i) const {
     const uint32_t x = it.code & 0x7fffffffu;
     const uint32_t a = (it.code >> 31) ? DELTA_NONE : x;
     const uint32_t b = (it.code >> 31) ? x : ((it.what & KVG_CH_REMOVED) ? DELTA_NONE : i - x);
     const bool hp = a != DELTA_NONE, hn = b != DELTA_NONE;
     const Rec p = hp ? rec_prev(a) : Rec{};
     const Rec q = hn ? rec_now(b) : Rec{};
-    Tr::emit(out, pos, it.what, hp, hn, a, b, p, q, k0, k1, tag);
+    if constexpr (ENTRY)
+      Tr::emit(out, pos, it.what, hp, hn, a, b, p, q, k0, k1, tag);
+    else
+      Tr::mark(it.what, hp, hn, p, q, k0, k1, tag);
+  }
+  __device__ __forceinline__ void emit(uint32_t pos, const Item& it, uint32_t i, uint32_t) const {
+    apply<true>(pos, it, i);
   }
   __device__ __forceinline__ void tile_epilogue() {}
   __device__ __forceinline__ void finish(uint32_t total) { ctrl->reserved2[DELTA_W_CHANGES] = total; }
 };
 
-// One CTA per DELTA_TILE merged positions.  O(n_prev + n_now): two diagonal searches per CTA, a shared-memory merge,
-// one pass of the look-back compaction.  The tag doubles as the look-back epoch.  Static shared memory: DELTA_TILE
-// staged survivors (16 KiB PCI, 32 KiB mdev) and the merge codes (4 KiB).
+// Stage merge tile `tile` of o in the CTA: the two diagonal searches, both list slices in s_rec (checking that the
+// new one ascends strictly) and the merge codes in s_code.  Sets o's slice fields and shared-memory pointers.
 template <class Tr>
-__global__ void __launch_bounds__(DELTA_THREADS) k_delta_merge(DeltaMergeOp<Tr> op, uint64_t* tile_state) {
+__device__ __forceinline__ void delta_stage(DeltaMergeOp<Tr>& o, uint32_t tile, typename Tr::Rec* s_rec,
+                                            uint32_t* s_code, uint32_t* s_split) {
   using Rec = typename Tr::Rec;
-  pdl_enter();
-  __shared__ Rec s_rec[DELTA_TILE];
-  __shared__ uint32_t s_code[DELTA_TILE];
-  __shared__ uint32_t s_split[2];
-  __shared__ uint32_t s_wtot[DELTA_THREADS / 32], s_woff[DELTA_THREADS / 32];
-  __shared__ uint32_t s_base;
-  DeltaMergeOp<Tr> o = op;
-  const uint32_t n_tiles = (o.n + DELTA_TILE - 1) / DELTA_TILE, tile = blockIdx.x;
-  if (n_tiles == 0) {
-    if (tile == 0 && threadIdx.x == 0) o.finish(0);
-    return;
-  }
-  if (tile >= n_tiles) return;
   const uint32_t d0 = tile * DELTA_TILE, d1 = min(o.n, d0 + DELTA_TILE);
   if (threadIdx.x == 0 || threadIdx.x == 32) {
     const uint32_t hi = threadIdx.x != 0;
@@ -298,7 +300,68 @@ __global__ void __launch_bounds__(DELTA_THREADS) k_delta_merge(DeltaMergeOp<Tr> 
   __syncthreads();
   o.s_rec = s_rec;
   o.s_code = s_code;
+}
+
+// One CTA per DELTA_TILE merged positions.  O(n_prev + n_now): two diagonal searches per CTA, a shared-memory merge,
+// one pass of the look-back compaction.  The tag doubles as the look-back epoch.  Static shared memory: DELTA_TILE
+// staged survivors (16 KiB PCI, 32 KiB mdev) and the merge codes (4 KiB).
+template <class Tr>
+__global__ void __launch_bounds__(DELTA_THREADS) k_delta_merge(DeltaMergeOp<Tr> op, uint64_t* tile_state) {
+  using Rec = typename Tr::Rec;
+  pdl_enter();
+  __shared__ Rec s_rec[DELTA_TILE];
+  __shared__ uint32_t s_code[DELTA_TILE];
+  __shared__ uint32_t s_split[2];
+  __shared__ uint32_t s_wtot[DELTA_THREADS / 32], s_woff[DELTA_THREADS / 32];
+  __shared__ uint32_t s_base;
+  DeltaMergeOp<Tr> o = op;
+  const uint32_t n_tiles = (o.n + DELTA_TILE - 1) / DELTA_TILE, tile = blockIdx.x;
+  if (n_tiles == 0) {
+    if (tile == 0 && threadIdx.x == 0) o.finish(0);
+    return;
+  }
+  if (tile >= n_tiles) return;
+  delta_stage<Tr>(o, tile, s_rec, s_code, s_split);
   lookback_tile<DeltaMergeOp<Tr>, DELTA_THREADS, DELTA_ROWS>(o, tile, n_tiles, tile_state, o.tag, s_wtot, s_woff, s_base);
+}
+
+// The sharded PCI form (kvg_dev_scan_pci_shard_fetch_delta): one merge per blockIdx.y over one pair of this rank's
+// lists, all three checked for strict ascent.
+//   y = 0  the local survivors: change entries through the look-back tile body; its DeltaKeys are empty, so it
+//          tags no key
+//   y = 1  the members of the owned device ids: deviceMap tags only (k1 empty), no entries
+//   y = 2  the members of the owned groups: iommuMap tags only (k0 empty), no entries
+// Each row has its own tile count and its surplus CTAs exit before any look-back.  Only row 0 takes part in one
+// (words tile_state[0 ..)), and a tile waits only on earlier tiles of that row, as in k_delta_lists.
+struct DeltaShardArgs {
+  DeltaMergeOp<PciDeltaRec> o[3];
+};
+__global__ void __launch_bounds__(DELTA_THREADS) k_delta_merge_shard(DeltaShardArgs args, uint64_t* tile_state) {
+  using Tr = PciDeltaRec;
+  pdl_enter();
+  __shared__ Tr::Rec s_rec[DELTA_TILE];
+  __shared__ uint32_t s_code[DELTA_TILE];
+  __shared__ uint32_t s_split[2];
+  __shared__ uint32_t s_wtot[DELTA_THREADS / 32], s_woff[DELTA_THREADS / 32];
+  __shared__ uint32_t s_base;
+  // picked by value: indexing the parameter array by blockIdx.y made ptxas spill (64 registers, 8-byte stack frame)
+  DeltaMergeOp<Tr> o = blockIdx.y == 0 ? args.o[0] : blockIdx.y == 1 ? args.o[1] : args.o[2];
+  const uint32_t n_tiles = (o.n + DELTA_TILE - 1) / DELTA_TILE, tile = blockIdx.x;
+  if (n_tiles == 0) {
+    if (blockIdx.y == 0 && tile == 0 && threadIdx.x == 0) o.finish(0);
+    return;
+  }
+  if (tile >= n_tiles) return;
+  delta_stage<Tr>(o, tile, s_rec, s_code, s_split);
+  if (blockIdx.y == 0) {
+    lookback_tile<DeltaMergeOp<Tr>, DELTA_THREADS, DELTA_ROWS>(o, tile, n_tiles, tile_state, o.tag, s_wtot, s_woff,
+                                                               s_base);
+    return;
+  }
+  for (uint32_t k = threadIdx.x; k < o.na + o.nb; k += DELTA_THREADS) {
+    const DeltaMergeOp<Tr>::Item it = o.load(o.d0 + k, true);
+    if (it.what) o.apply<false>(0, it, o.d0 + k);
+  }
 }
 
 // One of the four key lists: keys whose tag word holds this call's tag, ascending.  Dirty lists give the key's

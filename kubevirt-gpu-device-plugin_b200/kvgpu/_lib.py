@@ -185,6 +185,8 @@ def load() -> C.CDLL:
         "kvg_debug_radix_plan": (C.c_int, [C.c_uint32, C.c_uint32, C.c_uint32, vp, vp, vp]),
         "kvg_dev_scan_pci_sharded": (C.c_int, [vp, vp, sz]),
         "kvg_dev_scan_pci_shard_fetch": (C.c_int, [vp, P(P(PciShardResultC))]),
+        "kvg_dev_scan_pci_shard_fetch_delta": (C.c_int, [vp, P(P(PciShardResultC)), P(P(PciDeltaC))]),
+        "kvg_dev_scan_pci_shard_delta_reset": (C.c_int, [vp]),
         "kvg_dev_scan_mdev_sharded": (C.c_int, [vp, vp, sz, P(TypeDict)]),
         "kvg_dev_scan_mdev_shard_fetch": (C.c_int, [vp, P(P(MdevShardResultC))]),
     }

@@ -268,13 +268,7 @@ class Context:
     def health_reset(self):
         self._ck(self._lib.kvg_health_reset(self._h))
 
-    def scan_pci_delta(self, recs: np.ndarray):
-        """scan_pci plus the keyed diff against the previous scan_pci_delta on this context -> (PciResult, PciDelta).
-        Meaningful for numeric (packed-BDF) snapshots; with index-mode handles it is relative to the handles."""
-        recs = np.ascontiguousarray(recs, dtype=L.PCI_REC)
-        res = C.POINTER(L.PciResultC)()
-        dl = C.POINTER(L.PciDeltaC)()
-        self._ck(self._lib.kvg_scan_pci_delta(self._h, recs.ctypes.data, len(recs), C.byref(res), C.byref(dl)))
+    def _take_pci_delta(self, dl) -> PciDelta:
         d = dl.contents
         delta = PciDelta(int(d.n_prev), L._arr(d.changes, int(d.n_changes), L.PCI_CHANGE),
                          L._arr(d.dev_dirty, int(d.n_dev_dirty), np.uint32),
@@ -282,6 +276,16 @@ class Context:
                          L._arr(d.grp_dirty, int(d.n_grp_dirty), np.uint32),
                          L._arr(d.grp_gone, int(d.n_grp_gone), np.uint32))
         self._lib.kvg_result_free(dl)
+        return delta
+
+    def scan_pci_delta(self, recs: np.ndarray):
+        """scan_pci plus the keyed diff against the previous scan_pci_delta on this context -> (PciResult, PciDelta).
+        Meaningful for numeric (packed-BDF) snapshots; with index-mode handles it is relative to the handles."""
+        recs = np.ascontiguousarray(recs, dtype=L.PCI_REC)
+        res = C.POINTER(L.PciResultC)()
+        dl = C.POINTER(L.PciDeltaC)()
+        self._ck(self._lib.kvg_scan_pci_delta(self._h, recs.ctypes.data, len(recs), C.byref(res), C.byref(dl)))
+        delta = self._take_pci_delta(dl)
         return self._take_pci(res), delta
 
     def scan_pci_delta_reset(self):
@@ -399,6 +403,23 @@ class Context:
     def dev_scan_pci_shard_fetch(self) -> PciShardResult:
         res = C.POINTER(L.PciShardResultC)()
         self._ck(self._lib.kvg_dev_scan_pci_shard_fetch(self._h, C.byref(res)))
+        return self._take_pci_shard(res)
+
+    def dev_scan_pci_shard_fetch_delta(self):
+        """dev_scan_pci_shard_fetch plus this rank's share of the re-scan delta, against the previous successful call
+        on this context -> (PciShardResult, PciDelta).  changes are the local shard's (indices into `local`),
+        dev_dirty / grp_dirty index the owned keys (res.dev.dev_keys / res.grp.grp_keys), dev_gone / grp_gone are
+        owned keys that went.  Not collective; kvgpu.merge_pci_shard_deltas fuses the ranks' parts."""
+        res = C.POINTER(L.PciShardResultC)()
+        dl = C.POINTER(L.PciDeltaC)()
+        self._ck(self._lib.kvg_dev_scan_pci_shard_fetch_delta(self._h, C.byref(res), C.byref(dl)))
+        delta = self._take_pci_delta(dl)
+        return self._take_pci_shard(res), delta
+
+    def dev_scan_pci_shard_delta_reset(self):
+        self._ck(self._lib.kvg_dev_scan_pci_shard_delta_reset(self._h))
+
+    def _take_pci_shard(self, res) -> PciShardResult:
         r = res.contents
         KD, G = int(r.n_dev_keys), int(r.n_groups)
         pool = C.string_at(r.name_pool, r.name_pool_len) if r.name_pool_len else b""

@@ -7,13 +7,23 @@ rank ends up with all members of the keys it owns — constant volume per GPU wh
 stores into the owners' peer windows over NVLink (CUDA IPC), or — fallback — one NCCL allgatherv of the
 survivor lists followed by a local select.  The pci.ids table is parsed by every rank itself.
 
+Re-scan deltas (Context.dev_scan_pci_shard_fetch_delta): each rank diffs its own shard and the keys it owns with no
+communication; apply_pci_shard_delta patches its part of the maps, and merge_pci_shard_deltas over the ranks'
+shard_delta_part summaries gives the delta of the whole snapshot.
+
 `ShardedScan` needs only byte collectives (broadcast for the 128-byte NCCL unique id, all-gather for the
 64-byte IPC handles), so the same class is driven by torch.distributed (bench.py) or any other launcher.
 """
 from __future__ import annotations
 
+from dataclasses import dataclass
+
+import numpy as np
+
+from . import _lib as L
 from .context import Context, MdevShardResult, PciResult, PciShardResult
-from .plugin import Maps, mdev_maps_from_result, pci_maps_from_result
+from .plugin import (Maps, PciMapsTouched, _fully_numeric, _patch_pci_maps, _rebuild_into, mdev_maps_from_result,
+                     pci_maps_from_result)
 
 
 def shard_range(n: int, rank: int, world: int) -> tuple[int, int]:
@@ -76,6 +86,81 @@ def mdev_maps_from_shard(sh: MdevShardResult) -> Maps:
     return Maps(vGpuMap=a.vGpuMap, gpuVgpuMap=b.gpuVgpuMap, deviceNames=a.deviceNames)
 
 
+def apply_pci_shard_delta(part: Maps, res: PciShardResult, delta, snap=None, prev_snap=None) -> PciMapsTouched:
+    """Patch one rank's part of the maps (pci_maps_from_shard of its previous fetch_delta result) into what
+    pci_maps_from_shard(res) builds: the owned deviceMap / iommuMap keys that are dirty or gone and the local
+    bdfToIommuMap entries of changed addresses, nothing else.  As in apply_pci_delta, a snapshot that is not fully
+    numeric has no stable handles: the part is then rebuilt and every key is reported."""
+    if not (_fully_numeric(snap) and _fully_numeric(prev_snap)):
+        def build(m):
+            fresh = pci_maps_from_shard(res)
+            for key in set(m.deviceMap) - set(fresh.deviceMap):
+                m.deviceNames.pop(key, None)
+            m.deviceMap, m.iommuMap, m.bdfToIommuMap = fresh.deviceMap, fresh.iommuMap, fresh.bdfToIommuMap
+            m.deviceNames.update(fresh.deviceNames)
+        return _rebuild_into(part, build)
+    return _patch_pci_maps(part, res.dev, res.grp, delta)
+
+
+@dataclass
+class PciShardDelta:
+    """A re-scan delta with its keys as values: one rank's part (shard_delta_part; indices local to its shard) or
+    the whole snapshot's (merge_pci_shard_deltas; indices into the concatenated survivor lists)."""
+    n_prev: int                 # survivors of the previous result
+    n_now: int                  # survivors now
+    changes: np.ndarray         # PCI_CHANGE, ascending addr
+    dev_dirty: np.ndarray       # u16 device ids whose (addr, numa) member sequence changed, ascending
+    dev_gone: np.ndarray        # u16 device ids absent now, ascending
+    grp_dirty: np.ndarray       # u32 groups, ascending
+    grp_gone: np.ndarray        # u32 groups absent now, ascending
+
+
+def shard_delta_part(res: PciShardResult, delta) -> PciShardDelta:
+    """The small summary of one rank's fetch_delta that the merge needs: counts, changes and key values (no member
+    arrays, so all_gather_object ships little)."""
+    return PciShardDelta(int(delta.n_prev), len(res.local), delta.changes,
+                         res.dev.dev_keys[delta.dev_dirty].astype(np.uint16), delta.dev_gone,
+                         res.grp.grp_keys[delta.grp_dirty].astype(np.uint32), delta.grp_gone)
+
+
+def merge_pci_shard_deltas(parts: list) -> PciShardDelta:
+    """The delta of the whole snapshot from the ranks' shard_delta_part summaries (rank order): equal to
+    kvg_scan_pci_delta on the concatenated snapshot (changes byte for byte, dirty keys as values).  Changes are
+    sorted by address; an address that crossed a shard boundary is REMOVED on one rank and ADDED on another, and
+    the pair fuses into one entry whose bits compare the two survivors (none: no entry).  Local indices become
+    global through prefix sums of the per-rank counts; the key lists are unions (ranks own disjoint keys)."""
+    none = np.uint32(0xFFFFFFFF)
+    prev_off = np.cumsum([0] + [p.n_prev for p in parts])
+    now_off = np.cumsum([0] + [p.n_now for p in parts])
+    chs = []
+    for r, p in enumerate(parts):
+        c = p.changes.copy()
+        c["prev_index"] = np.where(c["prev_index"] == none, none, c["prev_index"] + np.uint32(prev_off[r]))
+        c["now_index"] = np.where(c["now_index"] == none, none, c["now_index"] + np.uint32(now_off[r]))
+        chs.append(c)
+    ch = np.concatenate(chs) if chs else np.zeros(0, L.PCI_CHANGE)
+    ch = ch[np.argsort(ch["addr"], kind="stable")]
+    dup = np.nonzero(ch["addr"][1:] == ch["addr"][:-1])[0]      # pairs: i (one side), i + 1 (the other)
+    if len(dup):
+        rem = (ch["what"][dup] & L.CH_REMOVED) != 0             # which of the two is the REMOVED entry
+        gone_, new_ = ch[np.where(rem, dup, dup + 1)], ch[np.where(rem, dup + 1, dup)]
+        if not ((gone_["what"] == L.CH_REMOVED) & (new_["what"] == L.CH_ADDED)).all():
+            raise ValueError("one address twice, not as REMOVED + ADDED: the shards overlap")
+        f = new_.copy()
+        for side in ("prev_group", "prev_device", "prev_numa", "prev_index"):
+            f[side] = gone_[side]
+        f["what"] = ((f["prev_group"] != f["now_group"]) * L.CH_GROUP | (f["prev_device"] != f["now_device"]) * L.CH_DEVICE
+                     | (f["prev_numa"] != f["now_numa"]) * L.CH_NUMA).astype(np.uint32)
+        keep = np.ones(len(ch), dtype=bool)
+        keep[dup + 1] = False
+        ch[dup] = f
+        keep[dup[f["what"] == 0]] = False
+        ch = ch[keep]
+    cat = lambda name, dt: np.unique(np.concatenate([getattr(p, name) for p in parts] + [np.zeros(0, dt)])).astype(dt)
+    return PciShardDelta(int(prev_off[-1]), int(now_off[-1]), np.ascontiguousarray(ch), cat("dev_dirty", np.uint16),
+                         cat("dev_gone", np.uint16), cat("grp_dirty", np.uint32), cat("grp_gone", np.uint32))
+
+
 def merge_parts(parts: list) -> Maps:
     """Union of the ranks' parts (rank order): key sets are disjoint, bdfToIommuMap concatenates in rank
     order == Walk order."""
@@ -100,6 +185,7 @@ class ShardedScan:
         record takes two): also set up the peer windows (CUDA IPC over NVLink); on any failure the NCCL
         path is used."""
         self.ctx, self.rank, self.world = ctx, rank, world
+        self._bcast, self._allgather = broadcast_bytes, allgather_bytes
         self.mode = "nccl"
         uid = ctx.comm_unique_id() if rank == 0 else None
         uid = broadcast_bytes(uid, 0)
@@ -126,6 +212,34 @@ class ShardedScan:
 
     def fetch(self) -> PciShardResult:
         return self.ctx.dev_scan_pci_shard_fetch()
+
+    def fetch_delta(self):
+        """fetch plus this rank's share of the re-scan delta -> (PciShardResult, PciDelta), see
+        Context.dev_scan_pci_shard_fetch_delta.  Collective here (not in the library): every rank learns every
+        rank's status.  If any rank's call failed, EVERY rank resets its previous result and raises KvgError, so that
+        the ranks never diff against previous results of different steps; the next step then reports everything as
+        added on every rank."""
+        err, out = None, None
+        try:
+            out = self.ctx.dev_scan_pci_shard_fetch_delta()
+        except L.KvgError as e:
+            err = e
+        if all(s[:1] == b"\1" for s in self._statuses(b"\0" if err else b"\1")):
+            return out
+        self.ctx.dev_scan_pci_shard_delta_reset()
+        if err is not None:
+            raise err
+        raise L.KvgError(L.KVG_ESTATE, "fetch_delta failed on another rank; every rank's previous result is reset")
+
+    def delta_reset(self):
+        """Forget this rank's previous result (call it on every rank)."""
+        self.ctx.dev_scan_pci_shard_delta_reset()
+
+    def _statuses(self, mine: bytes) -> list:
+        """every rank's status byte, in rank order"""
+        if self._allgather is not None:
+            return self._allgather(mine)
+        return [self._bcast(mine if q == self.rank else None, q) for q in range(self.world)]
 
     def scan_device_mdev_shard(self, d_recs: int, n_local: int, raw_types: list):
         self.ctx.dev_scan_mdev_sharded(d_recs, n_local, raw_types)

@@ -385,33 +385,32 @@ def _fully_numeric(snap: PciSnapshot | None) -> bool:
     return snap is None or (snap.packed_addr and snap.group_names is None and snap.device_names is None)
 
 
-def _rebuild_pci_maps(maps: Maps, res: PciResult, snap, name_of) -> PciMapsTouched:
-    """pci_maps_from_result into `maps`, reporting every key of the new maps and every key that went."""
+def _rebuild_into(maps: Maps, build) -> PciMapsTouched:
+    """build(maps) rebuilds the PCI maps in `maps`; reports every key of the new maps and every key that went."""
     before_dev, before_grp = set(maps.deviceMap), set(maps.iommuMap)
-    pci_maps_from_result(res, snap, maps, name_of=name_of)
+    build(maps)
     return PciMapsTouched(list(maps.deviceMap), sorted(before_dev - set(maps.deviceMap)),
                           list(maps.iommuMap), sorted(before_grp - set(maps.iommuMap)))
 
 
-def apply_pci_delta(maps: Maps, res: PciResult, delta, snap: PciSnapshot | None = None,
-                    prev_snap: PciSnapshot | None = None, name_of=None) -> PciMapsTouched:
-    """Patch deviceMap, iommuMap and bdfToIommuMap of `maps` (built from the previous delta scan's result) into
-    what pci_maps_from_result(res) builds, touching only dirty or gone keys and changed addresses.  A snapshot
-    that is not fully numeric (index-mode addresses, groups or device strings) has no stable handles: the maps are
-    then rebuilt and every key is reported."""
-    if not (_fully_numeric(snap) and _fully_numeric(prev_snap)):
-        return _rebuild_pci_maps(maps, res, snap, name_of)
-    s = res.survivors
+def _rebuild_pci_maps(maps: Maps, res: PciResult, snap, name_of) -> PciMapsTouched:
+    """pci_maps_from_result into `maps`, reporting every key of the new maps and every key that went."""
+    return _rebuild_into(maps, lambda m: pci_maps_from_result(res, snap, m, name_of=name_of))
 
-    def members(perm, off, k):
+
+def _patch_pci_maps(maps: Maps, dev: PciResult, grp: PciResult, delta) -> PciMapsTouched:
+    """The numeric patch of apply_pci_delta: deviceMap keys from `dev`, iommuMap keys from `grp` (each result's
+    permutation indexes its own survivors), bdfToIommuMap from the changes."""
+    def members(res, perm, off, k):
+        s = res.survivors
         idx = perm[off[k]:off[k + 1]]
         return [NvidiaGpuDevice(format_bdf(int(s["addr"][i])), int(s["numa"][i])) for i in idx]
 
     t = PciMapsTouched([], [], [], [])
     for k in delta.dev_dirty:
-        key = "%04x" % int(res.dev_keys[k])
-        maps.deviceMap[key] = members(res.dev_perm, res.dev_off, k)
-        maps.deviceNames[key] = res.name_at(int(res.dev_name_slot[k]))
+        key = "%04x" % int(dev.dev_keys[k])
+        maps.deviceMap[key] = members(dev, dev.dev_perm, dev.dev_off, k)
+        maps.deviceNames[key] = dev.name_at(int(dev.dev_name_slot[k]))
         t.dev_dirty.append(key)
     for d in delta.dev_gone:
         key = "%04x" % int(d)
@@ -419,8 +418,8 @@ def apply_pci_delta(maps: Maps, res: PciResult, delta, snap: PciSnapshot | None 
         maps.deviceNames.pop(key, None)
         t.dev_gone.append(key)
     for k in delta.grp_dirty:
-        key = str(int(res.grp_keys[k]))
-        maps.iommuMap[key] = members(res.grp_perm, res.grp_off, k)
+        key = str(int(grp.grp_keys[k]))
+        maps.iommuMap[key] = members(grp, grp.grp_perm, grp.grp_off, k)
         t.grp_dirty.append(key)
     for g in delta.grp_gone:
         key = str(int(g))
@@ -433,6 +432,17 @@ def apply_pci_delta(maps: Maps, res: PciResult, delta, snap: PciSnapshot | None 
         else:
             maps.bdfToIommuMap[addr] = str(int(c["now_group"]))
     return t
+
+
+def apply_pci_delta(maps: Maps, res: PciResult, delta, snap: PciSnapshot | None = None,
+                    prev_snap: PciSnapshot | None = None, name_of=None) -> PciMapsTouched:
+    """Patch deviceMap, iommuMap and bdfToIommuMap of `maps` (built from the previous delta scan's result) into
+    what pci_maps_from_result(res) builds, touching only dirty or gone keys and changed addresses.  A snapshot
+    that is not fully numeric (index-mode addresses, groups or device strings) has no stable handles: the maps are
+    then rebuilt and every key is reported."""
+    if not (_fully_numeric(snap) and _fully_numeric(prev_snap)):
+        return _rebuild_pci_maps(maps, res, snap, name_of)
+    return _patch_pci_maps(maps, res, res, delta)
 
 
 def mdev_maps_from_result(res: MdevResult, snap: MdevSnapshot | None = None, maps: Maps | None = None) -> Maps:

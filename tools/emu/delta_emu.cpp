@@ -50,6 +50,54 @@ int emu_delta(const uint4* prev, uint32_t n_prev, const uint4* now, uint32_t n_n
   return 0;
 }
 
+// One rank of the sharded delta.  prev[y] / now[y] with n_prev[y] / n_now[y] entries (16-byte kvg_pci_surv, Walk
+// order): y = 0 the local survivors, 1 the members of the owned device ids, 2 the members of the owned groups.  keys:
+// the owned device ids now, before, the owned groups now, before.  flags, tag, changes (room for n_prev[0] +
+// n_now[0] entries), the four lists and counts as for emu_delta.
+int emu_shard_delta(const uint4* const* prev, const uint32_t* n_prev, const uint4* const* now, const uint32_t* n_now,
+                    const uint32_t* const* keys, const uint32_t* n_keys, uint32_t* flags, uint32_t flag_cap,
+                    uint32_t tag, uint4* changes, uint32_t* dev_dirty, uint16_t* dev_gone, uint32_t* grp_dirty,
+                    uint32_t* grp_gone, uint32_t* counts) {
+  ScanCtrl ctrl;
+  memset(&ctrl, 0, sizeof ctrl);
+  const uint32_t M = n_prev[0] + n_now[0];
+  const uint32_t merge_tiles = M ? (M + DELTA_TILE - 1) / DELTA_TILE : 1;
+  uint32_t list_tiles = 1;
+  for (int k = 0; k < 4; k++) list_tiles = max(list_tiles, (n_keys[k] + C_TILE - 1) / C_TILE);
+  std::vector<uint64_t> state(merge_tiles + 1 + 4 * (list_tiles + 1), 0);
+  uint32_t* f[4];
+  for (int k = 0; k < 4; k++) f[k] = flags + (size_t)k * flag_cap;
+  DeltaShardArgs a;
+  uint32_t cols = merge_tiles;
+  for (int y = 0; y < 3; y++) {
+    DeltaMergeOp<PciDeltaRec>& o = a.o[y];
+    o = {};
+    o.prev = prev[y];
+    o.n_prev = n_prev[y];
+    o.now = now[y];
+    o.n_now = n_now[y];
+    o.n = n_prev[y] + n_now[y];
+    o.out = y == 0 ? changes : nullptr;
+    o.ctrl = &ctrl;
+    if (y == 1) o.k0 = {keys[0], n_keys[0], f[0], keys[1], n_keys[1], f[1], nullptr};
+    if (y == 2) o.k1 = {keys[2], n_keys[2], f[2], keys[3], n_keys[3], f[3], nullptr};
+    o.tag = tag;
+    cols = max(cols, (o.n + DELTA_TILE - 1) / DELTA_TILE);
+  }
+  emu_launch(k_delta_merge_shard, dim3(cols, 3), DELTA_THREADS, a, state.data());
+  DeltaListArgs la;
+  uint32_t* cnt = &ctrl.reserved2[DELTA_W_LISTS];
+  la.o[0] = {f[0], n_keys[0], tag, nullptr, dev_dirty, nullptr, cnt + 0};
+  la.o[1] = {f[1], n_keys[1], tag, keys[1], nullptr, dev_gone, cnt + 1};
+  la.o[2] = {f[2], n_keys[2], tag, nullptr, grp_dirty, nullptr, cnt + 2};
+  la.o[3] = {f[3], n_keys[3], tag, keys[3], grp_gone, nullptr, cnt + 3};
+  emu_launch(k_delta_lists, dim3(list_tiles, 4), KVG_BLOCK, la, state.data() + merge_tiles + 1, list_tiles + 1, tag + 1);
+  counts[0] = ctrl.reserved2[DELTA_W_CHANGES];
+  counts[1] = ctrl.reserved2[DELTA_W_ERROR];
+  for (int k = 0; k < 4; k++) counts[2 + k] = cnt[k];
+  return 0;
+}
+
 // prev / now: survivor lists (32-byte kvg_mdev_surv).  keys: the distinct type ids now, before, the distinct parents
 // now, before (u32 each, ascending) with their lengths in n_keys[4].  labels[0] / [1]: the new / previous dictionary
 // (label bytes, offsets, lengths, FNV-1a hashes, indexed by canonical id).  table: XMAP_SLOTS words and xlate: 65,536

@@ -1,5 +1,7 @@
 """Timing of the re-scan deltas against the plain scans on one GPU: kvg_scan_pci_delta against kvg_scan_pci
-(--kind pci, the default), kvg_scan_mdev_delta against kvg_scan_mdev (--kind mdev).
+(--kind pci, the default), kvg_scan_mdev_delta against kvg_scan_mdev (--kind mdev), and kvg_dev_scan_pci_sharded +
+kvg_dev_scan_pci_shard_fetch_delta against kvg_dev_scan_pci_sharded + kvg_dev_scan_pci_shard_fetch (--kind shard:
+one rank, world 1, over peer windows; sizes are records per rank).
 
 A sequence of snapshots changes about 0.1 % of the records per step (PCI: regroups, NUMA moves, re-binds,
 hot-removes and hot-adds in turn; mdev: retypes, NUMA moves, parent moves, destroys and hot-adds).  For each size both
@@ -7,7 +9,7 @@ entry points walk the same sequence, alternating in rounds; the host wall time o
 result on the host) is recorded.  A separate pass with kernel timing on reports the device time of the delta kernels.
 The card name and power limit are read in the same run.
 
-    python tools/time_delta.py [--kind pci|mdev] [--sizes 10000,1000000] [--steps 200] [--types 256]
+    python tools/time_delta.py [--kind pci|mdev|shard] [--sizes 10000,1000000] [--steps 200] [--types 256]
                                [--out results.json]
 """
 import argparse
@@ -31,12 +33,17 @@ import util  # noqa: E402
 
 
 def snapshots(n, ids, steps, seed=1):
+    return list(pci_sequence(n, ids, steps, seed))
+
+
+def pci_sequence(n, ids, steps, seed=1):
+    """The PCI snapshots one after the other (steps + 1 of them)."""
     rng = np.random.default_rng(seed)
     recs = O.gen_pci(seed, n, ids, 16)
     recs["addr"] = np.arange(n, dtype=np.uint32) * 4
-    out = [recs]
+    yield recs
     for s in range(steps):
-        r = out[-1].copy()
+        r = recs.copy()
         k = max(1, n // 1000)
         pick = rng.choice(np.nonzero(util.pci_alive(r))[0], k, replace=False)
         kind = s % 5
@@ -52,9 +59,10 @@ def snapshots(n, ids, steps, seed=1):
             add = r[pick].copy()
             add["addr"] += 1 + rng.integers(0, 3, k).astype(np.uint32)
             add = add[~np.isin(add["addr"], r["addr"])]
+            add = add[np.unique(add["addr"], return_index=True)[1]]   # two picks may land on one free address
             r = np.sort(np.concatenate([r, add]), order="addr", kind="stable")
-        out.append(np.ascontiguousarray(r))
-    return out
+        recs = np.ascontiguousarray(r)
+        yield recs
 
 
 def mdev_snapshots(n, steps, n_types, seed=1):
@@ -158,18 +166,91 @@ def main_mdev(a, card):
     return out
 
 
+def main_shard(a, card):
+    """Each step: the next snapshot goes to the device untimed, then scan + fetch and scan + fetch_delta on it, in
+    turn (the plain fetch leaves the delta's previous result alone)."""
+    import torch
+    text = util.pciids_text()
+    ids = O.nv_ids(text)
+    sizes = [int(x) for x in a.sizes.split(",")]
+    cap = max(sizes) + max(sizes) // 50 + 64
+    ctx = kvgpu.Context(0)
+    ctx.pciids_load(text)
+    sh = kvgpu.ShardedScan(ctx, 0, 1, lambda b, src: b, lambda b: [b], cap)
+    lib, h = ctx._lib, ctx.handle
+    buf = torch.empty(cap * 16, dtype=torch.uint8, device="cuda")
+    out = {"card": card, "kind": "shard", "world": 1, "exchange": sh.mode, "steps": a.steps, "sizes": {}}
+    res, dl = C.POINTER(L.PciShardResultC)(), C.POINTER(L.PciDeltaC)()
+
+    def plain(n):
+        t0 = time.perf_counter()
+        rc = lib.kvg_dev_scan_pci_sharded(h, buf.data_ptr(), n)
+        rc = rc or lib.kvg_dev_scan_pci_shard_fetch(h, C.byref(res))
+        t1 = time.perf_counter()
+        assert rc == 0
+        lib.kvg_result_free(res)
+        return t1 - t0
+
+    def delta(n):
+        t0 = time.perf_counter()
+        rc = lib.kvg_dev_scan_pci_sharded(h, buf.data_ptr(), n)
+        rc = rc or lib.kvg_dev_scan_pci_shard_fetch_delta(h, C.byref(res), C.byref(dl))
+        t1 = time.perf_counter()
+        assert rc == 0, (rc, lib.kvg_last_error(h))
+        n_changes = int(dl.contents.n_changes)
+        lib.kvg_result_free(res)
+        lib.kvg_result_free(dl)
+        return t1 - t0, n_changes
+
+    for n in sizes:
+        tp, td, changes, per = [], [], [], {}
+        sh.delta_reset()
+        for i, r in enumerate(pci_sequence(n, ids, a.steps + 19)):
+            buf[:r.nbytes].copy_(torch.from_numpy(r.view(np.uint8)))
+            torch.cuda.synchronize()
+            if i < 10:                           # warm-up: buffers, pinned blocks, radix hints
+                plain(len(r))
+                delta(len(r))
+                continue
+            if i >= a.steps + 10:                # the last ten steps: kernel times, in a pass of their own
+                ctx.set_kernel_timing(True)
+                delta(len(r))
+                for name, t in ctx.kernel_times():
+                    if name.startswith("shard_delta_"):
+                        per.setdefault(name, []).append(t * 1e3)
+                ctx.set_kernel_timing(False)
+                continue
+            tp.append(plain(len(r)))
+            t, c = delta(len(r))
+            td.append(t)
+            changes.append(c)
+        q = lambda v, p: round(float(np.percentile(np.array(v) * 1e6, p)), 1)
+        out["sizes"][n] = {
+            "scan_fetch_us": {"p50": q(tp, 50), "p90": q(tp, 90)},
+            "scan_fetch_delta_us": {"p50": q(td, 50), "p90": q(td, 90)},
+            "changes_per_step_median": int(np.median(changes)),
+            "kernel_us_median": {k: round(float(np.median(v)), 2) for k, v in per.items()},
+        }
+        print(n, json.dumps(out["sizes"][n]), flush=True)
+    del buf
+    torch.cuda.synchronize()
+    sh.close()
+    ctx.close()
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--sizes", default="10000,1000000")
     ap.add_argument("--steps", type=int, default=200)
     ap.add_argument("--out", help="also write the JSON result to this file")
-    ap.add_argument("--kind", choices=("pci", "mdev"), default="pci")
+    ap.add_argument("--kind", choices=("pci", "mdev", "shard"), default="pci")
     ap.add_argument("--types", type=int, default=256, help="--kind mdev: entries of the type dictionary")
     a = ap.parse_args()
     card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"],
                           capture_output=True, text=True).stdout.strip().splitlines()
-    if a.kind == "mdev":
-        out = main_mdev(a, card[0] if card else "unknown")
+    if a.kind in ("mdev", "shard"):
+        out = (main_mdev if a.kind == "mdev" else main_shard)(a, card[0] if card else "unknown")
         if a.out:
             with open(a.out, "w") as f:
                 json.dump(out, f, indent=1)
