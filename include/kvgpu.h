@@ -18,6 +18,7 @@
  *   kvg_scan_mdev_delta                   <- (no reference equivalent: createVgpuIDMap runs once)
  *   kvg_comm_*, kvg_scan_pci_sharded      <- (no reference equivalent; BASELINE.json config 4)
  *   kvg_dev_scan_pci_shard_fetch_delta    <- (no reference equivalent: the re-scan delta of the sharded scan)
+ *   kvg_dev_scan_mdev_shard_fetch_delta   <- (no reference equivalent: the re-scan delta of the sharded vGPU scan)
  *
  * Plain C: pointers + sizes only, no C++ types, no exceptions cross this boundary.
  * Return value: 0 = KVG_OK, negative = error; text via kvg_last_error().
@@ -242,7 +243,8 @@ typedef struct kvg_health_delta {
 } kvg_health_delta;
 
 /* ---- re-scan delta (K7): what changed since the previous kvg_scan_pci_delta / kvg_scan_mdev_delta
- * (kvg_pci_delta also serves kvg_dev_scan_pci_shard_fetch_delta, where "survivors" are the local shard's) */
+ * (kvg_pci_delta also serves kvg_dev_scan_pci_shard_fetch_delta and kvg_mdev_delta
+ * kvg_dev_scan_mdev_shard_fetch_delta, where "survivors" are the local shard's) */
 enum {
   KVG_CH_ADDED = 1u << 0,   /* survives now, did not before                    */
   KVG_CH_REMOVED = 1u << 1, /* survived before, does not now                    */
@@ -525,6 +527,47 @@ int kvg_dev_scan_pci_shard_delta_reset(kvg_ctx *ctx);
 /* the same for mdev records (createVgpuIDMap): type / parent orderings of the owned members */
 int kvg_dev_scan_mdev_sharded(kvg_ctx *ctx, const void *d_recs, size_t n_local, const kvg_type_dict *types);
 int kvg_dev_scan_mdev_shard_fetch(kvg_ctx *ctx, kvg_mdev_shard_result **res);
+/* Fetch the last kvg_dev_scan_mdev_sharded like kvg_dev_scan_mdev_shard_fetch, and diff it against the previous
+ * successful call of this function on this context: this rank's share of the re-scan delta of the whole snapshot.
+ *
+ * *res is byte for byte what kvg_dev_scan_mdev_shard_fetch returns for the same scan.  *res and *delta are both freed
+ * with kvg_result_free.  The call is NOT collective: it reads nothing from peers.
+ *
+ * "Previous" is the result of the last SUCCESSFUL call of this function on this context since kvg_ctx_create or
+ * kvg_dev_scan_mdev_shard_delta_reset; before any such call it is empty, so every local survivor is KVG_CH_ADDED,
+ * every owned key is dirty and nothing is gone.  The library keeps its own copy of it (the local survivors, both
+ * owned member lists, both owned key lists, the dictionary's labels and its canonical ids), separate from the other
+ * deltas': kvg_dev_scan_mdev_shard_fetch, the other scans, kvg_scan_mdev_delta, kvg_scan_pci_delta,
+ * kvg_dev_scan_pci_shard_fetch_delta and their resets, the health calls and kvg_pciids_load in between leave it
+ * unchanged, and this call leaves theirs unchanged.
+ *
+ * changes: the local shard's survivors (res->local), keyed by UUID and in ascending UUID order, diffed against the
+ * previous local list by the rules of kvg_scan_mdev_delta; type identity is the sanitised label.  A local survivor's
+ * type may be a label another rank owns, so the labels of every canonical id of both dictionaries are translated, not
+ * only this rank's keys.  now_index / prev_index index res->local / the previous local list, and n_prev is the
+ * previous local count.  A UUID that crossed a shard boundary between the two scans shows as KVG_CH_REMOVED on one
+ * rank and KVG_CH_ADDED on another; merging the ranks' changes in UUID order and fusing such pairs gives exactly the
+ * changes of kvg_scan_mdev_delta on the concatenated snapshot.
+ *
+ * type_dirty / type_gone / par_dirty / par_gone: the key rules of kvg_scan_mdev_delta applied to this rank's previous
+ * and new OWNED member lists.  type_dirty indexes res->type_keys, par_dirty res->par_keys; type_gone holds labels and
+ * par_gone parent handles.  A parent handle's owner never changes, so the par lists are exactly this rank's share of
+ * the global lists.  A vGpuMap key is owned by canonical id % nranks in each scan's own dictionary: when the
+ * dictionary renumbers, a label can move to another rank.  It is then in type_gone on its old owner and dirty on its
+ * new one, even if its members did not change, which is what a server per rank must do (stop serving the label
+ * here, start serving it there).  Outside such moves the type lists are exactly this rank's share of the global lists;
+ * the global ones follow from the merged changes alone (a key is dirty iff some merged change touches it).
+ *
+ * Precondition: survivor UUIDs ascend strictly in global Walk order (shards in rank order), and a parent handle means
+ * the same GPU in both snapshots.  The local list and both owned member lists are checked for strict ascent on the
+ * device: if that fails the call returns KVG_EINVAL (text in kvg_last_error), hands out no objects, and the previous
+ * result stays as it was; so does every error of the fetch itself (e.g. KVG_ENCCL when a peer timed out).  KVG_EINVAL
+ * when the last scan on the context was not kvg_dev_scan_mdev_sharded.
+ *
+ * Cost beyond kvg_dev_scan_mdev_shard_fetch: three kernel launches and one synchronisation. */
+int kvg_dev_scan_mdev_shard_fetch_delta(kvg_ctx *ctx, kvg_mdev_shard_result **res, kvg_mdev_delta **delta);
+/* forget the previous result: the next kvg_dev_scan_mdev_shard_fetch_delta reports everything as added */
+int kvg_dev_scan_mdev_shard_delta_reset(kvg_ctx *ctx);
 
 #ifdef __cplusplus
 }

@@ -1,5 +1,5 @@
 // kvg_delta.cuh — K7: the keyed diff of two scans (kvg_scan_pci_delta, kvg_scan_mdev_delta,
-// kvg_dev_scan_pci_shard_fetch_delta).
+// kvg_dev_scan_pci_shard_fetch_delta, kvg_dev_scan_mdev_shard_fetch_delta).
 //
 //   k_delta_merge<Tr>  merge path over the previous scan's survivors and the new ones (ascending key), one change
 //                      entry per key whose survivor differs, compacted in key order by the look-back tile body of
@@ -7,8 +7,8 @@
 //                      changes.  Also checks that the new list ascends strictly.  Tr is the record trait:
 //                      PciDeltaRec (16-byte survivors keyed by address) or MdevDeltaRec (32-byte survivors keyed by
 //                      the 128-bit big-endian UUID).
-//   k_delta_merge_shard  the same merge over a rank's three PCI lists, one per blockIdx.y: its local survivors
-//                      (change entries), the members of the device ids and of the groups it owns (key tags only)
+//   k_delta_merge_shard<Tr>  the same merge over a rank's three lists, one per blockIdx.y: its local survivors
+//                      (change entries), the members of the two kinds of keys it owns (key tags only)
 //   k_delta_lists      the four key lists (dirty / gone of both maps) from those tags: one look-back compaction per
 //                      list (blockIdx.y) through the same tile body
 //   k_mdev_delta_types the previous result's type keys in the new key space: same sanitised label, or none
@@ -153,6 +153,11 @@ struct MdevDeltaRec {
     st_stream(out + 3 * (size_t)pos, hp ? p.lo : q.lo);
     st_stream(out + 3 * (size_t)pos + 1, make_uint4(what, p.hi.x, q.hi.x, (p.hi.y & 0xffffu) | (q.hi.y << 16)));
     st_stream(out + 3 * (size_t)pos + 2, make_uint4((p.hi.y >> 16) | (q.hi.y & 0xffff0000u), b, a, 0u));
+    mark(what, hp, hn, p, q, type, par, tag);
+  }
+  // the keys alone (the sharded merge's owned lists tag keys and write no entry)
+  __device__ __forceinline__ static void mark(uint32_t what, bool hp, bool hn, const Rec& p, const Rec& q,
+                                              const DeltaKeys& type, const DeltaKeys& par, uint32_t tag) {
     if (what & (KVG_CH_ADDED | KVG_CH_REMOVED | KVG_CH_TYPE | KVG_CH_NUMA))
       type.mark<true>(hn, q.hi.y & 0xffffu, hp, p.hi.y & 0xffffu, tag);
     if (what & (KVG_CH_ADDED | KVG_CH_REMOVED | KVG_CH_PARENT)) par.mark(hn, q.hi.x, hp, p.hi.x, tag);
@@ -325,21 +330,22 @@ __global__ void __launch_bounds__(DELTA_THREADS) k_delta_merge(DeltaMergeOp<Tr> 
   lookback_tile<DeltaMergeOp<Tr>, DELTA_THREADS, DELTA_ROWS>(o, tile, n_tiles, tile_state, o.tag, s_wtot, s_woff, s_base);
 }
 
-// The sharded PCI form (kvg_dev_scan_pci_shard_fetch_delta): one merge per blockIdx.y over one pair of this rank's
-// lists, all three checked for strict ascent.
-//   y = 0  the local survivors: change entries through the look-back tile body; its DeltaKeys are empty, so it
-//          tags no key
-//   y = 1  the members of the owned device ids: deviceMap tags only (k1 empty), no entries
-//   y = 2  the members of the owned groups: iommuMap tags only (k0 empty), no entries
+// The sharded forms (kvg_dev_scan_pci_shard_fetch_delta, kvg_dev_scan_mdev_shard_fetch_delta): one merge per
+// blockIdx.y over one pair of this rank's lists, all three checked for strict ascent.
+//   y = 0  the local survivors: change entries through the look-back tile body; its DeltaKeys hold no keys, so it
+//          tags none (mdev: k0 still carries the label cross-map that KVG_CH_TYPE reads)
+//   y = 1  the members of the owned device ids / type ids: deviceMap / vGpuMap tags only (k1 empty), no entries
+//   y = 2  the members of the owned groups / parents: iommuMap / gpuVgpuMap tags only (k0 keyless), no entries
 // Each row has its own tile count and its surplus CTAs exit before any look-back.  Only row 0 takes part in one
 // (words tile_state[0 ..)), and a tile waits only on earlier tiles of that row, as in k_delta_lists.
+template <class Tr>
 struct DeltaShardArgs {
-  DeltaMergeOp<PciDeltaRec> o[3];
+  DeltaMergeOp<Tr> o[3];
 };
-__global__ void __launch_bounds__(DELTA_THREADS) k_delta_merge_shard(DeltaShardArgs args, uint64_t* tile_state) {
-  using Tr = PciDeltaRec;
+template <class Tr>
+__global__ void __launch_bounds__(DELTA_THREADS) k_delta_merge_shard(DeltaShardArgs<Tr> args, uint64_t* tile_state) {
   pdl_enter();
-  __shared__ Tr::Rec s_rec[DELTA_TILE];
+  __shared__ typename Tr::Rec s_rec[DELTA_TILE];
   __shared__ uint32_t s_code[DELTA_TILE];
   __shared__ uint32_t s_split[2];
   __shared__ uint32_t s_wtot[DELTA_THREADS / 32], s_woff[DELTA_THREADS / 32];
@@ -359,8 +365,8 @@ __global__ void __launch_bounds__(DELTA_THREADS) k_delta_merge_shard(DeltaShardA
     return;
   }
   for (uint32_t k = threadIdx.x; k < o.na + o.nb; k += DELTA_THREADS) {
-    const DeltaMergeOp<Tr>::Item it = o.load(o.d0 + k, true);
-    if (it.what) o.apply<false>(0, it, o.d0 + k);
+    const typename DeltaMergeOp<Tr>::Item it = o.load(o.d0 + k, true);
+    if (it.what) o.template apply<false>(0, it, o.d0 + k);
   }
 }
 
@@ -413,15 +419,17 @@ __global__ void __launch_bounds__(KVG_BLOCK) k_delta_lists(DeltaListArgs args, u
 
 // The previous result's type keys in the new key space.  The canonical ids of two scans are not comparable (each
 // numbers its own dictionary), labels are: xlate[c] for every previous type key c is the new type key with a
-// byte-identical label, or DELTA_NONE.  A label that is in the new dictionary without a survivor is no key and maps
-// to DELTA_NONE.  One CTA: the new keys go into an open-addressed table in global memory (slot = tag << 32 | new key
-// index; a slot holding another call's tag is empty, so the table is never cleared), then every previous key probes
-// it.  The FNV-1a hashes of k_mdev_labels place and filter; equality is decided on length and bytes.
+// byte-identical label, or DELTA_NONE.  kvg_scan_mdev_delta passes the survivors' type keys, so a label that is in
+// the new dictionary without a survivor is no key and maps to DELTA_NONE.  The sharded form passes every canonical id
+// of both dictionaries: a rank's local survivors may carry types another rank owns, so every id needs its image, and
+// DeltaKeys::mark<true> then finds the image among the rank's owned keys or not at all (gone).  One CTA: the new keys
+// go into an open-addressed table in global memory (slot = tag << 32 | new key index; a slot holding another call's
+// tag is empty, so the table is never cleared), then every previous key probes it.  The FNV-1a hashes of k_mdev_labels place and filter; equality is decided on length and bytes.
 // O(KT_prev + KT_now) expected probes.
 constexpr uint32_t XMAP_THREADS = 1024;
 constexpr uint32_t XMAP_SLOTS = 1u << 17;  // >= 2 x 65,535 type keys
 struct MdevTypeLabels {  // one dictionary: labels indexed by canonical id, and the ids that are keys
-  const uint32_t* keys;  // distinct canonical ids of the survivors, ascending
+  const uint32_t* keys;  // the canonical ids to translate (from) / to look up (into), ascending
   uint32_t n_keys;
   const uint8_t* bytes;  // label of id c at bytes + off[c], len[c] bytes
   const uint32_t* off;

@@ -11,8 +11,9 @@ from .plugin import (DiscoveryScan, Maps, MdevMapsTouched, MdevSnapshot, NvidiaG
                      mdev_maps_from_result, parse_bdf, pci_maps_from_result, plugin_specs_from_maps,
                      snapshot_mdev_tree,
                      snapshot_pci_tree)
-from .parallel import (PciShardDelta, ShardedScan, allgatherv_torch, apply_pci_shard_delta, concat_in_rank_order,
-                       mdev_maps_from_shard, merge_parts, merge_pci_shard_deltas, pci_maps_from_shard, shard_delta_part,
-                       shard_range)
+from .parallel import (MdevShardDelta, PciShardDelta, ShardedScan, allgatherv_torch, apply_mdev_shard_delta,
+                       apply_pci_shard_delta, concat_in_rank_order, mdev_maps_from_shard, mdev_shard_delta_part,
+                       merge_mdev_shard_deltas, merge_parts, merge_pci_shard_deltas, pci_maps_from_shard,
+                       shard_delta_part, shard_range)
 
 __all__ = [n for n in dir() if not n.startswith("_")]

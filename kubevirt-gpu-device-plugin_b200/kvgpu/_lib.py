@@ -189,6 +189,8 @@ def load() -> C.CDLL:
         "kvg_dev_scan_pci_shard_delta_reset": (C.c_int, [vp]),
         "kvg_dev_scan_mdev_sharded": (C.c_int, [vp, vp, sz, P(TypeDict)]),
         "kvg_dev_scan_mdev_shard_fetch": (C.c_int, [vp, P(P(MdevShardResultC))]),
+        "kvg_dev_scan_mdev_shard_fetch_delta": (C.c_int, [vp, P(P(MdevShardResultC)), P(P(MdevDeltaC))]),
+        "kvg_dev_scan_mdev_shard_delta_reset": (C.c_int, [vp]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(L, name)

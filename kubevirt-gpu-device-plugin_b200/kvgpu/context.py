@@ -302,6 +302,10 @@ class Context:
         self._ck(self._lib.kvg_scan_mdev_delta(self._h, recs.ctypes.data, len(recs), C.byref(td), C.byref(res),
                                                C.byref(dl)))
         del keep
+        delta = self._take_mdev_delta(dl)
+        return self._take_mdev(res), delta
+
+    def _take_mdev_delta(self, dl) -> MdevDelta:
         d = dl.contents
         ng = int(d.n_type_gone)
         goff = L._arr(d.type_gone_off, ng + 1, np.uint32)
@@ -312,7 +316,7 @@ class Context:
                           L._arr(d.par_dirty, int(d.n_par_dirty), np.uint32),
                           L._arr(d.par_gone, int(d.n_par_gone), np.uint32))
         self._lib.kvg_result_free(dl)
-        return self._take_mdev(res), delta
+        return delta
 
     def scan_mdev_delta_reset(self):
         self._ck(self._lib.kvg_scan_mdev_delta_reset(self._h))
@@ -444,6 +448,24 @@ class Context:
     def dev_scan_mdev_shard_fetch(self) -> MdevShardResult:
         res = C.POINTER(L.MdevShardResultC)()
         self._ck(self._lib.kvg_dev_scan_mdev_shard_fetch(self._h, C.byref(res)))
+        return self._take_mdev_shard(res)
+
+    def dev_scan_mdev_shard_fetch_delta(self):
+        """dev_scan_mdev_shard_fetch plus this rank's share of the re-scan delta, against the previous successful call
+        on this context -> (MdevShardResult, MdevDelta).  changes are the local shard's (indices into `local`),
+        type_dirty / par_dirty index the owned keys (res.by_type.type_keys / res.by_parent.par_keys), type_gone
+        (labels) / par_gone are owned keys that went; a label whose owner moved between the scans is gone on its old
+        owner and dirty on its new one.  Not collective; kvgpu.merge_mdev_shard_deltas fuses the ranks' parts."""
+        res = C.POINTER(L.MdevShardResultC)()
+        dl = C.POINTER(L.MdevDeltaC)()
+        self._ck(self._lib.kvg_dev_scan_mdev_shard_fetch_delta(self._h, C.byref(res), C.byref(dl)))
+        delta = self._take_mdev_delta(dl)
+        return self._take_mdev_shard(res), delta
+
+    def dev_scan_mdev_shard_delta_reset(self):
+        self._ck(self._lib.kvg_dev_scan_mdev_shard_delta_reset(self._h))
+
+    def _take_mdev_shard(self, res) -> MdevShardResult:
         r = res.contents
         KT, NP, nt = int(r.n_type_keys), int(r.n_parents), int(r.n_types)
         loff = L._arr(r.label_off, nt + 1, np.uint32)

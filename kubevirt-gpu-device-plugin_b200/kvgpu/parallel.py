@@ -9,7 +9,10 @@ survivor lists followed by a local select.  The pci.ids table is parsed by every
 
 Re-scan deltas (Context.dev_scan_pci_shard_fetch_delta): each rank diffs its own shard and the keys it owns with no
 communication; apply_pci_shard_delta patches its part of the maps, and merge_pci_shard_deltas over the ranks'
-shard_delta_part summaries gives the delta of the whole snapshot.
+shard_delta_part summaries gives the delta of the whole snapshot.  The mdev form (dev_scan_mdev_shard_fetch_delta,
+apply_mdev_shard_delta, mdev_shard_delta_part, merge_mdev_shard_deltas) works the same way; a vGpuMap label whose owner
+moved between two scans (the dictionary renumbered) is gone on one rank and dirty on the other, and the merge derives
+the global type lists from the fused changes.
 
 `ShardedScan` needs only byte collectives (broadcast for the 128-byte NCCL unique id, all-gather for the
 64-byte IPC handles), so the same class is driven by torch.distributed (bench.py) or any other launcher.
@@ -22,8 +25,8 @@ import numpy as np
 
 from . import _lib as L
 from .context import Context, MdevShardResult, PciResult, PciShardResult
-from .plugin import (Maps, PciMapsTouched, _fully_numeric, _patch_pci_maps, _rebuild_into, mdev_maps_from_result,
-                     pci_maps_from_result)
+from .plugin import (Maps, MdevMapsTouched, PciMapsTouched, _fully_numeric, _numeric_mdev, _patch_mdev_maps,
+                     _patch_pci_maps, _rebuild_into, mdev_maps_from_result, pci_maps_from_result)
 
 
 def shard_range(n: int, rank: int, world: int) -> tuple[int, int]:
@@ -161,6 +164,124 @@ def merge_pci_shard_deltas(parts: list) -> PciShardDelta:
                          cat("dev_gone", np.uint16), cat("grp_dirty", np.uint32), cat("grp_gone", np.uint32))
 
 
+def apply_mdev_shard_delta(part: Maps, res: MdevShardResult, delta, snap=None, prev_snap=None) -> MdevMapsTouched:
+    """Patch one rank's part of the mdev maps (mdev_maps_from_shard of its previous fetch_mdev_delta result) IN PLACE
+    into what mdev_maps_from_shard(res) builds: the owned vGpuMap / gpuVgpuMap keys that are dirty or gone, nothing
+    else.  As in apply_mdev_delta, a snapshot without canonical UUIDs and packed-BDF parents has no stable handles: the
+    part is then rebuilt (in place) and every key is reported."""
+    if not (_numeric_mdev(snap) and _numeric_mdev(prev_snap)):
+        a, b = mdev_maps_from_result(res.by_type, snap), mdev_maps_from_result(res.by_parent, snap)
+        type_gone = sorted(set(part.vGpuMap) - set(a.vGpuMap))
+        par_gone = sorted(set(part.gpuVgpuMap) - set(b.gpuVgpuMap))
+        for label in type_gone:
+            if label not in part.deviceMap:
+                part.deviceNames.pop(label, None)
+        part.vGpuMap.clear()
+        part.vGpuMap.update(a.vGpuMap)
+        part.gpuVgpuMap.clear()
+        part.gpuVgpuMap.update(b.gpuVgpuMap)
+        part.deviceNames.update(a.deviceNames)
+        return MdevMapsTouched(list(a.vGpuMap), type_gone, list(b.gpuVgpuMap), par_gone)
+    return _patch_mdev_maps(part, res.by_type, res.by_parent, delta)
+
+
+@dataclass
+class MdevShardDelta:
+    """An mdev re-scan delta with its keys as values: one rank's part (mdev_shard_delta_part; indices local to its
+    shard, key lists over the keys it owns) or the whole snapshot's (merge_mdev_shard_deltas; indices into the
+    concatenated survivor lists)."""
+    n_prev: int                 # survivors of the previous result
+    n_now: int                  # survivors now
+    changes: np.ndarray         # MDEV_CHANGE, ascending UUID
+    type_keys: np.ndarray       # u16 canonical ids of the vGpuMap keys now (a part: the ones the rank owns), ascending
+    type_dirty: np.ndarray      # u16 canonical ids (this result's dictionary) whose (uuid, numa) sequence changed
+    type_gone: list             # labels (bytes) absent now, ascending previous canonical id
+    par_dirty: np.ndarray       # u32 parent handles whose uuid sequence changed, ascending
+    par_gone: np.ndarray        # u32 parent handles absent now, ascending
+
+
+def mdev_shard_delta_part(res: MdevShardResult, delta) -> MdevShardDelta:
+    """The small summary of one rank's fetch_mdev_delta that the merge needs: counts, changes, the owned type keys and
+    the key values (no member arrays)."""
+    keys = res.by_type.type_keys.astype(np.uint16)
+    return MdevShardDelta(int(delta.n_prev), len(res.local), delta.changes, keys, keys[delta.type_dirty],
+                          list(delta.type_gone), res.by_parent.par_keys[delta.par_dirty].astype(np.uint32),
+                          np.asarray(delta.par_gone, np.uint32))
+
+
+def _canonical_ids(labels: list) -> dict:
+    """label -> canonical id (the smallest raw index with that label) of one dictionary"""
+    out = {}
+    for i, lb in enumerate(labels):
+        out.setdefault(bytes(lb), i)
+    return out
+
+
+def merge_mdev_shard_deltas(parts: list, prev_labels: list, now_labels: list) -> MdevShardDelta:
+    """The delta of the whole snapshot from the ranks' mdev_shard_delta_part summaries (rank order): equal to
+    kvg_scan_mdev_delta on the concatenated snapshot.  prev_labels / now_labels: the labels of the previous and the new
+    dictionary (MdevResult.labels; every rank loads the same dictionary).  Changes are fused as in
+    merge_pci_shard_deltas (KVG_CH_TYPE compares the labels through the two dictionaries) and come out byte for byte.
+    The vGpuMap lists follow from the fused changes by the rule of the kernels: a change dirties the label it joined,
+    and the label it left if that label is still a key somewhere (some rank owns it now), else that label is gone.  They
+    are not the union of the ranks' lists: a label that moved between ranks with unchanged members is gone on one rank
+    and dirty on the other, yet neither in the whole snapshot's delta.  Parent handles never change owner, so the
+    gpuVgpuMap lists are unions."""
+    none = np.uint32(0xFFFFFFFF)
+    prev_off = np.cumsum([0] + [p.n_prev for p in parts])
+    now_off = np.cumsum([0] + [p.n_now for p in parts])
+    chs = []
+    for r, p in enumerate(parts):
+        c = p.changes.copy()
+        c["prev_index"] = np.where(c["prev_index"] == none, none, c["prev_index"] + np.uint32(prev_off[r]))
+        c["now_index"] = np.where(c["now_index"] == none, none, c["now_index"] + np.uint32(now_off[r]))
+        chs.append(c)
+    ch = np.concatenate(chs) if chs else np.zeros(0, L.MDEV_CHANGE)
+    words = np.ascontiguousarray(ch["uuid"]).reshape(-1, 16).view(">u8").astype(np.uint64)
+    ch = ch[np.lexsort((words[:, 1], words[:, 0]))]
+    u = np.ascontiguousarray(ch["uuid"]).reshape(-1, 16)
+    dup = np.nonzero((u[1:] == u[:-1]).all(axis=1))[0]          # pairs: i (one side), i + 1 (the other)
+    prev_lab = [bytes(b) for b in prev_labels]
+    now_lab = [bytes(b) for b in now_labels]
+    if len(dup):
+        rem = (ch["what"][dup] & L.CH_REMOVED) != 0
+        gone_, new_ = ch[np.where(rem, dup, dup + 1)], ch[np.where(rem, dup + 1, dup)]
+        if not ((gone_["what"] == L.CH_REMOVED) & (new_["what"] == L.CH_ADDED)).all():
+            raise ValueError("one UUID twice, not as REMOVED + ADDED: the shards overlap")
+        f = new_.copy()
+        for side in ("prev_parent", "prev_type", "prev_numa", "prev_index"):
+            f[side] = gone_[side]
+        relabel = np.array([prev_lab[int(a)] != now_lab[int(b)] for a, b in zip(f["prev_type"], f["now_type"])], bool)
+        f["what"] = (relabel * L.CH_TYPE | (f["prev_parent"] != f["now_parent"]) * L.CH_PARENT
+                     | (f["prev_numa"] != f["now_numa"]) * L.CH_NUMA).astype(np.uint32)
+        keep = np.ones(len(ch), dtype=bool)
+        keep[dup + 1] = False
+        ch[dup] = f
+        keep[dup[f["what"] == 0]] = False
+        ch = ch[keep]
+    type_keys = np.unique(np.concatenate([p.type_keys for p in parts] + [np.zeros(0, np.uint16)])).astype(np.uint16)
+    now_id = _canonical_ids(now_lab)
+    live = set(type_keys.tolist())
+    dirty, gone = set(), set()
+    for c in ch[(ch["what"] & (L.CH_ADDED | L.CH_REMOVED | L.CH_TYPE | L.CH_NUMA)) != 0]:
+        has_now, has_prev = c["now_index"] != none, c["prev_index"] != none
+        if has_now:
+            dirty.add(int(c["now_type"]))
+        if has_prev:
+            label = prev_lab[int(c["prev_type"])]
+            if has_now and label == now_lab[int(c["now_type"])]:
+                continue
+            same = now_id.get(label)
+            if same is not None and same in live:
+                dirty.add(same)
+            else:
+                gone.add(int(c["prev_type"]))
+    cat = lambda name: np.unique(np.concatenate([getattr(p, name) for p in parts] + [np.zeros(0, np.uint32)]))
+    return MdevShardDelta(int(prev_off[-1]), int(now_off[-1]), np.ascontiguousarray(ch), type_keys,
+                          np.array(sorted(dirty), np.uint16), [prev_lab[c] for c in sorted(gone)],
+                          cat("par_dirty").astype(np.uint32), cat("par_gone").astype(np.uint32))
+
+
 def merge_parts(parts: list) -> Maps:
     """Union of the ranks' parts (rank order): key sets are disjoint, bdfToIommuMap concatenates in rank
     order == Walk order."""
@@ -186,6 +307,7 @@ class ShardedScan:
         path is used."""
         self.ctx, self.rank, self.world = ctx, rank, world
         self._bcast, self._allgather = broadcast_bytes, allgather_bytes
+        self.mdev_prev_labels, self.mdev_labels = [], []   # dictionaries of the last fetch_mdev_delta: before, now
         self.mode = "nccl"
         uid = ctx.comm_unique_id() if rank == 0 else None
         uid = broadcast_bytes(uid, 0)
@@ -246,6 +368,33 @@ class ShardedScan:
 
     def fetch_mdev(self) -> MdevShardResult:
         return self.ctx.dev_scan_mdev_shard_fetch()
+
+    def fetch_mdev_delta(self):
+        """fetch_mdev plus this rank's share of the mdev re-scan delta -> (MdevShardResult, MdevDelta), see
+        Context.dev_scan_mdev_shard_fetch_delta.  Collective here exactly like fetch_delta: if any rank's call failed,
+        EVERY rank resets its previous result and raises KvgError.  The labels of the dictionary the delta was taken
+        against are kept, so that merge_mdev_deltas needs only the ranks' parts."""
+        err, out = None, None
+        try:
+            out = self.ctx.dev_scan_mdev_shard_fetch_delta()
+        except L.KvgError as e:
+            err = e
+        if all(s[:1] == b"\1" for s in self._statuses(b"\0" if err else b"\1")):
+            self.mdev_prev_labels, self.mdev_labels = self.mdev_labels, list(out[0].by_type.labels)
+            return out
+        self.mdev_delta_reset()
+        if err is not None:
+            raise err
+        raise L.KvgError(L.KVG_ESTATE, "fetch_mdev_delta failed on another rank; every rank's previous result is reset")
+
+    def mdev_delta_reset(self):
+        """Forget this rank's previous mdev result (call it on every rank)."""
+        self.ctx.dev_scan_mdev_shard_delta_reset()
+        self.mdev_labels = []
+
+    def merge_mdev_deltas(self, parts: list) -> MdevShardDelta:
+        """merge_mdev_shard_deltas of the ranks' parts of the last fetch_mdev_delta, with the labels it kept."""
+        return merge_mdev_shard_deltas(parts, self.mdev_prev_labels, self.mdev_labels)
 
     def close(self):
         self.ctx.comm_destroy()

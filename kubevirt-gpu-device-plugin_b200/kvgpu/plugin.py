@@ -507,14 +507,20 @@ def apply_mdev_delta(maps: Maps, res: MdevResult, delta, snap: MdevSnapshot | No
     not packed BDFs has no stable handles: the maps are then rebuilt (in place as well) and every key is reported."""
     if not (_numeric_mdev(snap) and _numeric_mdev(prev_snap)):
         return _rebuild_mdev_maps(maps, res, snap)
-    s = res.survivors
+    return _patch_mdev_maps(maps, res, res, delta)
+
+
+def _patch_mdev_maps(maps: Maps, by_type: MdevResult, by_par: MdevResult, delta) -> MdevMapsTouched:
+    """The numeric patch of apply_mdev_delta: vGpuMap keys from `by_type`, gpuVgpuMap keys from `by_par` (each result's
+    permutation indexes its own survivors)."""
     t = MdevMapsTouched([], [], [], [])
+    s = by_type.survivors
     for k in delta.type_dirty:
-        c = int(res.type_keys[k])
-        label = res.labels[c].decode("latin-1")
-        idx = res.type_perm[res.type_off[k]:res.type_off[k + 1]]
+        c = int(by_type.type_keys[k])
+        label = by_type.labels[c].decode("latin-1")
+        idx = by_type.type_perm[by_type.type_off[k]:by_type.type_off[k + 1]]
         maps.vGpuMap[label] = [NvidiaGpuDevice(format_uuid(s["uuid"][i]), int(s["numa"][i])) for i in idx]
-        maps.deviceNames[label] = res.type_names[c]
+        maps.deviceNames[label] = by_type.type_names[c]
         t.type_dirty.append(label)
     for g in delta.type_gone:
         label = g.decode("latin-1")
@@ -522,9 +528,10 @@ def apply_mdev_delta(maps: Maps, res: MdevResult, delta, snap: MdevSnapshot | No
         if label not in maps.deviceMap:
             maps.deviceNames.pop(label, None)
         t.type_gone.append(label)
+    s = by_par.survivors
     for k in delta.par_dirty:
-        key = format_bdf(int(res.par_keys[k]))
-        idx = res.par_perm[res.par_off[k]:res.par_off[k + 1]]
+        key = format_bdf(int(by_par.par_keys[k]))
+        idx = by_par.par_perm[by_par.par_off[k]:by_par.par_off[k + 1]]
         maps.gpuVgpuMap[key] = [format_uuid(s["uuid"][i]) for i in idx]
         t.par_dirty.append(key)
     for p in delta.par_gone:

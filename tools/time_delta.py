@@ -1,7 +1,9 @@
 """Timing of the re-scan deltas against the plain scans on one GPU: kvg_scan_pci_delta against kvg_scan_pci
 (--kind pci, the default), kvg_scan_mdev_delta against kvg_scan_mdev (--kind mdev), and kvg_dev_scan_pci_sharded +
 kvg_dev_scan_pci_shard_fetch_delta against kvg_dev_scan_pci_sharded + kvg_dev_scan_pci_shard_fetch (--kind shard:
-one rank, world 1, over peer windows; sizes are records per rank).
+one rank, world 1, over peer windows; sizes are records per rank), and the same for the sharded mdev scan
+(--kind mdev-shard: kvg_dev_scan_mdev_sharded + kvg_dev_scan_mdev_shard_fetch_delta against
+kvg_dev_scan_mdev_sharded + kvg_dev_scan_mdev_shard_fetch).
 
 A sequence of snapshots changes about 0.1 % of the records per step (PCI: regroups, NUMA moves, re-binds,
 hot-removes and hot-adds in turn; mdev: retypes, NUMA moves, parent moves, destroys and hot-adds).  For each size both
@@ -9,7 +11,7 @@ entry points walk the same sequence, alternating in rounds; the host wall time o
 result on the host) is recorded.  A separate pass with kernel timing on reports the device time of the delta kernels.
 The card name and power limit are read in the same run.
 
-    python tools/time_delta.py [--kind pci|mdev|shard] [--sizes 10000,1000000] [--steps 200] [--types 256]
+    python tools/time_delta.py [--kind pci|mdev|shard|mdev-shard] [--sizes 10000,1000000] [--steps 200] [--types 256]
                                [--out results.json]
 """
 import argparse
@@ -239,18 +241,92 @@ def main_shard(a, card):
     return out
 
 
+def main_mdev_shard(a, card):
+    """As main_shard, over the mdev snapshots of main_mdev (an mdev record takes two PCI records of window)."""
+    import torch
+    sizes = [int(x) for x in a.sizes.split(",")]
+    cap = 2 * (max(sizes) + max(sizes) // 50 + 64)
+    ctx = kvgpu.Context(0)
+    ctx.pciids_load(util.pciids_text())
+    sh = kvgpu.ShardedScan(ctx, 0, 1, lambda b, src: b, lambda b: [b], cap)
+    lib, h = ctx._lib, ctx.handle
+    types = [b"GRID T%05d\n" % k for k in range(a.types)]
+    td_c, keep = ctx._type_dict(types)
+    buf = torch.empty(cap * 16, dtype=torch.uint8, device="cuda")
+    out = {"card": card, "kind": "mdev-shard", "world": 1, "exchange": sh.mode, "steps": a.steps, "types": a.types,
+           "sizes": {}}
+    res, dl = C.POINTER(L.MdevShardResultC)(), C.POINTER(L.MdevDeltaC)()
+
+    def plain(n):
+        t0 = time.perf_counter()
+        rc = lib.kvg_dev_scan_mdev_sharded(h, buf.data_ptr(), n, C.byref(td_c))
+        rc = rc or lib.kvg_dev_scan_mdev_shard_fetch(h, C.byref(res))
+        t1 = time.perf_counter()
+        assert rc == 0, (rc, lib.kvg_last_error(h))
+        lib.kvg_result_free(res)
+        return t1 - t0
+
+    def delta(n):
+        t0 = time.perf_counter()
+        rc = lib.kvg_dev_scan_mdev_sharded(h, buf.data_ptr(), n, C.byref(td_c))
+        rc = rc or lib.kvg_dev_scan_mdev_shard_fetch_delta(h, C.byref(res), C.byref(dl))
+        t1 = time.perf_counter()
+        assert rc == 0, (rc, lib.kvg_last_error(h))
+        n_changes = int(dl.contents.n_changes)
+        lib.kvg_result_free(res)
+        lib.kvg_result_free(dl)
+        return t1 - t0, n_changes
+
+    for n in sizes:
+        tp, td, changes, per = [], [], [], {}
+        sh.mdev_delta_reset()
+        for i, r in enumerate(mdev_snapshots(n, a.steps + 19, a.types)):
+            buf[:r.nbytes].copy_(torch.from_numpy(r.view(np.uint8).ravel()))
+            torch.cuda.synchronize()
+            if i < 10:                           # warm-up: buffers, pinned blocks, radix hints
+                plain(len(r))
+                delta(len(r))
+                continue
+            if i >= a.steps + 10:                # the last ten steps: kernel times, in a pass of their own
+                ctx.set_kernel_timing(True)
+                delta(len(r))
+                for name, t in ctx.kernel_times():
+                    if name.startswith("shard_mdev_delta_"):
+                        per.setdefault(name, []).append(t * 1e3)
+                ctx.set_kernel_timing(False)
+                continue
+            tp.append(plain(len(r)))
+            t, c = delta(len(r))
+            td.append(t)
+            changes.append(c)
+        q = lambda v, p: round(float(np.percentile(np.array(v) * 1e6, p)), 1)
+        out["sizes"][n] = {
+            "scan_fetch_us": {"p50": q(tp, 50), "p90": q(tp, 90)},
+            "scan_fetch_delta_us": {"p50": q(td, 50), "p90": q(td, 90)},
+            "changes_per_step_median": int(np.median(changes)),
+            "kernel_us_median": {k: round(float(np.median(v)), 2) for k, v in per.items()},
+        }
+        print(n, json.dumps(out["sizes"][n]), flush=True)
+    del keep, buf
+    torch.cuda.synchronize()
+    sh.close()
+    ctx.close()
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--sizes", default="10000,1000000")
     ap.add_argument("--steps", type=int, default=200)
     ap.add_argument("--out", help="also write the JSON result to this file")
-    ap.add_argument("--kind", choices=("pci", "mdev", "shard"), default="pci")
-    ap.add_argument("--types", type=int, default=256, help="--kind mdev: entries of the type dictionary")
+    ap.add_argument("--kind", choices=("pci", "mdev", "shard", "mdev-shard"), default="pci")
+    ap.add_argument("--types", type=int, default=256, help="--kind mdev / mdev-shard: entries of the type dictionary")
     a = ap.parse_args()
     card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"],
                           capture_output=True, text=True).stdout.strip().splitlines()
-    if a.kind in ("mdev", "shard"):
-        out = (main_mdev if a.kind == "mdev" else main_shard)(a, card[0] if card else "unknown")
+    if a.kind in ("mdev", "shard", "mdev-shard"):
+        run = {"mdev": main_mdev, "shard": main_shard, "mdev-shard": main_mdev_shard}[a.kind]
+        out = run(a, card[0] if card else "unknown")
         if a.out:
             with open(a.out, "w") as f:
                 json.dump(out, f, indent=1)
