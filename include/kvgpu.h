@@ -14,6 +14,8 @@
  *                                            (+ readVgpuIDFromFileFunc label rule :334-344, join :152-155)
  *   kvg_health_rescan                     <- health flips fed to ListAndWatch
  *                                            generic_device_plugin.go:325-342, :611-690
+ *   kvg_health_rescan_mdev                <- the vGPU health check: device-path Create / Remove / Rename and
+ *                                            NVML XID critical errors, generic_vgpu_device_plugin.go:280-385
  *   kvg_scan_pci_delta                    <- (no reference equivalent: the reference never re-scans)
  *   kvg_scan_mdev_delta                   <- (no reference equivalent: createVgpuIDMap runs once)
  *   kvg_comm_*, kvg_scan_pci_sharded      <- (no reference equivalent; BASELINE.json config 4)
@@ -359,6 +361,37 @@ int kvg_scan_mdev(kvg_ctx *ctx, const kvg_mdev_rec *recs, size_t n, const kvg_ty
  * not checked.  Pageable memory is staged and has no alignment requirement. */
 int kvg_health_rescan(kvg_ctx *ctx, const kvg_pci_rec *recs, size_t n, kvg_health_delta **delta);
 int kvg_health_reset(kvg_ctx *ctx);
+
+/* Health re-scan of mdev records: a vGPU is healthy while its record is present (createVgpuIDMap's keep rule) and not
+ * marked by a critical XID on its parent GPU.
+ *
+ * `xid_parents` holds the parent handles (kvg_mdev_rec.parent) of the GPUs that reported an XID since the previous
+ * call: a one-shot list of events, not a standing set.  Order and duplicates do not matter; membership is exact
+ * uint32 equality, so a handle no record carries marks nothing.  Record i keeps two bits from the previous call, p
+ * (present) and m (marked), m implies p:
+ *
+ *   p' = record i passes createVgpuIDMap's keep rule with n_types dictionary entries
+ *   m' = p' && (parent(i) in xid_parents || (p && m))
+ *   healthy before h = p && !m, healthy now h' = p' && !m'; i is listed iff h' != h
+ *
+ * So a mark stays until the record vanishes; a vGPU that comes back is healthy unless its parent is in xid_parents on
+ * that same call (generic_vgpu_device_plugin.go:330-351: only a Create sends `healthy`).  The delta is
+ * kvg_health_delta: n_alive counts the records healthy now, changed[] holds (index << 1) | healthy_now in ascending
+ * index order.
+ *
+ * A call with a different n re-arms the state to "nothing present, nothing marked", as does kvg_health_mdev_reset();
+ * n = 0 returns an empty delta.  n_xid > KVG_HEALTH_MAX_XID, or xid_parents == NULL with n_xid > 0, returns
+ * KVG_EINVAL and leaves the state unchanged.  The state is the context's own, separate from kvg_health_rescan's:
+ * kvg_health_rescan, kvg_health_reset, every scan, every delta and kvg_pciids_load leave it unchanged, and this call
+ * leaves theirs unchanged.
+ *
+ * Up to 32,768 records and with kernel timing off, the call is one kernel launch with no driver synchronisation on the
+ * way back; pinned `recs` are then read in place and must be 16-byte aligned (not checked).  Pageable memory is staged
+ * and has no alignment requirement. */
+#define KVG_HEALTH_MAX_XID 1024 /* parent handles per call */
+int kvg_health_rescan_mdev(kvg_ctx *ctx, const kvg_mdev_rec *recs, size_t n, uint32_t n_types,
+                           const uint32_t *xid_parents, size_t n_xid, kvg_health_delta **delta);
+int kvg_health_mdev_reset(kvg_ctx *ctx);
 
 /* Scan `recs` and diff the result against the previous one, keyed by survivor address.
  *

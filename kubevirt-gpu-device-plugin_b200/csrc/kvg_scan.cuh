@@ -7,6 +7,8 @@
 //        PciClassifyOp       createIommuDeviceMap's filter (device_plugin.go:201-244) + name join
 //        MdevClassifyOp      createVgpuIDMap's filter (:268-289)
 //        HealthOp            K6: alive-set diff against the previous scan
+//        MdevHealthOp        K6 for vGPUs: present / XID-marked state diff
+//   k_health_small<Rec>    K6 at poll-loop sizes: one CTA, TMA-staged, transitions into mapped host memory
 //   k_mdev_labels / _canon K5: label rule (:341-342) + merge of equal labels
 //   k_gen_*                counter-based synthetic snapshots (twins of oracle/kvg_oracle.c kvo_gen_*)
 #pragma once
@@ -47,9 +49,13 @@ struct ScanCtrl {
 //   (no ticket needed).  One CTA per tile measured about 5 % slower at 4 Mi records (39.5 against 37.7 us, H100 SXM
 //   with a 400 W power limit).
 // ------------------------------------------------------------------------------------------------
+// An operator that keeps a per-CTA table in shared memory fills it in an overload of compact_enter (MdevHealthOp).
+template <class Op>
+__device__ __forceinline__ void compact_enter(Op&) {}
 template <class Op, int THREADS, int ROWS>
 __global__ void __launch_bounds__(THREADS) k_compact(Op op, uint64_t* tile_state, uint32_t epoch) {
   pdl_enter();
+  compact_enter(op);
   lookback_tiles<Op, THREADS, ROWS>(op, tile_state, epoch);
 }
 
@@ -146,6 +152,12 @@ __global__ void __launch_bounds__(KVG_BLOCK) k_join_names(uint4* __restrict__ re
 struct MdevItem {
   uint4 lo, hi;
 };
+// createVgpuIDMap's keep rule (:270-279): the type and the parent were read, and the type is in the dictionary.
+// hi = {parent, type_idx | flags<<16 | pad<<24, parent_numa | pad.., pad}
+__device__ __forceinline__ bool mdev_record_alive(const uint4& hi, uint32_t n_types) {
+  const uint32_t flags = (hi.y >> 16) & 0xffu;
+  return (flags & (KVG_MF_TYPE_ERR | KVG_MF_PARENT_ERR)) == 0 && (hi.y & 0xffffu) < n_types;
+}
 struct MdevClassifyOp : SurvivorOp<MdevClassifyOp> {
   using Item = MdevItem;
   static constexpr int UNITS = 2;  // 16-byte units per survivor
@@ -165,12 +177,7 @@ struct MdevClassifyOp : SurvivorOp<MdevClassifyOp> {
     }
     return it;
   }
-  // hi = {parent, type_idx | flags<<16 | pad<<24, parent_numa | pad.., pad}
-  __device__ __forceinline__ bool pred(const Item& r, uint32_t) const {
-    uint32_t flags = (r.hi.y >> 16) & 0xffu;
-    uint32_t type_idx = r.hi.y & 0xffffu;
-    return (flags & (KVG_MF_TYPE_ERR | KVG_MF_PARENT_ERR)) == 0 && type_idx < n_types;
-  }
+  __device__ __forceinline__ bool pred(const Item& r, uint32_t) const { return mdev_record_alive(r.hi, n_types); }
   __device__ __forceinline__ uint32_t prepare(const Item& r) const { return type_canon[r.hi.y & 0xffffu]; }
   // the survivor record (kvgpu.h kvg_mdev_surv)
   __device__ __forceinline__ void make(const Item& r, uint32_t i, uint32_t canon, uint4* s) const {
@@ -220,30 +227,134 @@ struct HealthOp {
   __device__ __forceinline__ void finish(uint32_t total) { ctrl->n_changed = total; }
 };
 
+// ---- K6 for vGPUs: health = present and not marked by a critical XID on the parent GPU -------------------------------
+// Per record two bits, p (present: mdev_record_alive) and m (marked), m => p.  A tick with the sorted, deduplicated
+// parent handles X:  p' = alive,  m' = p' && (parent in X || (p && m)),  healthy = p && !m.  The state byte keeps them
+// as bit 0 = healthy (p && !m), bit 1 = marked (p && m), so that bit 0 is the health in every K6 state byte.
+constexpr uint32_t HEALTH_MDEV_HEALTHY = 1u, HEALTH_MDEV_MARKED = 2u;
+// membership in the sorted set xs[0..n), n <= KVG_HEALTH_MAX_XID: lo = the last position whose value is <= v, found
+// by 10 fixed steps (no data-dependent trip count), then one compare; nothing is loaded when n == 0
+__device__ __forceinline__ bool sorted_has(const uint32_t* xs, uint32_t n, uint32_t v) {
+  static_assert(KVG_HEALTH_MAX_XID == 1024, "10 steps");
+  if (n == 0) return false;
+  uint32_t lo = 0;
+#pragma unroll
+  for (uint32_t step = KVG_HEALTH_MAX_XID / 2; step; step >>= 1)
+    if (lo + step < n && xs[lo + step] <= v) lo += step;
+  return xs[lo] == v;
+}
+__device__ __forceinline__ uint32_t health_mdev_next(const uint4& hi, uint32_t s, uint32_t n_types, const uint32_t* xs,
+                                                     uint32_t n_xid) {
+  if (!mdev_record_alive(hi, n_types)) return 0;
+  const bool marked = (s & HEALTH_MDEV_MARKED) || sorted_has(xs, n_xid, hi.x);
+  return marked ? HEALTH_MDEV_MARKED : HEALTH_MDEV_HEALTHY;
+}
+// every thread of the CTA copies its share of X into shared memory (the caller synchronises before the first use)
+__device__ __forceinline__ void load_xid_set(uint32_t* dst, const uint32_t* src, uint32_t n_xid) {
+  for (uint32_t k = threadIdx.x; k < n_xid; k += blockDim.x) dst[k] = src[k];
+}
+
+// the look-back form (above HEALTH_SMALL_MAX records, or with kernel timing on): k_compact<MdevHealthOp, 256, 8>.
+// Item.x = new state | old state << 2; the state byte is written whenever it changes, a transition or not (a marked
+// vGPU that vanishes loses its mark without a health change).
+struct MdevHealthOp {
+  using Item = uint4;
+  const uint4* recs;  // 2 x uint4 per record
+  uint32_t n;
+  uint32_t n_types;
+  const uint32_t* xid;  // X in device memory, copied into s_xid by enter()
+  uint32_t n_xid;
+  const uint32_t* s_xid;
+  uint8_t* state;  // one byte per record, updated in place
+  uint32_t* changed;
+  ScanCtrl* ctrl;
+  uint32_t local_alive;
+  __device__ __forceinline__ void enter() {
+    __shared__ uint32_t s_set[KVG_HEALTH_MAX_XID];
+    load_xid_set(s_set, xid, n_xid);
+    s_xid = s_set;
+    __syncthreads();
+  }
+  __device__ __forceinline__ uint32_t prepare(const Item&) const { return 0; }
+  __device__ __forceinline__ Item load(uint32_t i, bool ok) const {
+    if (!ok) return make_uint4(0, 0, 0, 0);
+    uint4 r = ld_stream(recs + 2 * (size_t)i + 1);
+    const uint32_t s = state[i];
+    r.x = health_mdev_next(r, s, n_types, s_xid, n_xid) | (s << 2);
+    return r;
+  }
+  __device__ __forceinline__ bool pred(const Item& r, uint32_t i) {
+    const uint32_t now = r.x & 3u, was = r.x >> 2;
+    if (now != was) state[i] = (uint8_t)now;
+    local_alive += now & 1u;
+    return ((now ^ was) & 1u) != 0;
+  }
+  __device__ __forceinline__ void emit(uint32_t pos, const Item& r, uint32_t i, uint32_t) {
+    changed[pos] = (i << 1) | (r.x & 1u);
+  }
+  __device__ __forceinline__ void tile_epilogue() {
+    uint32_t a = warp_sum(local_alive);
+    if (lane_id() == 0 && a) atomicAdd(&ctrl->n_alive, a);
+    local_alive = 0;
+  }
+  __device__ __forceinline__ void finish(uint32_t total) { ctrl->n_changed = total; }
+};
+__device__ __forceinline__ void compact_enter(MdevHealthOp& op) { op.enter(); }
+
 // K6 at poll-loop sizes (BASELINE.json config 5: 10,000 devices at 1 kHz): ONE CTA, one launch, one host
 // synchronisation.  The records are read where the host left them (mapped pinned memory: zero-copy over PCIe,
 // every load of a thread in flight at once), the transitions are written — in record order — straight into
 // the host-visible result block, and the two counters follow.  No staging copy, no look-back, no second
 // device-to-host copy.
+//   Rec (the record operator) says what a record is and how its state byte moves; bit 0 of a state byte is the
+//   health the transition list reports:
+//     UNITS, STAGE_ROWS       16-byte units per record, rows of 1024 records per 192 KiB TMA round
+//     SMEM                    dynamic shared memory: the stage, then whatever enter() keeps
+//     enter(smem)             once per CTA before the first round (every thread; a __syncthreads follows)
+//     next(rec, s, smem)      the state byte after this tick from the staged record and the previous byte
 constexpr uint32_t HEALTH_SMALL_THREADS = 1024;
 constexpr uint32_t HEALTH_SMALL_ROWS = 32;                                        // rows of 1024 records
 constexpr uint32_t HEALTH_SMALL_MAX = HEALTH_SMALL_THREADS * HEALTH_SMALL_ROWS;  // 32,768 records
-constexpr uint32_t HEALTH_STAGE_ROWS = 12;                                        // rows staged per round
-constexpr uint32_t HEALTH_SMALL_SMEM = HEALTH_STAGE_ROWS * HEALTH_SMALL_THREADS * 16;  // 192 KiB
-__global__ void __launch_bounds__(HEALTH_SMALL_THREADS) k_health_small(const uint4* __restrict__ recs, uint32_t n,
-                                                                       uint8_t* __restrict__ alive_prev,
+constexpr uint32_t HEALTH_STAGE_BYTES = 192u << 10;                               // one TMA round
+// PCI: 16-byte records, 12 rows per round, state = alive (0 / 1)
+struct PciHealthRec {
+  static constexpr uint32_t UNITS = 1, STAGE_ROWS = 12;
+  static constexpr uint32_t SMEM = STAGE_ROWS * HEALTH_SMALL_THREADS * 16 * UNITS;
+  __device__ __forceinline__ void enter(uint8_t*) const {}
+  __device__ __forceinline__ uint32_t next(const uint4* r, uint32_t, const uint8_t*) const {
+    return pci_record_alive(r[0]) ? 1u : 0u;
+  }
+};
+// mdev: 32-byte records, 6 rows per round, state = healthy | marked << 1, X kept in shared memory behind the stage
+struct MdevHealthRec {
+  static constexpr uint32_t UNITS = 2, STAGE_ROWS = 6;
+  static constexpr uint32_t XID_AT = STAGE_ROWS * HEALTH_SMALL_THREADS * 16 * UNITS;
+  static constexpr uint32_t SMEM = XID_AT + KVG_HEALTH_MAX_XID * 4;
+  const uint32_t* xid;  // X in the mapped result block
+  uint32_t n_xid, n_types;
+  __device__ __forceinline__ void enter(uint8_t* smem) const {
+    load_xid_set(reinterpret_cast<uint32_t*>(smem + XID_AT), xid, n_xid);
+  }
+  __device__ __forceinline__ uint32_t next(const uint4* r, uint32_t s, const uint8_t* smem) const {
+    return health_mdev_next(r[1], s, n_types, reinterpret_cast<const uint32_t*>(smem + XID_AT), n_xid);
+  }
+};
+static_assert(PciHealthRec::SMEM == HEALTH_STAGE_BYTES && MdevHealthRec::XID_AT == HEALTH_STAGE_BYTES, "one round");
+template <class Rec>
+__global__ void __launch_bounds__(HEALTH_SMALL_THREADS) k_health_small(Rec op, const uint4* __restrict__ recs, uint32_t n,
+                                                                       uint8_t* __restrict__ state,
                                                                        uint32_t* __restrict__ changed_host,
                                                                        uint32_t* __restrict__ hdr_host, uint32_t seq) {
   pdl_enter();
-  constexpr uint32_t NW = HEALTH_SMALL_THREADS / 32;
+  constexpr uint32_t NW = HEALTH_SMALL_THREADS / 32, U = Rec::UNITS, SR = Rec::STAGE_ROWS;
 #ifndef KVG_HOST_EMU
   extern __shared__ __align__(128) uint8_t hs_smem[];
 #else
-  static __attribute__((aligned(128))) uint8_t hs_smem[HEALTH_SMALL_SMEM];
+  static __attribute__((aligned(128))) uint8_t hs_smem[Rec::SMEM];
 #endif
   __shared__ __align__(8) uint64_t s_bar;
   __shared__ uint32_t s_bal[HEALTH_SMALL_ROWS][NW];  // "changed" ballot of (row, warp) -> its position in the list
-  __shared__ uint32_t s_now[HEALTH_SMALL_ROWS][NW];  // "alive now" ballot of (row, warp)
+  __shared__ uint32_t s_now[HEALTH_SMALL_ROWS][NW];  // "healthy now" ballot of (row, warp)
   __shared__ uint32_t s_scan[NW], s_alv[NW];
   const uint4* stage = reinterpret_cast<const uint4*>(hs_smem);
   const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -252,34 +363,38 @@ __global__ void __launch_bounds__(HEALTH_SMALL_THREADS) k_health_small(const uin
     mbar_init(&s_bar, 1);
     mbar_fence_init();
   }
+  op.enter(hs_smem);
   __syncthreads();
   uint32_t n_alive = 0, phase = 0;
-  for (uint32_t r0 = 0; r0 < rows; r0 += HEALTH_STAGE_ROWS) {
+  for (uint32_t r0 = 0; r0 < rows; r0 += SR) {
     // the whole round (<= 192 KiB of the snapshot) is requested at once by the TMA unit: over PCIe what counts
     // is bytes in flight, and a bulk copy keeps them in flight without a register per load
     const uint32_t first = r0 * HEALTH_SMALL_THREADS;
-    const uint32_t cnt = min(n - first, HEALTH_STAGE_ROWS * HEALTH_SMALL_THREADS);
+    const uint32_t cnt = min(n - first, SR * HEALTH_SMALL_THREADS);
     if (tid == 0) {
-      mbar_arrive_expect_tx(&s_bar, cnt * 16);
-      for (uint32_t off = 0; off < cnt * 16; off += 16384)
-        tma_load_1d(hs_smem + off, reinterpret_cast<const uint8_t*>(recs + first) + off, min(16384u, cnt * 16 - off), &s_bar);
+      mbar_arrive_expect_tx(&s_bar, cnt * 16 * U);
+      for (uint32_t off = 0; off < cnt * 16 * U; off += 16384)
+        tma_load_1d(hs_smem + off, reinterpret_cast<const uint8_t*>(recs + first * U) + off,
+                    min(16384u, cnt * 16 * U - off), &s_bar);
     }
-    uint32_t was[HEALTH_STAGE_ROWS];
+    uint32_t was[SR];
 #pragma unroll
-    for (uint32_t k = 0; k < HEALTH_STAGE_ROWS; k++) {  // the previous state (device memory) meanwhile
+    for (uint32_t k = 0; k < SR; k++) {  // the previous state (device memory) meanwhile
       const uint32_t i = first + k * HEALTH_SMALL_THREADS + tid;
-      was[k] = i < n ? alive_prev[i] : 0;
+      was[k] = i < n ? state[i] : 0;
     }
     mbar_wait(&s_bar, phase);
     phase ^= 1;
 #pragma unroll
-    for (uint32_t k = 0; k < HEALTH_STAGE_ROWS; k++) {
+    for (uint32_t k = 0; k < SR; k++) {
       if (r0 + k < rows) {  // uniform
         const uint32_t i = first + k * HEALTH_SMALL_THREADS + tid;
         const bool in = i < n;
-        const bool now = in && pci_record_alive(stage[k * HEALTH_SMALL_THREADS + tid]);
-        const bool chg = in && (now ? 1u : 0u) != was[k];
-        if (chg) alive_prev[i] = now ? 1 : 0;
+        // (lanes past n compute s from stale stage bytes and use none of it)
+        const uint32_t s = op.next(stage + (k * HEALTH_SMALL_THREADS + tid) * U, was[k], hs_smem);
+        const bool now = in && (s & 1u) != 0;
+        const bool chg = in && (now ? 1u : 0u) != (was[k] & 1u);
+        if (in && s != was[k]) state[i] = (uint8_t)s;
         const uint32_t bc = __ballot_sync(KVG_FULL, chg), bn = __ballot_sync(KVG_FULL, now);
         if (lane == 0) {
           s_bal[r0 + k][warp] = bc;

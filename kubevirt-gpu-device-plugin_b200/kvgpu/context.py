@@ -255,18 +255,35 @@ class Context:
         del keep
         return self._take_mdev(res)
 
-    def health_rescan(self, recs: np.ndarray) -> HealthDelta:
-        recs = np.ascontiguousarray(recs, dtype=L.PCI_REC)
-        res = C.POINTER(L.HealthDeltaC)()
-        self._ck(self._lib.kvg_health_rescan(self._h, recs.ctypes.data, len(recs), C.byref(res)))
+    def _take_health(self, res) -> HealthDelta:
         r = res.contents
         out = HealthDelta(int(r.n_records), int(r.n_alive),
                           L._arr(r.changed, int(r.n_changed), np.uint32))
         self._lib.kvg_result_free(res)
         return out
 
+    def health_rescan(self, recs: np.ndarray) -> HealthDelta:
+        recs = np.ascontiguousarray(recs, dtype=L.PCI_REC)
+        res = C.POINTER(L.HealthDeltaC)()
+        self._ck(self._lib.kvg_health_rescan(self._h, recs.ctypes.data, len(recs), C.byref(res)))
+        return self._take_health(res)
+
     def health_reset(self):
         self._ck(self._lib.kvg_health_reset(self._h))
+
+    def health_rescan_mdev(self, recs: np.ndarray, n_types: int, xid_parents=()) -> HealthDelta:
+        """vGPU health re-scan (include/kvgpu.h kvg_health_rescan_mdev): a record is healthy while it passes
+        createVgpuIDMap's keep rule and no XID on its parent marked it since it last appeared.  `xid_parents`: the
+        parent handles of the GPUs that reported a critical XID since the previous call (at most 1024)."""
+        recs = np.ascontiguousarray(recs, dtype=L.MDEV_REC)
+        x = np.ascontiguousarray(np.asarray(xid_parents, dtype=np.uint32).reshape(-1))
+        res = C.POINTER(L.HealthDeltaC)()
+        self._ck(self._lib.kvg_health_rescan_mdev(self._h, recs.ctypes.data, len(recs), int(n_types),
+                                                  x.ctypes.data if len(x) else None, len(x), C.byref(res)))
+        return self._take_health(res)
+
+    def health_mdev_reset(self):
+        self._ck(self._lib.kvg_health_mdev_reset(self._h))
 
     def _take_pci_delta(self, dl) -> PciDelta:
         d = dl.contents

@@ -6,6 +6,8 @@ filter / join / bucketing run in libkvgpu.so on the GPU:
     snapshot_pci_tree / snapshot_mdev_tree   the five sysfs readers (:294-357) turned into a flat
                                              record array (syscalls stay on the CPU, nothing is
                                              pre-filtered: read failures travel as flag bits)
+    snapshot_mdev_ids                        the same readers over a fixed UUID list (the vGPU
+                                             health re-scan)
     DiscoveryScan.create_iommu_device_map    createIommuDeviceMap  (:187-247)
     DiscoveryScan.create_vgpu_id_map         createVgpuIDMap       (:255-291)
     DiscoveryScan.get_device_name            getDeviceName         (:371-422)
@@ -319,6 +321,46 @@ def snapshot_mdev_tree(vgpu_base: str, pci_base: str) -> MdevSnapshot:
         recs[i]["parent"], recs[i]["type_idx"], recs[i]["flags"] = p, tidx, flags
         recs[i]["parent_numa"] = numa
     return MdevSnapshot(recs, names, raw_types, parent_names, uuid_ok)
+
+
+def snapshot_mdev_ids(vgpu_base: str, pci_base: str, uuids, intern: dict) -> MdevSnapshot:
+    """Snapshot the mdevs `uuids` in THAT order (the health re-scan's fixed record order; a Walk would re-index when
+    one vanishes, which is the very event health has to see), with the readers and flag rules of snapshot_mdev_tree.
+    A UUID whose entry is gone reads as a type error, so its record is absent.
+
+    Parent strings become handles through `intern`, a dict the caller keeps across snapshots (handles from 1; 0 = no
+    parent), so a GPU keeps its handle and an NVML bus id resolves through the same dict.  names = uuids,
+    parent_names[h] = the string of handle h."""
+    uuids = list(uuids)
+    recs = np.zeros(len(uuids), dtype=L.MDEV_REC)
+    type_ids, raw_types, uuid_ok = {}, [], True
+    for i, name in enumerate(uuids):
+        flags, tidx, parent, numa = 0, 0, "", 0
+        raw, e = _read_vgpu_raw(vgpu_base, name, "mdev_type/name")
+        if e:
+            flags |= L.MF_TYPE_ERR
+        else:
+            tidx = type_ids.setdefault(raw, len(type_ids))
+            if tidx == len(raw_types):
+                raw_types.append(raw)
+            parent, e2 = _read_gpu_id_for_vgpu(vgpu_base, name)
+            if e2:
+                flags |= L.MF_PARENT_ERR
+            else:
+                numa, e3 = _read_numa(pci_base, parent)
+                if e3:
+                    flags |= L.MF_NUMA_ERR
+        if not -32768 <= numa <= 32767:
+            raise L.KvgError(L.KVG_ERANGE, "numa_node %d of %s does not fit int16" % (numa, parent))
+        h = intern.setdefault(parent, len(intern) + 1) if parent else 0
+        hx = name.replace("-", "")
+        if len(name) == 36 and len(hx) == 32 and all(c in HEXD for c in hx) and format_uuid(bytes.fromhex(hx)) == name:
+            recs[i]["uuid"] = np.frombuffer(bytes.fromhex(hx), dtype=np.uint8)
+        else:
+            uuid_ok = False
+            recs[i]["uuid"][:4] = np.frombuffer(int(i).to_bytes(4, "big"), dtype=np.uint8)
+        recs[i]["parent"], recs[i]["type_idx"], recs[i]["flags"], recs[i]["parent_numa"] = h, tidx, flags, numa
+    return MdevSnapshot(recs, uuids, raw_types, [""] + sorted(intern, key=intern.get), uuid_ok)
 
 
 # ------------------------------------------------------------------------------------------------

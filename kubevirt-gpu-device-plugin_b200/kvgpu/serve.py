@@ -15,8 +15,8 @@ Allocate" is testable end to end in an image without a Go toolchain.
 
 Nothing here computes on the CPU what the scan computes on the GPU: the maps come from
 plugin.DiscoveryScan (libkvgpu.so); the re-validation's classification goes through
-Context.scan_pci (K3); the health feed through Context.health_rescan (K6); the hot-plug feeds through
-Context.scan_pci_delta and Context.scan_mdev_delta (K7).
+Context.scan_pci (K3); the health feeds through Context.health_rescan and Context.health_rescan_mdev (K6); the
+hot-plug feeds through Context.scan_pci_delta and Context.scan_mdev_delta (K7).
 """
 from __future__ import annotations
 
@@ -700,6 +700,95 @@ class XidEventRouter:
         if not uuid:
             return sum(self._mark(bus) for _, bus in self.gpus)
         return sum(self._mark(bus) for u, bus in self.gpus if u == uuid)
+
+
+class VgpuHealthFeed:
+    """The vGPU health check of generic_vgpu_device_plugin.go:280-385 on the GPU: periodic re-snapshot plus the XID
+    events since the last tick -> Context.health_rescan_mdev (K6) -> healthy / unhealthy events.
+
+      device path   an mdev whose entry vanishes (or stops passing createVgpuIDMap's keep rule) goes unhealthy, and
+                    healthy again when it returns (Create / Remove / Rename, :340-351)
+      XID           on_event / on_unsupported queue the bus ids of the GPUs to mark, with XidEventRouter's filters
+                    (31 / 43 / 45 ignored, no UUID = every GPU, :392-424); each vGPU on such a GPU goes unhealthy and
+                    stays so until its path is created again (:330-339)
+
+    `health_rescan_mdev(recs, n_types, xid_parents)` is Context.health_rescan_mdev; `snapshot(uuids, intern)` returns
+    an MdevSnapshot of `uuids` in that order with parent handles from `intern` (plugin.snapshot_mdev_ids over the
+    sysfs paths); `plugins` are the vGPU plugins, whose devices are the advertised UUIDs; `gpus` is [(nvml_uuid,
+    bus_id)] as in XidEventRouter.  A bus id resolves through the same intern dict as the sysfs parent strings, so
+    a bus id string that differs from the parent's sysfs name marks nothing, as the reference's map lookup misses.
+
+    tick(): snapshot, take the queued bus ids, one kernel call, then each transition to the plugin advertising that
+    UUID.  An arming tick (the first, or one whose UUID list differs from the previous tick's) resets the state and
+    sends each vGPU whose health differs from what its plugin advertises, so a vGPU already absent, or on a GPU marked
+    before the first tick, goes unhealthy at once.  Deliberate difference: only transitions are sent, where the
+    reference re-sends `unhealthy` for a vGPU already unhealthy on every repeated XID (ListAndWatch then re-sends an
+    unchanged list)."""
+
+    def __init__(self, health_rescan_mdev, snapshot, plugins, gpus, period_s: float = 0.001):
+        self.health_rescan_mdev, self.snapshot, self.period_s = health_rescan_mdev, snapshot, period_s
+        self.plugins, self.gpus = list(plugins), list(gpus)
+        self.intern = {}
+        self._uuids = None
+        self._queued = []
+        self._lock = threading.Lock()
+        self._stop = threading.Event()
+        self._thread = None
+
+    def _queue(self, buses) -> int:
+        with self._lock:
+            self._queued.extend(buses)
+        return len(buses)
+
+    def on_unsupported(self, uuid) -> int:
+        return self._queue([bus for u, bus in self.gpus if u == uuid])
+
+    def on_event(self, xid: int, uuid=None) -> int:
+        if xid in XID_APPLICATION_ERRORS:
+            return 0
+        return self._queue([bus for u, bus in self.gpus if not uuid or u == uuid])
+
+    def tick(self) -> int:
+        devs = [(d, p) for p in self.plugins for d in p.devs]
+        uuids = [d.ID for d, _ in devs]
+        snap = self.snapshot(uuids, self.intern)
+        with self._lock:
+            buses, self._queued = self._queued, []
+        xids = [self.intern[b] for b in buses if b in self.intern]
+        arming = uuids != self._uuids
+        if arming:
+            self.health_rescan_mdev(snap.recs[:0], len(snap.raw_types))    # a different n re-arms the state
+            self._uuids = uuids
+        delta = self.health_rescan_mdev(snap.recs, len(snap.raw_types), xids)
+        sent = 0
+        if arming:
+            healthy = np.zeros(len(uuids), dtype=bool)
+            ch = np.asarray(delta.changed, dtype=np.int64)
+            healthy[ch[(ch & 1) == 1] >> 1] = True
+            for k, (d, plugin) in enumerate(devs):
+                if (d.health == dpapi.HEALTHY) != healthy[k]:
+                    (plugin.healthy if healthy[k] else plugin.unhealthy)(d.ID)
+                    sent += 1
+            return sent
+        for word in delta.changed:
+            k, ok = int(word) >> 1, int(word) & 1
+            d, plugin = devs[k]
+            (plugin.healthy if ok else plugin.unhealthy)(d.ID)
+            sent += 1
+        return sent
+
+    def start(self):
+        def loop():
+            while not self._stop.is_set():
+                self.tick()
+                time.sleep(self.period_s)
+        self._thread = threading.Thread(target=loop, daemon=True)
+        self._thread.start()
+
+    def stop(self):
+        self._stop.set()
+        if self._thread:
+            self._thread.join(2.0)
 
 
 # ------------------------------------------------------------------------------------------------

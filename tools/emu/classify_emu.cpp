@@ -72,7 +72,46 @@ int emu_health_rescan(const uint4* recs, uint32_t n, uint8_t* alive_prev, uint32
 // host reads them.  hdr_out: {n_alive, n_changed}.
 int emu_health_small(const uint4* recs, uint32_t n, uint8_t* alive_prev, uint32_t* changed_out, uint32_t* hdr_out) {
   if (n == 0 || n > HEALTH_SMALL_MAX) return -1;
-  emu_launch(k_health_small, dim3(1), HEALTH_SMALL_THREADS, recs, n, alive_prev, changed_out, hdr_out, 7u);
+  emu_launch(k_health_small<PciHealthRec>, dim3(1), HEALTH_SMALL_THREADS, PciHealthRec{}, recs, n, alive_prev, changed_out,
+             hdr_out, 7u);
+  return 0;
+}
+
+// K6 for vGPUs (kvg_health_rescan_mdev), both forms on the same state bytes (bit 0 present, bit 1 marked).
+// recs: n x 32 B records; xid: the sorted, deduplicated parent handles.  Small form (n <= 32,768): hdr_out
+// {n_alive, n_changed, seq}.  Look-back form, one CTA per tile: ctrl_out {n_changed, n_alive}.
+int emu_health_mdev_small(const uint4* recs, uint32_t n, uint32_t n_types, const uint32_t* xid, uint32_t n_xid,
+                          uint8_t* state, uint32_t* changed_out, uint32_t* hdr_out) {
+  if (n == 0 || n > HEALTH_SMALL_MAX || n_xid > KVG_HEALTH_MAX_XID) return -1;
+  MdevHealthRec op;
+  op.xid = xid;
+  op.n_xid = n_xid;
+  op.n_types = n_types;
+  emu_launch(k_health_small<MdevHealthRec>, dim3(1), HEALTH_SMALL_THREADS, op, recs, n, state, changed_out, hdr_out, 9u);
+  return 0;
+}
+
+int emu_health_mdev_compact(const uint4* recs, uint32_t n, uint32_t n_types, const uint32_t* xid, uint32_t n_xid,
+                            uint8_t* state, uint32_t* changed_out, uint32_t* ctrl_out) {
+  if (n_xid > KVG_HEALTH_MAX_XID) return -1;
+  const size_t tiles = (n + C_TILE - 1) / C_TILE;
+  ScanCtrl ctrl;
+  memset(&ctrl, 0, sizeof ctrl);
+  std::vector<uint64_t> st(tiles + 4, 0);
+  MdevHealthOp op;
+  op.recs = recs;
+  op.n = n;
+  op.n_types = n_types;
+  op.xid = xid;
+  op.n_xid = n_xid;
+  op.s_xid = nullptr;
+  op.state = state;
+  op.changed = changed_out;
+  op.ctrl = &ctrl;
+  op.local_alive = 0;
+  emu_launch(k_compact<MdevHealthOp, KVG_BLOCK, C_ROWS>, dim3((unsigned)(tiles ? tiles : 1)), KVG_BLOCK, op, st.data(), 13u);
+  ctrl_out[0] = ctrl.n_changed;
+  ctrl_out[1] = ctrl.n_alive;
   return 0;
 }
 

@@ -1,0 +1,155 @@
+"""Latency of the vGPU health re-scan (kvg_health_rescan_mdev) in a 1 kHz poll loop, beside the PCI health re-scan of
+BASELINE.json config 5 (kvg_health_rescan, 10,000 records) in the same process.
+
+Each tick flips the type / parent read-error bits of 10 records of a pinned snapshot, and every 100th tick carries one
+XID parent handle.  The host wall time of each call is recorded from "snapshot in the pinned buffer" to "transitions on
+the host" (the call returns with them); 50 warm-up ticks, whose results are also checked against the numpy state
+machine of tests/health_mdev_ref.py, precede the timed ones.  Sizes up to 32,768 records run the one-CTA
+k_health_small<MdevHealthRec>; 65,536 (the config-3 vGPU count) runs k_compact<MdevHealthOp, 256, 8>.  The card's
+name, power limit and maximum SM clock are read with a read-only nvidia-smi query in the same run.
+
+    python tools/time_health_mdev.py [--sizes 10000,32768,65536] [--ticks 10000] [--out DIR]
+"""
+import argparse
+import ctypes as C
+import json
+import os
+import subprocess
+import sys
+import time
+
+import numpy as np
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, os.path.join(ROOT, "kubevirt-gpu-device-plugin_b200"))
+sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tests"))
+import kvgpu  # noqa: E402
+from oracle import oracle as O  # noqa: E402
+import health_mdev_ref  # noqa: E402
+import util  # noqa: E402
+
+WARMUP = 50
+PERIOD = 1e-3
+N_TYPES = 256
+
+
+def pinned(n, itemsize):
+    import torch
+    t = torch.empty(n * itemsize, dtype=torch.uint8, pin_memory=True)
+    return t, t.data_ptr()
+
+
+def poll_loop(call, mutate, ticks, check=None):
+    """1 kHz loop: mutate the pinned snapshot, time one call; -> latencies in us of the timed ticks."""
+    lat = []
+    t_next = time.perf_counter()
+    for tick in range(ticks + WARMUP):
+        xids = mutate(tick)
+        t0 = time.perf_counter()                        # the snapshot is in the pinned buffer
+        res = call(xids)
+        dt = time.perf_counter() - t0                   # the transitions are on the host
+        if tick < WARMUP and check is not None:
+            check(res, xids)
+        kvgpu.load().kvg_result_free(res)
+        if tick >= WARMUP:
+            lat.append(dt)
+        t_next += PERIOD
+        while time.perf_counter() < t_next:
+            pass
+    lat = np.array(lat) * 1e6
+    return {"p50_us": float(np.percentile(lat, 50)), "p99_us": float(np.percentile(lat, 99)), "max_us": float(lat.max())}
+
+
+def mdev_leg(ctx, n, ticks):
+    lib = kvgpu.load()
+    buf, ptr = pinned(n, 32)
+    view = buf.numpy().view(kvgpu.MDEV_REC)
+    view[:] = O.gen_mdev(0, n)
+    parents = np.unique(view["parent"])
+    rng = np.random.default_rng(n)
+    ref = health_mdev_ref.HealthMdevRef()
+    lib.kvg_health_mdev_reset(ctx.handle)
+
+    def mutate(tick):
+        view["flags"][rng.integers(0, n, 10)] ^= rng.integers(1, 4, 10).astype(np.uint8)
+        return [int(parents[rng.integers(0, len(parents))])] if tick % 100 == 99 else []
+
+    def call(xids):
+        x = np.array(xids, dtype=np.uint32)
+        res = C.POINTER(kvgpu._lib.HealthDeltaC)()
+        rc = lib.kvg_health_rescan_mdev(ctx.handle, ptr, n, N_TYPES, x.ctypes.data if len(x) else None, len(x),
+                                        C.byref(res))
+        assert rc == 0, ctx._lib.kvg_last_error(ctx.handle)
+        return res
+
+    def check(res, xids):
+        r = res.contents
+        got = np.ctypeslib.as_array(C.cast(r.changed, C.POINTER(C.c_uint32)), (r.n_changed,)) if r.n_changed else np.zeros(0, np.uint32)
+        want = ref.rescan(view, N_TYPES, xids)
+        assert r.n_alive == want.n_alive and np.array_equal(got, want.changed), "parity at %d records" % n
+
+    out = poll_loop(call, mutate, ticks, check)
+    out["path"] = "k_health_small<MdevHealthRec>" if n <= 32768 else "k_compact<MdevHealthOp, 256, 8>"
+    return out
+
+
+def pci_leg(ctx, ticks, ids):
+    lib = kvgpu.load()
+    n = 10_000
+    buf, ptr = pinned(n, 16)
+    view = buf.numpy().view(kvgpu.PCI_REC)
+    view[:] = O.gen_pci(0, n, ids, 12)
+    rng = np.random.default_rng(5)
+    prev = [np.zeros(n, dtype=bool)]
+    lib.kvg_health_reset(ctx.handle)
+
+    def mutate(tick):
+        view["driver"][rng.integers(0, n, 10)] = rng.integers(0, 5, 10)
+        return None
+
+    def call(_):
+        res = C.POINTER(kvgpu._lib.HealthDeltaC)()
+        assert lib.kvg_health_rescan(ctx.handle, ptr, n, C.byref(res)) == 0
+        return res
+
+    def check(res, _):
+        r = res.contents
+        now = util.pci_alive(view)
+        idx = np.nonzero(now != prev[0])[0]
+        got = np.ctypeslib.as_array(C.cast(r.changed, C.POINTER(C.c_uint32)), (r.n_changed,)) if r.n_changed else np.zeros(0, np.uint32)
+        assert np.array_equal(got, (idx.astype(np.uint32) << 1) | now[idx].astype(np.uint32)), "PCI parity"
+        prev[0] = now
+
+    out = poll_loop(call, mutate, ticks, check)
+    out.update(devices=n, path="k_health_small<PciHealthRec>")
+    return out
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--sizes", default="10000,32768,65536")
+    ap.add_argument("--ticks", type=int, default=10_000)
+    ap.add_argument("--out", default="health_mdev_out", help="directory for health_mdev.json")
+    a = ap.parse_args()
+    card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                          capture_output=True, text=True, check=True).stdout.strip().splitlines()[0]
+    print(card, flush=True)
+    ids = O.nv_ids(util.pciids_text())
+    out = {"card": card, "poll_hz": 1000, "ticks": a.ticks, "warmup": WARMUP, "flips_per_tick": 10,
+           "xid_every": 100, "what": "host wall time from snapshot-in-pinned-buffer to transitions on the host",
+           "mdev": {}}
+    with kvgpu.Context(0) as ctx:
+        for n in [int(s) for s in a.sizes.split(",")]:
+            out["mdev"][n] = mdev_leg(ctx, n, a.ticks)
+            print("mdev", n, json.dumps(out["mdev"][n]), flush=True)
+        out["pci_config5"] = pci_leg(ctx, a.ticks, ids)
+        print("pci", json.dumps(out["pci_config5"]), flush=True)
+    os.makedirs(a.out, exist_ok=True)
+    with open(os.path.join(a.out, "health_mdev.json"), "w") as f:
+        json.dump(out, f, indent=1)
+    print(json.dumps(out))
+
+
+if __name__ == "__main__":
+    main()
