@@ -16,6 +16,8 @@
  *                                            generic_device_plugin.go:325-342, :611-690
  *   kvg_health_rescan_mdev                <- the vGPU health check: device-path Create / Remove / Rename and
  *                                            NVML XID critical errors, generic_vgpu_device_plugin.go:280-385
+ *   kvg_health_rescan_groups              <- the passthrough health check: Create / Remove / Rename of the IOMMU
+ *                                            group's VFIO node, generic_device_plugin.go:611-690
  *   kvg_scan_pci_delta                    <- (no reference equivalent: the reference never re-scans)
  *   kvg_scan_mdev_delta                   <- (no reference equivalent: createVgpuIDMap runs once)
  *   kvg_comm_*, kvg_scan_pci_sharded      <- (no reference equivalent; BASELINE.json config 4)
@@ -392,6 +394,37 @@ int kvg_health_reset(kvg_ctx *ctx);
 int kvg_health_rescan_mdev(kvg_ctx *ctx, const kvg_mdev_rec *recs, size_t n, uint32_t n_types,
                            const uint32_t *xid_parents, size_t n_xid, kvg_health_delta **delta);
 int kvg_health_mdev_reset(kvg_ctx *ctx);
+
+/* Health re-scan of PCI records by IOMMU group: a passthrough GPU is healthy while its record passes
+ * createIommuDeviceMap's filter and the VFIO node of its IOMMU group (/dev/vfio/<group>) exists.
+ *
+ * `group_nodes` holds the handles of the IOMMU groups whose device node exists now, in the encoding of
+ * kvg_pci_rec.iommu_group: a standing set (one listing of the VFIO device directory per tick), not a list of events.
+ * Order and duplicates do not matter; membership is exact uint32 equality, so a handle no record carries changes
+ * nothing.  Record i keeps one bit h from the previous call:
+ *
+ *   h' = record i passes createIommuDeviceMap's filter (as kvg_health_rescan) && iommu_group(i) in group_nodes
+ *   i is listed iff h' != h
+ *
+ * So when every group of the snapshot has a node, the call reports what kvg_health_rescan reports on the same
+ * sequence of snapshots; and when every record passes the filter, all devices of a group flip together, exactly when
+ * the group's node appears or vanishes (generic_device_plugin.go:611-690: a Create sends `healthy`, a Remove or Rename
+ * `unhealthy`, for every device of the group).  The delta is kvg_health_delta: n_alive counts the records healthy now,
+ * changed[] holds (index << 1) | healthy_now in ascending index order.
+ *
+ * A call with a different n re-arms the state to "nothing healthy", as does kvg_health_groups_reset(); n = 0 returns
+ * an empty delta.  n_nodes > KVG_HEALTH_MAX_GROUPS, or group_nodes == NULL with n_nodes > 0, returns KVG_EINVAL and
+ * leaves the state unchanged.  The state is the context's own, separate from those of kvg_health_rescan and
+ * kvg_health_rescan_mdev: those calls, their resets, every scan, every delta and kvg_pciids_load leave it unchanged,
+ * and this call leaves theirs unchanged.
+ *
+ * Up to 32,768 records and with kernel timing off, the call is one kernel launch with no driver synchronisation on the
+ * way back; pinned `recs` are then read in place and must be 16-byte aligned (not checked).  Pageable memory is staged
+ * and has no alignment requirement. */
+#define KVG_HEALTH_MAX_GROUPS 4096 /* group handles per call */
+int kvg_health_rescan_groups(kvg_ctx *ctx, const kvg_pci_rec *recs, size_t n, const uint32_t *group_nodes,
+                             size_t n_nodes, kvg_health_delta **delta);
+int kvg_health_groups_reset(kvg_ctx *ctx);
 
 /* Scan `recs` and diff the result against the previous one, keyed by survivor address.
  *

@@ -8,6 +8,7 @@
 //        MdevClassifyOp      createVgpuIDMap's filter (:268-289)
 //        HealthOp            K6: alive-set diff against the previous scan
 //        MdevHealthOp        K6 for vGPUs: present / XID-marked state diff
+//        PciGroupHealthOp    K6 for passthrough GPUs: alive and the IOMMU group's VFIO node exists
 //   k_health_small<Rec>    K6 at poll-loop sizes: one CTA, TMA-staged, transitions into mapped host memory
 //   k_mdev_labels / _canon K5: label rule (:341-342) + merge of equal labels
 //   k_gen_*                counter-based synthetic snapshots (twins of oracle/kvg_oracle.c kvo_gen_*)
@@ -49,11 +50,17 @@ struct ScanCtrl {
 //   (no ticket needed).  One CTA per tile measured about 5 % slower at 4 Mi records (39.5 against 37.7 us, H100 SXM
 //   with a 400 W power limit).
 // ------------------------------------------------------------------------------------------------
-// An operator that keeps a per-CTA table in shared memory fills it in an overload of compact_enter (MdevHealthOp).
+// An operator that keeps a per-CTA table in shared memory fills it in an overload of compact_enter (MdevHealthOp,
+// PciGroupHealthOp).
 template <class Op>
 __device__ __forceinline__ void compact_enter(Op&) {}
+// The min-blocks launch bound of k_compact<Op>; 0 emits none.  With 16 KiB of static shared memory (PciGroupHealthOp)
+// ptxas otherwise caps the kernel at 32 registers and spills 24 bytes; a bound of 1 block lifts the cap (48 registers,
+// no spill).  Every other operator keeps the plain bound, so its code is unchanged.
+template <class Op>
+constexpr int COMPACT_MIN_BLOCKS = 0;
 template <class Op, int THREADS, int ROWS>
-__global__ void __launch_bounds__(THREADS) k_compact(Op op, uint64_t* tile_state, uint32_t epoch) {
+__global__ void __launch_bounds__(THREADS, COMPACT_MIN_BLOCKS<Op>) k_compact(Op op, uint64_t* tile_state, uint32_t epoch) {
   pdl_enter();
   compact_enter(op);
   lookback_tiles<Op, THREADS, ROWS>(op, tile_state, epoch);
@@ -232,26 +239,29 @@ struct HealthOp {
 // parent handles X:  p' = alive,  m' = p' && (parent in X || (p && m)),  healthy = p && !m.  The state byte keeps them
 // as bit 0 = healthy (p && !m), bit 1 = marked (p && m), so that bit 0 is the health in every K6 state byte.
 constexpr uint32_t HEALTH_MDEV_HEALTHY = 1u, HEALTH_MDEV_MARKED = 2u;
-// membership in the sorted set xs[0..n), n <= KVG_HEALTH_MAX_XID: lo = the last position whose value is <= v, found
-// by 10 fixed steps (no data-dependent trip count), then one compare; nothing is loaded when n == 0
+// membership in the sorted set xs[0..n), n <= CAP (a power of two): lo = the last position whose value is <= v, found
+// by log2(CAP) fixed steps (no data-dependent trip count; 10 for the XID set, 12 for the group set), then one compare;
+// nothing is loaded when n == 0
+template <uint32_t CAP>
 __device__ __forceinline__ bool sorted_has(const uint32_t* xs, uint32_t n, uint32_t v) {
-  static_assert(KVG_HEALTH_MAX_XID == 1024, "10 steps");
+  static_assert(CAP >= 2 && (CAP & (CAP - 1)) == 0, "a power of two");
   if (n == 0) return false;
   uint32_t lo = 0;
 #pragma unroll
-  for (uint32_t step = KVG_HEALTH_MAX_XID / 2; step; step >>= 1)
+  for (uint32_t step = CAP / 2; step; step >>= 1)
     if (lo + step < n && xs[lo + step] <= v) lo += step;
   return xs[lo] == v;
 }
 __device__ __forceinline__ uint32_t health_mdev_next(const uint4& hi, uint32_t s, uint32_t n_types, const uint32_t* xs,
                                                      uint32_t n_xid) {
   if (!mdev_record_alive(hi, n_types)) return 0;
-  const bool marked = (s & HEALTH_MDEV_MARKED) || sorted_has(xs, n_xid, hi.x);
+  const bool marked = (s & HEALTH_MDEV_MARKED) || sorted_has<KVG_HEALTH_MAX_XID>(xs, n_xid, hi.x);
   return marked ? HEALTH_MDEV_MARKED : HEALTH_MDEV_HEALTHY;
 }
-// every thread of the CTA copies its share of X into shared memory (the caller synchronises before the first use)
-__device__ __forceinline__ void load_xid_set(uint32_t* dst, const uint32_t* src, uint32_t n_xid) {
-  for (uint32_t k = threadIdx.x; k < n_xid; k += blockDim.x) dst[k] = src[k];
+// every thread of the CTA copies its share of a sorted set into shared memory (the caller synchronises before the
+// first use)
+__device__ __forceinline__ void load_sorted_set(uint32_t* dst, const uint32_t* src, uint32_t n) {
+  for (uint32_t k = threadIdx.x; k < n; k += blockDim.x) dst[k] = src[k];
 }
 
 // the look-back form (above HEALTH_SMALL_MAX records, or with kernel timing on): k_compact<MdevHealthOp, 256, 8>.
@@ -271,7 +281,7 @@ struct MdevHealthOp {
   uint32_t local_alive;
   __device__ __forceinline__ void enter() {
     __shared__ uint32_t s_set[KVG_HEALTH_MAX_XID];
-    load_xid_set(s_set, xid, n_xid);
+    load_sorted_set(s_set, xid, n_xid);
     s_xid = s_set;
     __syncthreads();
   }
@@ -300,6 +310,58 @@ struct MdevHealthOp {
   __device__ __forceinline__ void finish(uint32_t total) { ctrl->n_changed = total; }
 };
 __device__ __forceinline__ void compact_enter(MdevHealthOp& op) { op.enter(); }
+
+// ---- K6 for passthrough GPUs by IOMMU group: healthy = alive and the group's VFIO node exists ------------------------
+// One bit per record, as for HealthOp.  A tick with the sorted, deduplicated handles G of the groups whose node exists
+// now (the encoding of kvg_pci_rec.iommu_group, r.z of the record):  h' = pci_record_alive(r) && r.z in G.
+__device__ __forceinline__ uint32_t health_group_next(const uint4& r, const uint32_t* gs, uint32_t n_groups) {
+  return pci_record_alive(r) && sorted_has<KVG_HEALTH_MAX_GROUPS>(gs, n_groups, r.z) ? 1u : 0u;
+}
+
+// the look-back form (above HEALTH_SMALL_MAX records, or with kernel timing on): k_compact<PciGroupHealthOp, 256, 8>.
+// Item.x = healthy now | healthy before << 1, as HealthOp.
+struct PciGroupHealthOp {
+  using Item = uint4;
+  const uint4* recs;
+  uint32_t n;
+  const uint32_t* groups;  // G in device memory, copied into s_groups by enter()
+  uint32_t n_groups;
+  const uint32_t* s_groups;
+  uint8_t* state;  // one byte per record, updated in place
+  uint32_t* changed;
+  ScanCtrl* ctrl;
+  uint32_t local_alive;
+  __device__ __forceinline__ void enter() {
+    __shared__ uint32_t s_set[KVG_HEALTH_MAX_GROUPS];
+    load_sorted_set(s_set, groups, n_groups);
+    s_groups = s_set;
+    __syncthreads();
+  }
+  __device__ __forceinline__ uint32_t prepare(const Item&) const { return 0; }
+  __device__ __forceinline__ Item load(uint32_t i, bool ok) const {
+    if (!ok) return make_uint4(0, 0, 0, 0);
+    uint4 r = ld_stream(recs + i);
+    r.x = health_group_next(r, s_groups, n_groups) | ((uint32_t)state[i] << 1);
+    return r;
+  }
+  __device__ __forceinline__ bool pred(const Item& r, uint32_t) {
+    local_alive += r.x & 1u;
+    return (r.x & 1u) != (r.x >> 1);
+  }
+  __device__ __forceinline__ void emit(uint32_t pos, const Item& r, uint32_t i, uint32_t) {
+    changed[pos] = (i << 1) | (r.x & 1u);
+    state[i] = (uint8_t)(r.x & 1u);
+  }
+  __device__ __forceinline__ void tile_epilogue() {
+    uint32_t a = warp_sum(local_alive);
+    if (lane_id() == 0 && a) atomicAdd(&ctrl->n_alive, a);
+    local_alive = 0;
+  }
+  __device__ __forceinline__ void finish(uint32_t total) { ctrl->n_changed = total; }
+};
+__device__ __forceinline__ void compact_enter(PciGroupHealthOp& op) { op.enter(); }
+template <>
+constexpr int COMPACT_MIN_BLOCKS<PciGroupHealthOp> = 1;
 
 // K6 at poll-loop sizes (BASELINE.json config 5: 10,000 devices at 1 kHz): ONE CTA, one launch, one host
 // synchronisation.  The records are read where the host left them (mapped pinned memory: zero-copy over PCIe,
@@ -333,13 +395,30 @@ struct MdevHealthRec {
   const uint32_t* xid;  // X in the mapped result block
   uint32_t n_xid, n_types;
   __device__ __forceinline__ void enter(uint8_t* smem) const {
-    load_xid_set(reinterpret_cast<uint32_t*>(smem + XID_AT), xid, n_xid);
+    load_sorted_set(reinterpret_cast<uint32_t*>(smem + XID_AT), xid, n_xid);
   }
   __device__ __forceinline__ uint32_t next(const uint4* r, uint32_t s, const uint8_t* smem) const {
     return health_mdev_next(r[1], s, n_types, reinterpret_cast<const uint32_t*>(smem + XID_AT), n_xid);
   }
 };
-static_assert(PciHealthRec::SMEM == HEALTH_STAGE_BYTES && MdevHealthRec::XID_AT == HEALTH_STAGE_BYTES, "one round");
+// PCI by IOMMU group: 16-byte records, 12 rows per round, state = healthy (0 / 1), G (16 KiB at the cap) kept in
+// shared memory behind the stage: 208 KiB of dynamic shared memory
+struct PciGroupHealthRec {
+  static constexpr uint32_t UNITS = 1, STAGE_ROWS = 12;
+  static constexpr uint32_t SET_AT = STAGE_ROWS * HEALTH_SMALL_THREADS * 16 * UNITS;
+  static constexpr uint32_t SMEM = SET_AT + KVG_HEALTH_MAX_GROUPS * 4;
+  const uint32_t* groups;  // G in the mapped result block
+  uint32_t n_groups;
+  __device__ __forceinline__ void enter(uint8_t* smem) const {
+    load_sorted_set(reinterpret_cast<uint32_t*>(smem + SET_AT), groups, n_groups);
+  }
+  __device__ __forceinline__ uint32_t next(const uint4* r, uint32_t, const uint8_t* smem) const {
+    return health_group_next(r[0], reinterpret_cast<const uint32_t*>(smem + SET_AT), n_groups);
+  }
+};
+static_assert(PciHealthRec::SMEM == HEALTH_STAGE_BYTES && MdevHealthRec::XID_AT == HEALTH_STAGE_BYTES &&
+                  PciGroupHealthRec::SET_AT == HEALTH_STAGE_BYTES,
+              "one round");
 template <class Rec>
 __global__ void __launch_bounds__(HEALTH_SMALL_THREADS) k_health_small(Rec op, const uint4* __restrict__ recs, uint32_t n,
                                                                        uint8_t* __restrict__ state,

@@ -285,6 +285,20 @@ class Context:
     def health_mdev_reset(self):
         self._ck(self._lib.kvg_health_mdev_reset(self._h))
 
+    def health_rescan_groups(self, recs: np.ndarray, group_nodes=()) -> HealthDelta:
+        """Passthrough health re-scan by IOMMU group (include/kvgpu.h kvg_health_rescan_groups): a record is healthy
+        while it passes createIommuDeviceMap's filter and the VFIO node of its group exists.  `group_nodes`: the
+        handles (kvg_pci_rec.iommu_group encoding) of the groups whose node exists now (at most 4096)."""
+        recs = np.ascontiguousarray(recs, dtype=L.PCI_REC)
+        g = np.ascontiguousarray(np.asarray(group_nodes, dtype=np.uint32).reshape(-1))
+        res = C.POINTER(L.HealthDeltaC)()
+        self._ck(self._lib.kvg_health_rescan_groups(self._h, recs.ctypes.data, len(recs),
+                                                    g.ctypes.data if len(g) else None, len(g), C.byref(res)))
+        return self._take_health(res)
+
+    def health_groups_reset(self):
+        self._ck(self._lib.kvg_health_groups_reset(self._h))
+
     def _take_pci_delta(self, dl) -> PciDelta:
         d = dl.contents
         delta = PciDelta(int(d.n_prev), L._arr(d.changes, int(d.n_changes), L.PCI_CHANGE),

@@ -160,6 +160,40 @@ class PciSnapshot:
     device_names: list | None = None   # None: recs.device is the id itself ("%04x"); else interned `device` strings
 
 
+def _read_pci_entry(base_path: str, name: str):
+    """What the readers of createIommuDeviceMap's walk callback return for one entry -> (vendor, device, group,
+    driver, flags, numa); `device` and `group` are the strings read, or 0 / "" when they were not read."""
+    flags, vendor, device, group, driver, numa = 0, 0xFFFF, 0, "", L.DRV_NONE, 0
+    v, e = _read_id(base_path, name, "vendor")
+    if e:
+        flags |= L.PF_VENDOR_ERR
+    elif len(v) == 4 and all(c in HEXD for c in v):
+        vendor = int(v, 16)
+    if not e and v == "10de":
+        # same short-circuit order as :212-238 — a later file is only touched when the
+        # reference would touch it (so a panic can only happen where the reference panics)
+        d, e = _read_link(base_path, name, "driver")
+        if e:
+            flags |= L.PF_DRIVER_ERR
+        else:
+            driver = {"vfio-pci": L.DRV_VFIO_PCI,
+                      "nvgrace_gpu_vfio_pci": L.DRV_NVGRACE}.get(d, L.DRV_OTHER)
+        if not e and driver in (L.DRV_VFIO_PCI, L.DRV_NVGRACE):
+            group, e = _read_link(base_path, name, "iommu_group")
+            if e:
+                flags |= L.PF_IOMMU_ERR
+            else:
+                numa, e = _read_numa(base_path, name)
+                if e:
+                    flags |= L.PF_NUMA_ERR
+                dv, e = _read_id(base_path, name, "device")
+                if e:
+                    flags |= L.PF_DEVICE_ERR
+                else:
+                    device = dv   # the reference keeps WHATEVER the file holds as the map key (:240, :294-302)
+    return vendor, device, group, driver, flags, numa
+
+
 def snapshot_pci_tree(base_path: str) -> PciSnapshot:
     """Walk `base_path` like createIommuDeviceMap and record what each reader returned."""
     rows, names = [], []
@@ -168,35 +202,7 @@ def snapshot_pci_tree(base_path: str) -> PciSnapshot:
             break
         if is_dir:   # :197-200
             continue
-        flags, vendor, device, group, driver, numa = 0, 0xFFFF, 0, "", L.DRV_NONE, 0
-        v, e = _read_id(base_path, name, "vendor")
-        if e:
-            flags |= L.PF_VENDOR_ERR
-        elif len(v) == 4 and all(c in HEXD for c in v):
-            vendor = int(v, 16)
-        if not e and v == "10de":
-            # same short-circuit order as :212-238 — a later file is only touched when the
-            # reference would touch it (so a panic can only happen where the reference panics)
-            d, e = _read_link(base_path, name, "driver")
-            if e:
-                flags |= L.PF_DRIVER_ERR
-            else:
-                driver = {"vfio-pci": L.DRV_VFIO_PCI,
-                          "nvgrace_gpu_vfio_pci": L.DRV_NVGRACE}.get(d, L.DRV_OTHER)
-            if not e and driver in (L.DRV_VFIO_PCI, L.DRV_NVGRACE):
-                group, e = _read_link(base_path, name, "iommu_group")
-                if e:
-                    flags |= L.PF_IOMMU_ERR
-                else:
-                    numa, e = _read_numa(base_path, name)
-                    if e:
-                        flags |= L.PF_NUMA_ERR
-                    dv, e = _read_id(base_path, name, "device")
-                    if e:
-                        flags |= L.PF_DEVICE_ERR
-                    else:
-                        device = dv   # the reference keeps WHATEVER the file holds as the map key (:240, :294-302)
-        rows.append((name, vendor, device, group, driver, flags, numa))
+        rows.append((name,) + _read_pci_entry(base_path, name))
         names.append(name)
     packed = [parse_bdf(n) for n in names]
     packed_ok = all(p is not None for p in packed) and all(
@@ -237,6 +243,51 @@ def snapshot_pci_tree(base_path: str) -> PciSnapshot:
             raise L.KvgError(L.KVG_ERANGE, "numa_node %d of %s does not fit int16" % (numa, name))
         recs[i] = (packed[i] if packed_ok else i, vendor, device, g, driver, flags, numa)
     return PciSnapshot(recs, names, packed_ok, group_names, device_names)
+
+
+def snapshot_pci_ids(base_path: str, bdfs, intern: dict) -> PciSnapshot:
+    """Snapshot the PCI devices `bdfs` in THAT order (the health re-scan's fixed record order; a Walk would re-index
+    when one vanishes), with the readers and flag rules of snapshot_pci_tree.  An address whose entry is gone reads as
+    a vendor error, so its record fails the filter.
+
+    Group strings become handles through `intern`, a dict the caller keeps across snapshots (handles from 1; 0 = no
+    group), so a group keeps its handle and a VFIO node name resolves through the same dict (group_nodes).  names =
+    bdfs; group_names[h] = the string of handle h; addr is the packed BDF when every address parses, else the index.
+    The `device` column follows snapshot_pci_tree: "%04x" strings as the number, otherwise interned strings."""
+    names = list(bdfs)
+    rows = [_read_pci_entry(base_path, name) for name in names]
+    packed = [parse_bdf(n) for n in names]
+    packed_ok = all(p is not None for p in packed)
+    devs = [r[1] for r in rows if isinstance(r[1], str)]
+    devices_numeric = all(len(d) == 4 and all(c in HEXD for c in d) for d in devs)
+    device_names, dintern = (None, None) if devices_numeric else ([], {})
+    recs = np.zeros(len(names), dtype=L.PCI_REC)
+    for i, (vendor, device, group, driver, flags, numa) in enumerate(rows):
+        if isinstance(device, str):
+            if devices_numeric:
+                device = int(device, 16)
+            else:
+                device = dintern.setdefault(device, len(dintern))
+                if device == len(device_names):
+                    device_names.append(rows[i][1])
+                if device > 0xFFFF:
+                    raise L.KvgError(L.KVG_ERANGE, "more than 65536 distinct non-canonical device strings")
+        if not -32768 <= numa <= 32767:
+            raise L.KvgError(L.KVG_ERANGE, "numa_node %d of %s does not fit int16" % (numa, names[i]))
+        g = intern.setdefault(group, len(intern) + 1) if group else 0
+        recs[i] = (packed[i] if packed_ok else i, vendor, device, g, driver, flags, numa)
+    return PciSnapshot(recs, names, packed_ok, [""] + sorted(intern, key=intern.get), device_names)
+
+
+def group_nodes(device_path: str, intern: dict) -> np.ndarray:
+    """The handles (from `intern`, as snapshot_pci_ids assigns them) of the IOMMU groups whose VFIO node exists under
+    `device_path` (/dev/vfio/<group>, generic_device_plugin.go:611-690), ascending.  Other names (`vfio`, `devices`,
+    groups no snapshot has seen) can match no record and are left out; a missing directory means no node exists."""
+    try:
+        entries = os.listdir(device_path)
+    except FileNotFoundError:
+        entries = []
+    return np.array(sorted(intern[e] for e in entries if e in intern), dtype=np.uint32)
 
 
 def _read_vgpu_raw(base, addr, prop):

@@ -15,7 +15,8 @@ Allocate" is testable end to end in an image without a Go toolchain.
 
 Nothing here computes on the CPU what the scan computes on the GPU: the maps come from
 plugin.DiscoveryScan (libkvgpu.so); the re-validation's classification goes through
-Context.scan_pci (K3); the health feeds through Context.health_rescan and Context.health_rescan_mdev (K6); the
+Context.scan_pci (K3); the health feeds through Context.health_rescan, Context.health_rescan_mdev and
+Context.health_rescan_groups (K6); the
 hot-plug feeds through Context.scan_pci_delta and Context.scan_mdev_delta (K7).
 """
 from __future__ import annotations
@@ -760,22 +761,84 @@ class VgpuHealthFeed:
             self.health_rescan_mdev(snap.recs[:0], len(snap.raw_types))    # a different n re-arms the state
             self._uuids = uuids
         delta = self.health_rescan_mdev(snap.recs, len(snap.raw_types), xids)
-        sent = 0
-        if arming:
-            healthy = np.zeros(len(uuids), dtype=bool)
-            ch = np.asarray(delta.changed, dtype=np.int64)
-            healthy[ch[(ch & 1) == 1] >> 1] = True
-            for k, (d, plugin) in enumerate(devs):
-                if (d.health == dpapi.HEALTHY) != healthy[k]:
-                    (plugin.healthy if healthy[k] else plugin.unhealthy)(d.ID)
-                    sent += 1
-            return sent
-        for word in delta.changed:
-            k, ok = int(word) >> 1, int(word) & 1
-            d, plugin = devs[k]
-            (plugin.healthy if ok else plugin.unhealthy)(d.ID)
-            sent += 1
+        return _send_health(devs, delta, arming)
+
+    def start(self):
+        def loop():
+            while not self._stop.is_set():
+                self.tick()
+                time.sleep(self.period_s)
+        self._thread = threading.Thread(target=loop, daemon=True)
+        self._thread.start()
+
+    def stop(self):
+        self._stop.set()
+        if self._thread:
+            self._thread.join(2.0)
+
+
+def _send_health(devs, delta, arming: bool) -> int:
+    """Route a health delta over [(device, plugin)] (record k = devs[k]) to the plugins' channels.  On an arming tick
+    (the state was just re-armed, so every healthy record is listed) send each device whose health differs from what
+    its plugin advertises; otherwise send each transition.  Returns the number of events sent."""
+    sent = 0
+    if arming:
+        healthy = np.zeros(len(devs), dtype=bool)
+        ch = np.asarray(delta.changed, dtype=np.int64)
+        healthy[ch[(ch & 1) == 1] >> 1] = True
+        for k, (d, plugin) in enumerate(devs):
+            if (d.health == dpapi.HEALTHY) != healthy[k]:
+                (plugin.healthy if healthy[k] else plugin.unhealthy)(d.ID)
+                sent += 1
         return sent
+    for word in delta.changed:
+        k, ok = int(word) >> 1, int(word) & 1
+        d, plugin = devs[k]
+        (plugin.healthy if ok else plugin.unhealthy)(d.ID)
+        sent += 1
+    return sent
+
+
+class GroupHealthFeed:
+    """The passthrough health check of generic_device_plugin.go:611-690 on the GPU: periodic re-snapshot plus one
+    listing of the VFIO device directory -> Context.health_rescan_groups (K6) -> healthy / unhealthy events.
+
+      device node   every device of an IOMMU group goes unhealthy when /dev/vfio/<group> vanishes (Remove / Rename)
+                    and healthy when it returns (Create), :659-668
+      sysfs         a device whose record stops passing createIommuDeviceMap's filter goes unhealthy, as with
+                    HealthRescanFeed, and healthy again when it passes and its node exists
+
+    `health_rescan_groups(recs, group_nodes)` is Context.health_rescan_groups; `snapshot(bdfs, intern)` returns a
+    PciSnapshot of `bdfs` in that order with group handles from `intern` (plugin.snapshot_pci_ids over the sysfs
+    tree); `list_nodes(intern)` returns the handles of the groups whose node exists (plugin.group_nodes over the device
+    directory), resolved through the same dict, so a node no advertised device's group has is ignored; `plugins` are
+    the passthrough plugins, whose devices are the advertised BDFs.
+
+    tick(): snapshot, list the nodes, one kernel call, then each transition to the plugin advertising that BDF.  An
+    arming tick (the first, or one whose BDF list differs from the previous tick's) resets the state and sends each
+    device whose health differs from what its plugin advertises, so a device whose node is already absent goes
+    unhealthy at once.  Deliberate difference: only transitions are sent, where the reference re-sends `healthy` for
+    every device of a group on a repeated Create of its node (ListAndWatch then re-sends an unchanged list)."""
+
+    def __init__(self, health_rescan_groups, snapshot, list_nodes, plugins, period_s: float = 0.001):
+        self.health_rescan_groups, self.snapshot, self.list_nodes = health_rescan_groups, snapshot, list_nodes
+        self.plugins, self.period_s = list(plugins), period_s
+        self.intern = {}
+        self._bdfs = None
+        self._stop = threading.Event()
+        self._thread = None
+
+    def tick(self) -> int:
+        devs = [(d, p) for p in self.plugins for d in p.devs]
+        bdfs = [d.ID for d, _ in devs]
+        snap = self.snapshot(bdfs, self.intern)
+        nodes = self.list_nodes(self.intern)
+        arming = bdfs != self._bdfs
+        if arming:
+            self.health_rescan_groups(snap.recs[:0])      # a different n re-arms the state
+            self._bdfs = bdfs
+        delta = self.health_rescan_groups(snap.recs, nodes)
+        return _send_health(devs, delta, arming)
 
     def start(self):
         def loop():

@@ -115,6 +115,44 @@ int emu_health_mdev_compact(const uint4* recs, uint32_t n, uint32_t n_types, con
   return 0;
 }
 
+// K6 for passthrough GPUs by IOMMU group (kvg_health_rescan_groups), both forms on the same state bytes (healthy bit).
+// recs: n x 16 B records; groups: the sorted, deduplicated handles of the groups whose node exists.  Small form
+// (n <= 32,768): hdr_out {n_alive, n_changed, seq}.  Look-back form, one CTA per tile: ctrl_out {n_changed, n_alive}.
+int emu_health_groups_small(const uint4* recs, uint32_t n, const uint32_t* groups, uint32_t n_groups, uint8_t* state,
+                            uint32_t* changed_out, uint32_t* hdr_out) {
+  if (n == 0 || n > HEALTH_SMALL_MAX || n_groups > KVG_HEALTH_MAX_GROUPS) return -1;
+  PciGroupHealthRec op;
+  op.groups = groups;
+  op.n_groups = n_groups;
+  emu_launch(k_health_small<PciGroupHealthRec>, dim3(1), HEALTH_SMALL_THREADS, op, recs, n, state, changed_out, hdr_out,
+             5u);
+  return 0;
+}
+
+int emu_health_groups_compact(const uint4* recs, uint32_t n, const uint32_t* groups, uint32_t n_groups, uint8_t* state,
+                              uint32_t* changed_out, uint32_t* ctrl_out) {
+  if (n_groups > KVG_HEALTH_MAX_GROUPS) return -1;
+  const size_t tiles = (n + C_TILE - 1) / C_TILE;
+  ScanCtrl ctrl;
+  memset(&ctrl, 0, sizeof ctrl);
+  std::vector<uint64_t> st(tiles + 4, 0);
+  PciGroupHealthOp op;
+  op.recs = recs;
+  op.n = n;
+  op.groups = groups;
+  op.n_groups = n_groups;
+  op.s_groups = nullptr;
+  op.state = state;
+  op.changed = changed_out;
+  op.ctrl = &ctrl;
+  op.local_alive = 0;
+  emu_launch(k_compact<PciGroupHealthOp, KVG_BLOCK, C_ROWS>, dim3((unsigned)(tiles ? tiles : 1)), KVG_BLOCK, op, st.data(),
+             17u);
+  ctrl_out[0] = ctrl.n_changed;
+  ctrl_out[1] = ctrl.n_alive;
+  return 0;
+}
+
 // K5 (kvg_dev_scan_mdev up to the survivor list): type dictionary -> labels -> canonical ids, then the
 // 32-byte mdev records through k_classify_ragged<MdevClassifyOp,128,4> -> k_tile_offsets -> k_pack_survivors<2>.
 // raw / raw_off: the dictionary blob with n_types+1 offsets.  Outputs: label bytes per entry (at raw_off),
