@@ -6,10 +6,10 @@
 //   k_compact<Op,T,R>      one launch, decoupled look-back on the tile counts: K3 at latency-bound sizes, K6
 //        PciClassifyOp       createIommuDeviceMap's filter (device_plugin.go:201-244) + name join
 //        MdevClassifyOp      createVgpuIDMap's filter (:268-289)
-//        HealthOp            K6: alive-set diff against the previous scan
-//        MdevHealthOp        K6 for vGPUs: present / XID-marked state diff
-//        PciGroupHealthOp    K6 for passthrough GPUs: alive and the IOMMU group's VFIO node exists
-//   k_health_small<Rec>    K6 at poll-loop sizes: one CTA, TMA-staged, transitions into mapped host memory
+//        HealthOp<Rule>      K6: state diff against the previous tick, one health rule per record kind:
+//                            PciHealthRule (alive), MdevHealthRule (present / XID-marked vGPUs),
+//                            GroupHealthRule (alive and the IOMMU group's VFIO node exists)
+//   k_health_small<Rule>   K6 at poll-loop sizes: one CTA, TMA-staged, transitions into mapped host memory
 //   k_mdev_labels / _canon K5: label rule (:341-342) + merge of equal labels
 //   k_gen_*                counter-based synthetic snapshots (twins of oracle/kvg_oracle.c kvo_gen_*)
 #pragma once
@@ -45,18 +45,18 @@ struct ScanCtrl {
 //   classic decoupled look-back usually finds an inclusive prefix close by.  (Measured alternative: every tile
 //   publishes its count and sums ALL earlier counts itself, a thread per earlier tile — no chain, but several
 //   dependent L2 round trips per thread for the last tiles; it was slower at 1 M records.  The chained scan stays.)
-//   K6, k_compact<HealthOp, KVG_BLOCK, C_ROWS>: a persistent, co-resident grid of 2048-record tiles (compact_grid).
+//   K6, k_compact<HealthOp<Rule>, KVG_BLOCK, C_ROWS>: a persistent, co-resident grid of 2048-record tiles (compact_grid).
 //   A look-back predecessor is owned by a resident CTA that reaches it no later than this CTA reaches its own tile
 //   (no ticket needed).  One CTA per tile measured about 5 % slower at 4 Mi records (39.5 against 37.7 us, H100 SXM
 //   with a 400 W power limit).
 // ------------------------------------------------------------------------------------------------
-// An operator that keeps a per-CTA table in shared memory fills it in an overload of compact_enter (MdevHealthOp,
-// PciGroupHealthOp).
+// An operator that keeps a per-CTA table in shared memory fills it in an overload of compact_enter (HealthOp<Rule>
+// with a set).
 template <class Op>
 __device__ __forceinline__ void compact_enter(Op&) {}
-// The min-blocks launch bound of k_compact<Op>; 0 emits none.  With 16 KiB of static shared memory (PciGroupHealthOp)
-// ptxas otherwise caps the kernel at 32 registers and spills 24 bytes; a bound of 1 block lifts the cap (48 registers,
-// no spill).  Every other operator keeps the plain bound, so its code is unchanged.
+// The min-blocks launch bound of k_compact<Op>; 0 emits none.  With 16 KiB of static shared memory
+// (HealthOp<GroupHealthRule>) ptxas otherwise caps the kernel at 32 registers and spills; a bound of 1 block lifts the
+// cap.  Every other operator keeps the plain bound, so its code is unchanged.
 template <class Op>
 constexpr int COMPACT_MIN_BLOCKS = 0;
 template <class Op, int THREADS, int ROWS>
@@ -201,44 +201,17 @@ struct MdevClassifyOp : SurvivorOp<MdevClassifyOp> {
   __device__ __forceinline__ uint2 keys(const Item& r, uint32_t canon) const { return make_uint2(canon, r.hi.x); }
 };
 
-// ---- K6: health diff ----------------------------------------------------------------------------
-struct HealthOp {
-  using Item = uint4;
-  const uint4* recs;
-  uint32_t n;
-  uint8_t* alive_prev;  // one byte per record, updated in place
-  uint32_t* changed;
-  ScanCtrl* ctrl;
-  uint32_t local_alive;
-  __device__ __forceinline__ uint32_t prepare(const Item&) const { return 0; }
-  __device__ __forceinline__ Item load(uint32_t i, bool ok) const {
-    if (!ok) return make_uint4(0, 0, 0, 0);
-    uint4 r = ld_stream(recs + i);
-    uint32_t alive = pci_record_alive(r) ? 1u : 0u;
-    r.x = alive | ((uint32_t)alive_prev[i] << 1);
-    return r;
-  }
-  __device__ __forceinline__ bool pred(const Item& r, uint32_t) {
-    local_alive += r.x & 1u;
-    return (r.x & 1u) != (r.x >> 1);
-  }
-  __device__ __forceinline__ void emit(uint32_t pos, const Item& r, uint32_t i, uint32_t) {
-    changed[pos] = (i << 1) | (r.x & 1u);
-    alive_prev[i] = (uint8_t)(r.x & 1u);
-  }
-  __device__ __forceinline__ void tile_epilogue() {
-    uint32_t a = warp_sum(local_alive);
-    if (lane_id() == 0 && a) atomicAdd(&ctrl->n_alive, a);
-    local_alive = 0;
-  }
-  __device__ __forceinline__ void finish(uint32_t total) { ctrl->n_changed = total; }
-};
+// ---- K6: health re-scan -------------------------------------------------------------------------
+// Every health source is one rule: what its record is and how the state byte of a record moves from tick to tick.
+// Bit 0 of a state byte is the health the transition list reports; the rest is the rule's own.
+//   UNITS, UNIT        16-byte units per record, and the one unit next() reads
+//   STATE_BITS         bits of the state byte the rule uses
+//   STAGE_ROWS         rows of 1024 records per 192 KiB TMA round of k_health_small
+//   SET_CAP            0, or the cap of a sorted, deduplicated set (set, n_set) every CTA copies into shared memory
+//   next(r, s, set)    the state byte after this tick from unit UNIT of the record, the previous byte and the shared
+//                      copy of the set
+// k_health_small<Rule> runs it at poll-loop sizes, k_compact<HealthOp<Rule>, KVG_BLOCK, C_ROWS> above them.
 
-// ---- K6 for vGPUs: health = present and not marked by a critical XID on the parent GPU -------------------------------
-// Per record two bits, p (present: mdev_record_alive) and m (marked), m => p.  A tick with the sorted, deduplicated
-// parent handles X:  p' = alive,  m' = p' && (parent in X || (p && m)),  healthy = p && !m.  The state byte keeps them
-// as bit 0 = healthy (p && !m), bit 1 = marked (p && m), so that bit 0 is the health in every K6 state byte.
-constexpr uint32_t HEALTH_MDEV_HEALTHY = 1u, HEALTH_MDEV_MARKED = 2u;
 // membership in the sorted set xs[0..n), n <= CAP (a power of two): lo = the last position whose value is <= v, found
 // by log2(CAP) fixed steps (no data-dependent trip count; 10 for the XID set, 12 for the group set), then one compare;
 // nothing is loaded when n == 0
@@ -252,55 +225,90 @@ __device__ __forceinline__ bool sorted_has(const uint32_t* xs, uint32_t n, uint3
     if (lo + step < n && xs[lo + step] <= v) lo += step;
   return xs[lo] == v;
 }
-__device__ __forceinline__ uint32_t health_mdev_next(const uint4& hi, uint32_t s, uint32_t n_types, const uint32_t* xs,
-                                                     uint32_t n_xid) {
-  if (!mdev_record_alive(hi, n_types)) return 0;
-  const bool marked = (s & HEALTH_MDEV_MARKED) || sorted_has<KVG_HEALTH_MAX_XID>(xs, n_xid, hi.x);
-  return marked ? HEALTH_MDEV_MARKED : HEALTH_MDEV_HEALTHY;
-}
 // every thread of the CTA copies its share of a sorted set into shared memory (the caller synchronises before the
 // first use)
 __device__ __forceinline__ void load_sorted_set(uint32_t* dst, const uint32_t* src, uint32_t n) {
   for (uint32_t k = threadIdx.x; k < n; k += blockDim.x) dst[k] = src[k];
 }
 
-// the look-back form (above HEALTH_SMALL_MAX records, or with kernel timing on): k_compact<MdevHealthOp, 256, 8>.
-// Item.x = new state | old state << 2; the state byte is written whenever it changes, a transition or not (a marked
-// vGPU that vanishes loses its mark without a health change).
-struct MdevHealthOp {
+// PCI (kvg_health_rescan): state = alive (0 / 1)
+struct PciHealthRule {
+  static constexpr uint32_t UNITS = 1, UNIT = 0, STAGE_ROWS = 12, SET_CAP = 0, STATE_BITS = 1;
+  __device__ __forceinline__ uint32_t next(const uint4& r, uint32_t, const uint32_t*) const {
+    return pci_record_alive(r) ? 1u : 0u;
+  }
+};
+
+// vGPUs (kvg_health_rescan_mdev): healthy = present and not marked by a critical XID on the parent GPU.
+// Per record two bits, p (present: mdev_record_alive) and m (marked), m => p.  A tick with the sorted, deduplicated
+// parent handles X:  p' = alive,  m' = p' && (parent in X || (p && m)),  healthy = p && !m.  The state byte keeps them
+// as bit 0 = healthy (p && !m), bit 1 = marked (p && m).  The rule reads the second unit of the 32-byte record.
+constexpr uint32_t HEALTH_MDEV_HEALTHY = 1u, HEALTH_MDEV_MARKED = 2u;
+__device__ __forceinline__ uint32_t health_mdev_next(const uint4& hi, uint32_t s, uint32_t n_types, const uint32_t* xs,
+                                                     uint32_t n_xid) {
+  if (!mdev_record_alive(hi, n_types)) return 0;
+  const bool marked = (s & HEALTH_MDEV_MARKED) || sorted_has<KVG_HEALTH_MAX_XID>(xs, n_xid, hi.x);
+  return marked ? HEALTH_MDEV_MARKED : HEALTH_MDEV_HEALTHY;
+}
+struct MdevHealthRule {
+  static constexpr uint32_t UNITS = 2, UNIT = 1, STAGE_ROWS = 6, SET_CAP = KVG_HEALTH_MAX_XID, STATE_BITS = 2;
+  const uint32_t* set;  // X
+  uint32_t n_set, n_types;
+  __device__ __forceinline__ uint32_t next(const uint4& r, uint32_t s, const uint32_t* xs) const {
+    return health_mdev_next(r, s, n_types, xs, n_set);
+  }
+};
+
+// passthrough GPUs by IOMMU group (kvg_health_rescan_groups): healthy = alive and the group's VFIO node exists.  One
+// bit per record, as for PCI.  A tick with the sorted, deduplicated handles G of the groups whose node exists now (the
+// encoding of kvg_pci_rec.iommu_group, r.z of the record):  h' = pci_record_alive(r) && r.z in G.
+__device__ __forceinline__ uint32_t health_group_next(const uint4& r, const uint32_t* gs, uint32_t n_groups) {
+  return pci_record_alive(r) && sorted_has<KVG_HEALTH_MAX_GROUPS>(gs, n_groups, r.z) ? 1u : 0u;
+}
+struct GroupHealthRule {
+  static constexpr uint32_t UNITS = 1, UNIT = 0, STAGE_ROWS = 12, SET_CAP = KVG_HEALTH_MAX_GROUPS, STATE_BITS = 1;
+  const uint32_t* set;  // G
+  uint32_t n_set;
+  __device__ __forceinline__ uint32_t next(const uint4& r, uint32_t, const uint32_t* gs) const {
+    return health_group_next(r, gs, n_set);
+  }
+};
+
+// the look-back form (above HEALTH_SMALL_MAX records, or with kernel timing on): k_compact<HealthOp<Rule>, 256, 8>.
+// Item.x = new state | old state byte << W.  The state byte is written whenever it changes, a transition or not (a
+// marked vGPU that vanishes loses its mark without a health change); a change of bit 0 is listed.  A one-bit state
+// changes only with a transition, so emit writes it, where pred writes a wider one.  That, and reading state[i] as an
+// argument of next() (a rule that ignores it loads it after its own work), keeps the group instantiation at 48
+// registers: with the write in pred for every width, or the byte read first, ptxas takes 53 to 56.
+template <class Rule>
+struct HealthOp {
   using Item = uint4;
-  const uint4* recs;  // 2 x uint4 per record
+  static constexpr uint32_t W = Rule::STATE_BITS;
+  const uint4* recs;  // Rule::UNITS x uint4 per record
   uint32_t n;
-  uint32_t n_types;
-  const uint32_t* xid;  // X in device memory, copied into s_xid by enter()
-  uint32_t n_xid;
-  const uint32_t* s_xid;
-  uint8_t* state;  // one byte per record, updated in place
+  Rule rule;
+  const uint32_t* set;  // the rule's set in shared memory (compact_enter); unused without one
+  uint8_t* state;       // one byte per record, updated in place
   uint32_t* changed;
   ScanCtrl* ctrl;
   uint32_t local_alive;
-  __device__ __forceinline__ void enter() {
-    __shared__ uint32_t s_set[KVG_HEALTH_MAX_XID];
-    load_sorted_set(s_set, xid, n_xid);
-    s_xid = s_set;
-    __syncthreads();
-  }
   __device__ __forceinline__ uint32_t prepare(const Item&) const { return 0; }
   __device__ __forceinline__ Item load(uint32_t i, bool ok) const {
     if (!ok) return make_uint4(0, 0, 0, 0);
-    uint4 r = ld_stream(recs + 2 * (size_t)i + 1);
-    const uint32_t s = state[i];
-    r.x = health_mdev_next(r, s, n_types, s_xid, n_xid) | (s << 2);
+    uint4 r = ld_stream(recs + (size_t)i * Rule::UNITS + Rule::UNIT);
+    r.x = rule.next(r, state[i], set) | ((uint32_t)state[i] << W);
     return r;
   }
   __device__ __forceinline__ bool pred(const Item& r, uint32_t i) {
-    const uint32_t now = r.x & 3u, was = r.x >> 2;
-    if (now != was) state[i] = (uint8_t)now;
+    const uint32_t now = r.x & ((1u << W) - 1), was = r.x >> W;
     local_alive += now & 1u;
+    if constexpr (W == 1) return now != was;
+    if (now != was) state[i] = (uint8_t)now;
     return ((now ^ was) & 1u) != 0;
   }
   __device__ __forceinline__ void emit(uint32_t pos, const Item& r, uint32_t i, uint32_t) {
     changed[pos] = (i << 1) | (r.x & 1u);
+    if constexpr (W == 1) state[i] = (uint8_t)(r.x & 1u);
   }
   __device__ __forceinline__ void tile_epilogue() {
     uint32_t a = warp_sum(local_alive);
@@ -309,140 +317,55 @@ struct MdevHealthOp {
   }
   __device__ __forceinline__ void finish(uint32_t total) { ctrl->n_changed = total; }
 };
-__device__ __forceinline__ void compact_enter(MdevHealthOp& op) { op.enter(); }
-
-// ---- K6 for passthrough GPUs by IOMMU group: healthy = alive and the group's VFIO node exists ------------------------
-// One bit per record, as for HealthOp.  A tick with the sorted, deduplicated handles G of the groups whose node exists
-// now (the encoding of kvg_pci_rec.iommu_group, r.z of the record):  h' = pci_record_alive(r) && r.z in G.
-__device__ __forceinline__ uint32_t health_group_next(const uint4& r, const uint32_t* gs, uint32_t n_groups) {
-  return pci_record_alive(r) && sorted_has<KVG_HEALTH_MAX_GROUPS>(gs, n_groups, r.z) ? 1u : 0u;
-}
-
-// the look-back form (above HEALTH_SMALL_MAX records, or with kernel timing on): k_compact<PciGroupHealthOp, 256, 8>.
-// Item.x = healthy now | healthy before << 1, as HealthOp.
-struct PciGroupHealthOp {
-  using Item = uint4;
-  const uint4* recs;
-  uint32_t n;
-  const uint32_t* groups;  // G in device memory, copied into s_groups by enter()
-  uint32_t n_groups;
-  const uint32_t* s_groups;
-  uint8_t* state;  // one byte per record, updated in place
-  uint32_t* changed;
-  ScanCtrl* ctrl;
-  uint32_t local_alive;
-  __device__ __forceinline__ void enter() {
-    __shared__ uint32_t s_set[KVG_HEALTH_MAX_GROUPS];
-    load_sorted_set(s_set, groups, n_groups);
-    s_groups = s_set;
+template <class Rule>
+__device__ __forceinline__ void compact_enter(HealthOp<Rule>& op) {
+  if constexpr (Rule::SET_CAP > 0) {
+    __shared__ uint32_t s_set[Rule::SET_CAP];
+    load_sorted_set(s_set, op.rule.set, op.rule.n_set);
+    op.set = s_set;
     __syncthreads();
   }
-  __device__ __forceinline__ uint32_t prepare(const Item&) const { return 0; }
-  __device__ __forceinline__ Item load(uint32_t i, bool ok) const {
-    if (!ok) return make_uint4(0, 0, 0, 0);
-    uint4 r = ld_stream(recs + i);
-    r.x = health_group_next(r, s_groups, n_groups) | ((uint32_t)state[i] << 1);
-    return r;
-  }
-  __device__ __forceinline__ bool pred(const Item& r, uint32_t) {
-    local_alive += r.x & 1u;
-    return (r.x & 1u) != (r.x >> 1);
-  }
-  __device__ __forceinline__ void emit(uint32_t pos, const Item& r, uint32_t i, uint32_t) {
-    changed[pos] = (i << 1) | (r.x & 1u);
-    state[i] = (uint8_t)(r.x & 1u);
-  }
-  __device__ __forceinline__ void tile_epilogue() {
-    uint32_t a = warp_sum(local_alive);
-    if (lane_id() == 0 && a) atomicAdd(&ctrl->n_alive, a);
-    local_alive = 0;
-  }
-  __device__ __forceinline__ void finish(uint32_t total) { ctrl->n_changed = total; }
-};
-__device__ __forceinline__ void compact_enter(PciGroupHealthOp& op) { op.enter(); }
+}
 template <>
-constexpr int COMPACT_MIN_BLOCKS<PciGroupHealthOp> = 1;
+constexpr int COMPACT_MIN_BLOCKS<HealthOp<GroupHealthRule>> = 1;
 
 // K6 at poll-loop sizes (BASELINE.json config 5: 10,000 devices at 1 kHz): ONE CTA, one launch, one host
 // synchronisation.  The records are read where the host left them (mapped pinned memory: zero-copy over PCIe,
 // every load of a thread in flight at once), the transitions are written — in record order — straight into
 // the host-visible result block, and the two counters follow.  No staging copy, no look-back, no second
-// device-to-host copy.
-//   Rec (the record operator) says what a record is and how its state byte moves; bit 0 of a state byte is the
-//   health the transition list reports:
-//     UNITS, STAGE_ROWS       16-byte units per record, rows of 1024 records per 192 KiB TMA round
-//     SMEM                    dynamic shared memory: the stage, then whatever enter() keeps
-//     enter(smem)             once per CTA before the first round (every thread; a __syncthreads follows)
-//     next(rec, s, smem)      the state byte after this tick from the staged record and the previous byte
+// device-to-host copy.  Dynamic shared memory: the stage, then the rule's set.
 constexpr uint32_t HEALTH_SMALL_THREADS = 1024;
 constexpr uint32_t HEALTH_SMALL_ROWS = 32;                                        // rows of 1024 records
 constexpr uint32_t HEALTH_SMALL_MAX = HEALTH_SMALL_THREADS * HEALTH_SMALL_ROWS;  // 32,768 records
 constexpr uint32_t HEALTH_STAGE_BYTES = 192u << 10;                               // one TMA round
-// PCI: 16-byte records, 12 rows per round, state = alive (0 / 1)
-struct PciHealthRec {
-  static constexpr uint32_t UNITS = 1, STAGE_ROWS = 12;
-  static constexpr uint32_t SMEM = STAGE_ROWS * HEALTH_SMALL_THREADS * 16 * UNITS;
-  __device__ __forceinline__ void enter(uint8_t*) const {}
-  __device__ __forceinline__ uint32_t next(const uint4* r, uint32_t, const uint8_t*) const {
-    return pci_record_alive(r[0]) ? 1u : 0u;
-  }
-};
-// mdev: 32-byte records, 6 rows per round, state = healthy | marked << 1, X kept in shared memory behind the stage
-struct MdevHealthRec {
-  static constexpr uint32_t UNITS = 2, STAGE_ROWS = 6;
-  static constexpr uint32_t XID_AT = STAGE_ROWS * HEALTH_SMALL_THREADS * 16 * UNITS;
-  static constexpr uint32_t SMEM = XID_AT + KVG_HEALTH_MAX_XID * 4;
-  const uint32_t* xid;  // X in the mapped result block
-  uint32_t n_xid, n_types;
-  __device__ __forceinline__ void enter(uint8_t* smem) const {
-    load_sorted_set(reinterpret_cast<uint32_t*>(smem + XID_AT), xid, n_xid);
-  }
-  __device__ __forceinline__ uint32_t next(const uint4* r, uint32_t s, const uint8_t* smem) const {
-    return health_mdev_next(r[1], s, n_types, reinterpret_cast<const uint32_t*>(smem + XID_AT), n_xid);
-  }
-};
-// PCI by IOMMU group: 16-byte records, 12 rows per round, state = healthy (0 / 1), G (16 KiB at the cap) kept in
-// shared memory behind the stage: 208 KiB of dynamic shared memory
-struct PciGroupHealthRec {
-  static constexpr uint32_t UNITS = 1, STAGE_ROWS = 12;
-  static constexpr uint32_t SET_AT = STAGE_ROWS * HEALTH_SMALL_THREADS * 16 * UNITS;
-  static constexpr uint32_t SMEM = SET_AT + KVG_HEALTH_MAX_GROUPS * 4;
-  const uint32_t* groups;  // G in the mapped result block
-  uint32_t n_groups;
-  __device__ __forceinline__ void enter(uint8_t* smem) const {
-    load_sorted_set(reinterpret_cast<uint32_t*>(smem + SET_AT), groups, n_groups);
-  }
-  __device__ __forceinline__ uint32_t next(const uint4* r, uint32_t, const uint8_t* smem) const {
-    return health_group_next(r[0], reinterpret_cast<const uint32_t*>(smem + SET_AT), n_groups);
-  }
-};
-static_assert(PciHealthRec::SMEM == HEALTH_STAGE_BYTES && MdevHealthRec::XID_AT == HEALTH_STAGE_BYTES &&
-                  PciGroupHealthRec::SET_AT == HEALTH_STAGE_BYTES,
-              "one round");
-template <class Rec>
-__global__ void __launch_bounds__(HEALTH_SMALL_THREADS) k_health_small(Rec op, const uint4* __restrict__ recs, uint32_t n,
-                                                                       uint8_t* __restrict__ state,
+template <class Rule>
+constexpr uint32_t HEALTH_SMALL_SMEM = HEALTH_STAGE_BYTES + Rule::SET_CAP * 4;
+template <class Rule>
+__global__ void __launch_bounds__(HEALTH_SMALL_THREADS) k_health_small(Rule rule, const uint4* __restrict__ recs,
+                                                                       uint32_t n, uint8_t* __restrict__ state,
                                                                        uint32_t* __restrict__ changed_host,
                                                                        uint32_t* __restrict__ hdr_host, uint32_t seq) {
   pdl_enter();
-  constexpr uint32_t NW = HEALTH_SMALL_THREADS / 32, U = Rec::UNITS, SR = Rec::STAGE_ROWS;
+  constexpr uint32_t NW = HEALTH_SMALL_THREADS / 32, U = Rule::UNITS, SR = Rule::STAGE_ROWS;
+  static_assert(SR * HEALTH_SMALL_THREADS * 16 * U == HEALTH_STAGE_BYTES, "one round");
 #ifndef KVG_HOST_EMU
   extern __shared__ __align__(128) uint8_t hs_smem[];
 #else
-  static __attribute__((aligned(128))) uint8_t hs_smem[Rec::SMEM];
+  static __attribute__((aligned(128))) uint8_t hs_smem[HEALTH_SMALL_SMEM<Rule>];
 #endif
   __shared__ __align__(8) uint64_t s_bar;
   __shared__ uint32_t s_bal[HEALTH_SMALL_ROWS][NW];  // "changed" ballot of (row, warp) -> its position in the list
   __shared__ uint32_t s_now[HEALTH_SMALL_ROWS][NW];  // "healthy now" ballot of (row, warp)
   __shared__ uint32_t s_scan[NW], s_alv[NW];
   const uint4* stage = reinterpret_cast<const uint4*>(hs_smem);
+  uint32_t* set = reinterpret_cast<uint32_t*>(hs_smem + HEALTH_STAGE_BYTES);
   const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const uint32_t rows = (n + HEALTH_SMALL_THREADS - 1) / HEALTH_SMALL_THREADS;
   if (tid == 0) {
     mbar_init(&s_bar, 1);
     mbar_fence_init();
   }
-  op.enter(hs_smem);
+  if constexpr (Rule::SET_CAP > 0) load_sorted_set(set, rule.set, rule.n_set);
   __syncthreads();
   uint32_t n_alive = 0, phase = 0;
   for (uint32_t r0 = 0; r0 < rows; r0 += SR) {
@@ -470,7 +393,7 @@ __global__ void __launch_bounds__(HEALTH_SMALL_THREADS) k_health_small(Rec op, c
         const uint32_t i = first + k * HEALTH_SMALL_THREADS + tid;
         const bool in = i < n;
         // (lanes past n compute s from stale stage bytes and use none of it)
-        const uint32_t s = op.next(stage + (k * HEALTH_SMALL_THREADS + tid) * U, was[k], hs_smem);
+        const uint32_t s = rule.next(stage[(k * HEALTH_SMALL_THREADS + tid) * U + Rule::UNIT], was[k], set);
         const bool now = in && (s & 1u) != 0;
         const bool chg = in && (now ? 1u : 0u) != (was[k] & 1u);
         if (in && s != was[k]) state[i] = (uint8_t)s;

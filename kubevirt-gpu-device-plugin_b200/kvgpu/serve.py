@@ -523,33 +523,13 @@ def plugins_from_specs(specs, maps: Maps, revalidate, **kw) -> list:
 # ------------------------------------------------------------------------------------------------
 # health feed driven by the K6 delta kernel (SURVEY.md 8(f) rank 3)
 # ------------------------------------------------------------------------------------------------
-class HealthRescanFeed:
-    """Periodic re-snapshot -> Context.health_rescan (K6) -> healthy / unhealthy events.
+class _PollFeed:
+    """A feed polled on a daemon thread: start() calls self.tick() every period_s seconds until stop()."""
 
-    `snapshot()` returns (records, ids): the PCI snapshot in a FIXED device order and the device id
-    of every record.  Each transition the kernel reports ((index << 1) | alive) is routed to the
-    plugin that advertises that id.  The first tick only establishes the alive set."""
-
-    def __init__(self, health_rescan, snapshot, plugins, period_s: float = 0.001):
-        self.health_rescan, self.snapshot, self.period_s = health_rescan, snapshot, period_s
-        self.owner = {d.ID: p for p in plugins for d in p.devs}
-        self._primed = False
+    def __init__(self, period_s: float):
+        self.period_s = period_s
         self._stop = threading.Event()
         self._thread = None
-
-    def tick(self) -> int:
-        recs, ids = self.snapshot()
-        delta = self.health_rescan(recs)
-        sent = 0
-        if self._primed:
-            for word in delta.changed:
-                idx, alive = int(word) >> 1, int(word) & 1
-                plugin = self.owner.get(ids[idx])
-                if plugin is not None:
-                    (plugin.healthy if alive else plugin.unhealthy)(ids[idx])
-                    sent += 1
-        self._primed = True
-        return sent
 
     def start(self):
         def loop():
@@ -565,18 +545,45 @@ class HealthRescanFeed:
             self._thread.join(2.0)
 
 
+class HealthRescanFeed(_PollFeed):
+    """Periodic re-snapshot -> Context.health_rescan (K6) -> healthy / unhealthy events.
+
+    `snapshot()` returns (records, ids): the PCI snapshot in a FIXED device order and the device id
+    of every record.  Each transition the kernel reports ((index << 1) | alive) is routed to the
+    plugin that advertises that id.  The first tick only establishes the alive set."""
+
+    def __init__(self, health_rescan, snapshot, plugins, period_s: float = 0.001):
+        super().__init__(period_s)
+        self.health_rescan, self.snapshot = health_rescan, snapshot
+        self.owner = {d.ID: p for p in plugins for d in p.devs}
+        self._primed = False
+
+    def tick(self) -> int:
+        recs, ids = self.snapshot()
+        delta = self.health_rescan(recs)
+        sent = 0
+        if self._primed:
+            for word in delta.changed:
+                idx, alive = int(word) >> 1, int(word) & 1
+                plugin = self.owner.get(ids[idx])
+                if plugin is not None:
+                    (plugin.healthy if alive else plugin.unhealthy)(ids[idx])
+                    sent += 1
+        self._primed = True
+        return sent
+
+
 # ------------------------------------------------------------------------------------------------
 # hot-plug feeds driven by the K7 re-scan deltas
 # ------------------------------------------------------------------------------------------------
-class _RescanFeed:
-    """The loop and the plugin lifecycle both re-scan feeds share; a subclass supplies tick()."""
+class _RescanFeed(_PollFeed):
+    """The plugin lifecycle both re-scan feeds share; a subclass supplies tick()."""
 
     def __init__(self, scan_delta, snapshot, maps: Maps, plugins: dict, make_plugin, period_s: float):
+        super().__init__(period_s)
         self.scan_delta, self.snapshot, self.maps = scan_delta, snapshot, maps
-        self.plugins, self.make_plugin, self.period_s = plugins, make_plugin, period_s
+        self.plugins, self.make_plugin = plugins, make_plugin
         self._prev_snap = None
-        self._stop = threading.Event()
-        self._thread = None
 
     def _follow(self, dirty: Maps, gone: list):
         """The plugins of the dirty keys (`dirty` holds their maps) get their new device list, or are started and
@@ -593,19 +600,6 @@ class _RescanFeed:
             plugin = self.plugins.pop(key, None)
             if plugin is not None:
                 plugin.stop()
-
-    def start(self):
-        def loop():
-            while not self._stop.is_set():
-                self.tick()
-                time.sleep(self.period_s)
-        self._thread = threading.Thread(target=loop, daemon=True)
-        self._thread.start()
-
-    def stop(self):
-        self._stop.set()
-        if self._thread:
-            self._thread.join(2.0)
 
 
 class PciRescanFeed(_RescanFeed):
@@ -703,7 +697,7 @@ class XidEventRouter:
         return sum(self._mark(bus) for u, bus in self.gpus if u == uuid)
 
 
-class VgpuHealthFeed:
+class VgpuHealthFeed(_PollFeed):
     """The vGPU health check of generic_vgpu_device_plugin.go:280-385 on the GPU: periodic re-snapshot plus the XID
     events since the last tick -> Context.health_rescan_mdev (K6) -> healthy / unhealthy events.
 
@@ -727,14 +721,13 @@ class VgpuHealthFeed:
     unchanged list)."""
 
     def __init__(self, health_rescan_mdev, snapshot, plugins, gpus, period_s: float = 0.001):
-        self.health_rescan_mdev, self.snapshot, self.period_s = health_rescan_mdev, snapshot, period_s
+        super().__init__(period_s)
+        self.health_rescan_mdev, self.snapshot = health_rescan_mdev, snapshot
         self.plugins, self.gpus = list(plugins), list(gpus)
         self.intern = {}
         self._uuids = None
         self._queued = []
         self._lock = threading.Lock()
-        self._stop = threading.Event()
-        self._thread = None
 
     def _queue(self, buses) -> int:
         with self._lock:
@@ -763,19 +756,6 @@ class VgpuHealthFeed:
         delta = self.health_rescan_mdev(snap.recs, len(snap.raw_types), xids)
         return _send_health(devs, delta, arming)
 
-    def start(self):
-        def loop():
-            while not self._stop.is_set():
-                self.tick()
-                time.sleep(self.period_s)
-        self._thread = threading.Thread(target=loop, daemon=True)
-        self._thread.start()
-
-    def stop(self):
-        self._stop.set()
-        if self._thread:
-            self._thread.join(2.0)
-
 
 def _send_health(devs, delta, arming: bool) -> int:
     """Route a health delta over [(device, plugin)] (record k = devs[k]) to the plugins' channels.  On an arming tick
@@ -799,7 +779,7 @@ def _send_health(devs, delta, arming: bool) -> int:
     return sent
 
 
-class GroupHealthFeed:
+class GroupHealthFeed(_PollFeed):
     """The passthrough health check of generic_device_plugin.go:611-690 on the GPU: periodic re-snapshot plus one
     listing of the VFIO device directory -> Context.health_rescan_groups (K6) -> healthy / unhealthy events.
 
@@ -821,12 +801,11 @@ class GroupHealthFeed:
     every device of a group on a repeated Create of its node (ListAndWatch then re-sends an unchanged list)."""
 
     def __init__(self, health_rescan_groups, snapshot, list_nodes, plugins, period_s: float = 0.001):
+        super().__init__(period_s)
         self.health_rescan_groups, self.snapshot, self.list_nodes = health_rescan_groups, snapshot, list_nodes
-        self.plugins, self.period_s = list(plugins), period_s
+        self.plugins = list(plugins)
         self.intern = {}
         self._bdfs = None
-        self._stop = threading.Event()
-        self._thread = None
 
     def tick(self) -> int:
         devs = [(d, p) for p in self.plugins for d in p.devs]
@@ -839,19 +818,6 @@ class GroupHealthFeed:
             self._bdfs = bdfs
         delta = self.health_rescan_groups(snap.recs, nodes)
         return _send_health(devs, delta, arming)
-
-    def start(self):
-        def loop():
-            while not self._stop.is_set():
-                self.tick()
-                time.sleep(self.period_s)
-        self._thread = threading.Thread(target=loop, daemon=True)
-        self._thread.start()
-
-    def stop(self):
-        self._stop.set()
-        if self._thread:
-            self._thread.join(2.0)
 
 
 # ------------------------------------------------------------------------------------------------

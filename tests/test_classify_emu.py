@@ -59,7 +59,7 @@ def test_classify_pipeline_matches_the_drop_rules(emu, variant):
 
 
 def test_health_diff_kernel_reports_transitions_in_record_order(emu):
-    """K6 = k_compact<HealthOp, 256, 8> (BASELINE.json config 5): the transition list of every tick, like
+    """K6 = k_compact<HealthOp<PciHealthRule>, 256, 8> (BASELINE.json config 5): the transition list of every tick, like
     tests/test_gpu_parity.py::test_health_rescan_transitions, from kernel source."""
     emu.emu_health_rescan.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]
     ids = O.nv_ids(util.pciids_text())

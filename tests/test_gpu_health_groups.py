@@ -1,7 +1,7 @@
 """kvg_health_rescan_groups on the H100 against the numpy state machine of tests/health_groups_ref.py, on both sides of
-every threshold the host uses to pick a kernel: k_health_small<PciGroupHealthRec> up to 32,768 records with kernel
-timing off, k_compact<PciGroupHealthOp, 256, 8> above it or with timing on, on the same state.  Pinned snapshots are
-changed in place and read in place; pageable ones are staged.  Also: P1 against kvg_health_rescan on a second
+every threshold the host uses to pick a kernel: k_health_small<GroupHealthRule> up to 32,768 records with kernel
+timing off, k_compact<HealthOp<GroupHealthRule>, 256, 8> above it or with timing on, on the same state.  Pinned
+snapshots are changed in place and read in place; pageable ones are staged.  Also: P1 against kvg_health_rescan on a second
 context, P2 with every record alive, the 4,096-handle cap, re-arming, and the state kept apart from the PCI and vGPU
 health states and from every scan, delta and pci.ids load in both directions."""
 import ctypes as C

@@ -1,7 +1,7 @@
 """kvg_health_rescan_mdev on the H100 against the numpy state machine of tests/health_mdev_ref.py, on both sides of
-every threshold the host uses to pick a kernel: k_health_small<MdevHealthRec> up to 32,768 records with kernel timing
-off (6 rows of 1024 records per TMA round), k_compact<MdevHealthOp, 256, 8> above it or with timing on, on the same
-state.  Pinned snapshots are changed in place and read in place; pageable ones are staged.  Also: the state is
+every threshold the host uses to pick a kernel: k_health_small<MdevHealthRule> up to 32,768 records with kernel timing
+off (6 rows of 1024 records per TMA round), k_compact<HealthOp<MdevHealthRule>, 256, 8> above it or with timing on, on
+the same state.  Pinned snapshots are changed in place and read in place; pageable ones are staged.  Also: the state is
 separate from the PCI health state and from every scan, delta and pci.ids load; bad XID lists are refused and leave
 the state as it was."""
 import ctypes as C

@@ -37,7 +37,7 @@ DIGITS8_MIN = 8 * Mi
 # kvg_api_scan.inc PIPE_MIN_RECORDS / PIPE_MAX_RECORDS: kvg_scan_pci pipelines its copies in between
 PIPE_MAX = 16 * Mi
 # kvg_scan.cuh HEALTH_STAGE_ROWS x HEALTH_SMALL_THREADS records per TMA round of k_health_small, and
-# HEALTH_SMALL_MAX = 32 rows of 1024: above it (or with kernel timing on) k_compact<HealthOp, 256, 8>
+# HEALTH_SMALL_MAX = 32 rows of 1024: above it (or with kernel timing on) k_compact<HealthOp<PciHealthRule>, 256, 8>
 HEALTH_ROUND = 12 * 1024
 HEALTH_SMALL_MAX = 32 * 1024
 # kvg_api_shard.inc FUSED_SEND_MAX: shards from this size on classify, then send with k_shard_send
@@ -397,7 +397,7 @@ def _flip_points(n, rng):
 def test_health_regimes(kv, ids, pinned):
     """Ticks with flips on row / round boundaries at every size regime, pageable and pinned snapshots (pinned:
     changed in place), sizes changed between calls (the state re-arms), and kernel timing switched on for one
-    tick (k_compact<HealthOp, 256, 8> on the same state) and off again."""
+    tick (k_compact<HealthOp<PciHealthRule>, 256, 8> on the same state) and off again."""
     import torch
     ctx = kv.Context(0)
     rng = np.random.default_rng(17 + pinned)
@@ -425,8 +425,8 @@ def test_health_regimes(kv, ids, pinned):
                 if timed:
                     labels = {name for name, _ in ctx.kernel_times(1 << 16)}
                     ctx.set_kernel_timing(False)
-                    # timing moves every size to k_compact<HealthOp, 256, 8>; the untimed ticks around it run
-                    # k_health_small up to HEALTH_SMALL_MAX records, on the same alive-set
+                    # timing moves every size to k_compact<HealthOp<PciHealthRule>, 256, 8>; the untimed ticks
+                    # around it run k_health_small up to HEALTH_SMALL_MAX records, on the same alive-set
                     assert "health_compact" in labels and "health_small" not in labels, sorted(labels)
                 now = util.pci_alive(recs)
                 idx = np.nonzero(now != prev)[0]

@@ -1,9 +1,9 @@
 """K6 for passthrough GPUs by IOMMU group (kvg_health_rescan_groups), both kernel forms executed on the CPU from their
 real source under the warp emulator of tools/emu/, against the numpy state machine of tests/health_groups_ref.py:
-k_health_small<PciGroupHealthRec> (one CTA, 12 rows of 1024 records per TMA round, the group set behind the stage)
-and k_compact<PciGroupHealthOp, 256, 8> (look-back over 2048-record tiles), on the same state bytes.  Also the two
-properties the call promises: with a node for every group it reports what kvg_health_rescan's kernels
-(PciHealthRec / HealthOp) report (P1), and with every record alive all devices of a group flip together (P2)."""
+k_health_small<GroupHealthRule> (one CTA, 12 rows of 1024 records per TMA round, the group set behind the stage)
+and k_compact<HealthOp<GroupHealthRule>, 256, 8> (look-back over 2048-record tiles), on the same state bytes.  Also the
+two properties the call promises: with a node for every group it reports what kvg_health_rescan's kernels
+(PciHealthRule) report (P1), and with every record alive all devices of a group flip together (P2)."""
 import ctypes as C
 import os
 import sys
@@ -17,7 +17,7 @@ import health_groups_ref as H
 sys.path.insert(0, os.path.join(conftest.ROOT, "tools", "emu"))
 import build as emu_build  # noqa: E402
 
-ROUND = 12 * 1024       # records per TMA round of k_health_small<PciGroupHealthRec>
+ROUND = 12 * 1024       # records per TMA round of k_health_small<GroupHealthRule>
 SMALL_MAX = 32 * 1024
 TILE = 2048             # records per look-back tile
 CAP = 4096              # KVG_HEALTH_MAX_GROUPS
@@ -68,7 +68,8 @@ class Kernel:
 
 
 class PlainHealth:
-    """kvg_health_rescan's kernels (k_health_small<PciHealthRec> / k_compact<HealthOp>) on their own state."""
+    """kvg_health_rescan's kernels (k_health_small<PciHealthRule> / k_compact<HealthOp<PciHealthRule>>) on their own
+    state."""
 
     def __init__(self, emu, form, n):
         self.emu, self.form, self.n = emu, form, n

@@ -1,7 +1,7 @@
 """K6 for vGPUs (kvg_health_rescan_mdev), both kernel forms executed on the CPU from their real source under the warp
-emulator of tools/emu/, against the numpy state machine of tests/health_mdev_ref.py: k_health_small<MdevHealthRec>
-(one CTA, 6 rows of 1024 records per TMA round) and k_compact<MdevHealthOp, 256, 8> (look-back over 2048-record
-tiles), on the same state bytes."""
+emulator of tools/emu/, against the numpy state machine of tests/health_mdev_ref.py: k_health_small<MdevHealthRule>
+(one CTA, 6 rows of 1024 records per TMA round) and k_compact<HealthOp<MdevHealthRule>, 256, 8> (look-back over
+2048-record tiles), on the same state bytes."""
 import ctypes as C
 import os
 import sys
@@ -16,7 +16,7 @@ from oracle import oracle as O
 sys.path.insert(0, os.path.join(conftest.ROOT, "tools", "emu"))
 import build as emu_build  # noqa: E402
 
-ROUND = 6 * 1024        # records per TMA round of k_health_small<MdevHealthRec>
+ROUND = 6 * 1024        # records per TMA round of k_health_small<MdevHealthRule>
 SMALL_MAX = 32 * 1024
 TILE = 2048             # records per look-back tile
 N_TYPES = 200           # gen_mdev draws type indices 0..255: some records are out of the dictionary

@@ -7,6 +7,42 @@
 #include "../../kubevirt-gpu-device-plugin_b200/csrc/kvg_scan.cuh"
 using namespace kvg;
 
+// K6, both forms of every health rule (kvg_scan.cuh) on the caller's state bytes, transitions in record order.
+// Small form (n <= 32,768): one CTA, transitions + counters written where the host reads them; hdr_out {n_alive,
+// n_changed, seq}.  Look-back form: changed_out has room for n words; ctrl_out {n_changed, n_alive}.  Its grid is one
+// CTA per tile — what compact_grid() picks whenever the tiles fit the GPU, and the only shape a sequential emulation of
+// a look-back kernel can run.
+template <class Rule>
+static int health_small(Rule rule, const uint4* recs, uint32_t n, uint8_t* state, uint32_t* changed_out,
+                        uint32_t* hdr_out, uint32_t seq) {
+  if (n == 0 || n > HEALTH_SMALL_MAX) return -1;
+  emu_launch(k_health_small<Rule>, dim3(1), HEALTH_SMALL_THREADS, rule, recs, n, state, changed_out, hdr_out, seq);
+  return 0;
+}
+
+template <class Rule>
+static int health_compact(Rule rule, const uint4* recs, uint32_t n, uint8_t* state, uint32_t* changed_out,
+                          uint32_t* ctrl_out, uint32_t epoch) {
+  const size_t tiles = (n + C_TILE - 1) / C_TILE;
+  ScanCtrl ctrl;
+  memset(&ctrl, 0, sizeof ctrl);
+  std::vector<uint64_t> st(tiles + 4, 0);
+  HealthOp<Rule> op;
+  op.rule = rule;
+  op.recs = recs;
+  op.n = n;
+  op.state = state;
+  op.changed = changed_out;
+  op.ctrl = &ctrl;
+  op.set = nullptr;
+  op.local_alive = 0;
+  emu_launch(k_compact<HealthOp<Rule>, KVG_BLOCK, C_ROWS>, dim3((unsigned)(tiles ? tiles : 1)), KVG_BLOCK, op, st.data(),
+             epoch);
+  ctrl_out[0] = ctrl.n_changed;
+  ctrl_out[1] = ctrl.n_alive;
+  return 0;
+}
+
 extern "C" {
 
 // recs: n x 16 B records; nv_index: 65536 name slots; surv_out: room for n survivors.
@@ -46,111 +82,41 @@ int emu_classify_pci(const uint4* recs, uint32_t n, const uint32_t* nv_index, in
   return 0;
 }
 
-// K6 (kvg_health_rescan): alive-set diff against the previous scan, transitions in record order.
-// alive_prev: n bytes, updated in place.  changed_out: room for n words.  ctrl_out: {n_changed, n_alive}.
-// The grid is one CTA per tile — what compact_grid() picks whenever the tiles fit the GPU, and the only
-// shape a sequential emulation of a look-back kernel can run.
+// K6 (kvg_health_rescan): alive-set diff against the previous scan.  recs: n x 16 B records.
 int emu_health_rescan(const uint4* recs, uint32_t n, uint8_t* alive_prev, uint32_t* changed_out, uint32_t* ctrl_out) {
-  const size_t tiles = (n + C_TILE - 1) / C_TILE;
-  ScanCtrl ctrl;
-  memset(&ctrl, 0, sizeof ctrl);
-  std::vector<uint64_t> state(tiles + 4, 0);
-  HealthOp op;
-  op.recs = recs;
-  op.n = n;
-  op.alive_prev = alive_prev;
-  op.changed = changed_out;
-  op.ctrl = &ctrl;
-  op.local_alive = 0;
-  emu_launch(k_compact<HealthOp, KVG_BLOCK, C_ROWS>, dim3((unsigned)(tiles ? tiles : 1)), KVG_BLOCK, op, state.data(), 11u);
-  ctrl_out[0] = ctrl.n_changed;
-  ctrl_out[1] = ctrl.n_alive;
-  return 0;
+  return health_compact(PciHealthRule{}, recs, n, alive_prev, changed_out, ctrl_out, 11u);
 }
 
-// K6 at poll-loop sizes (kvg_health_rescan, n <= 32,768): one CTA, transitions + counters written where the
-// host reads them.  hdr_out: {n_alive, n_changed}.
 int emu_health_small(const uint4* recs, uint32_t n, uint8_t* alive_prev, uint32_t* changed_out, uint32_t* hdr_out) {
-  if (n == 0 || n > HEALTH_SMALL_MAX) return -1;
-  emu_launch(k_health_small<PciHealthRec>, dim3(1), HEALTH_SMALL_THREADS, PciHealthRec{}, recs, n, alive_prev, changed_out,
-             hdr_out, 7u);
-  return 0;
+  return health_small(PciHealthRule{}, recs, n, alive_prev, changed_out, hdr_out, 7u);
 }
 
-// K6 for vGPUs (kvg_health_rescan_mdev), both forms on the same state bytes (bit 0 present, bit 1 marked).
-// recs: n x 32 B records; xid: the sorted, deduplicated parent handles.  Small form (n <= 32,768): hdr_out
-// {n_alive, n_changed, seq}.  Look-back form, one CTA per tile: ctrl_out {n_changed, n_alive}.
+// K6 for vGPUs (kvg_health_rescan_mdev): state bit 0 healthy, bit 1 marked.  recs: n x 32 B records; xid: the sorted,
+// deduplicated parent handles.
 int emu_health_mdev_small(const uint4* recs, uint32_t n, uint32_t n_types, const uint32_t* xid, uint32_t n_xid,
                           uint8_t* state, uint32_t* changed_out, uint32_t* hdr_out) {
-  if (n == 0 || n > HEALTH_SMALL_MAX || n_xid > KVG_HEALTH_MAX_XID) return -1;
-  MdevHealthRec op;
-  op.xid = xid;
-  op.n_xid = n_xid;
-  op.n_types = n_types;
-  emu_launch(k_health_small<MdevHealthRec>, dim3(1), HEALTH_SMALL_THREADS, op, recs, n, state, changed_out, hdr_out, 9u);
-  return 0;
+  if (n_xid > KVG_HEALTH_MAX_XID) return -1;
+  return health_small(MdevHealthRule{xid, n_xid, n_types}, recs, n, state, changed_out, hdr_out, 9u);
 }
 
 int emu_health_mdev_compact(const uint4* recs, uint32_t n, uint32_t n_types, const uint32_t* xid, uint32_t n_xid,
                             uint8_t* state, uint32_t* changed_out, uint32_t* ctrl_out) {
   if (n_xid > KVG_HEALTH_MAX_XID) return -1;
-  const size_t tiles = (n + C_TILE - 1) / C_TILE;
-  ScanCtrl ctrl;
-  memset(&ctrl, 0, sizeof ctrl);
-  std::vector<uint64_t> st(tiles + 4, 0);
-  MdevHealthOp op;
-  op.recs = recs;
-  op.n = n;
-  op.n_types = n_types;
-  op.xid = xid;
-  op.n_xid = n_xid;
-  op.s_xid = nullptr;
-  op.state = state;
-  op.changed = changed_out;
-  op.ctrl = &ctrl;
-  op.local_alive = 0;
-  emu_launch(k_compact<MdevHealthOp, KVG_BLOCK, C_ROWS>, dim3((unsigned)(tiles ? tiles : 1)), KVG_BLOCK, op, st.data(), 13u);
-  ctrl_out[0] = ctrl.n_changed;
-  ctrl_out[1] = ctrl.n_alive;
-  return 0;
+  return health_compact(MdevHealthRule{xid, n_xid, n_types}, recs, n, state, changed_out, ctrl_out, 13u);
 }
 
-// K6 for passthrough GPUs by IOMMU group (kvg_health_rescan_groups), both forms on the same state bytes (healthy bit).
-// recs: n x 16 B records; groups: the sorted, deduplicated handles of the groups whose node exists.  Small form
-// (n <= 32,768): hdr_out {n_alive, n_changed, seq}.  Look-back form, one CTA per tile: ctrl_out {n_changed, n_alive}.
+// K6 for passthrough GPUs by IOMMU group (kvg_health_rescan_groups): state = healthy bit.  recs: n x 16 B records;
+// groups: the sorted, deduplicated handles of the groups whose node exists.
 int emu_health_groups_small(const uint4* recs, uint32_t n, const uint32_t* groups, uint32_t n_groups, uint8_t* state,
                             uint32_t* changed_out, uint32_t* hdr_out) {
-  if (n == 0 || n > HEALTH_SMALL_MAX || n_groups > KVG_HEALTH_MAX_GROUPS) return -1;
-  PciGroupHealthRec op;
-  op.groups = groups;
-  op.n_groups = n_groups;
-  emu_launch(k_health_small<PciGroupHealthRec>, dim3(1), HEALTH_SMALL_THREADS, op, recs, n, state, changed_out, hdr_out,
-             5u);
-  return 0;
+  if (n_groups > KVG_HEALTH_MAX_GROUPS) return -1;
+  return health_small(GroupHealthRule{groups, n_groups}, recs, n, state, changed_out, hdr_out, 5u);
 }
 
 int emu_health_groups_compact(const uint4* recs, uint32_t n, const uint32_t* groups, uint32_t n_groups, uint8_t* state,
                               uint32_t* changed_out, uint32_t* ctrl_out) {
   if (n_groups > KVG_HEALTH_MAX_GROUPS) return -1;
-  const size_t tiles = (n + C_TILE - 1) / C_TILE;
-  ScanCtrl ctrl;
-  memset(&ctrl, 0, sizeof ctrl);
-  std::vector<uint64_t> st(tiles + 4, 0);
-  PciGroupHealthOp op;
-  op.recs = recs;
-  op.n = n;
-  op.groups = groups;
-  op.n_groups = n_groups;
-  op.s_groups = nullptr;
-  op.state = state;
-  op.changed = changed_out;
-  op.ctrl = &ctrl;
-  op.local_alive = 0;
-  emu_launch(k_compact<PciGroupHealthOp, KVG_BLOCK, C_ROWS>, dim3((unsigned)(tiles ? tiles : 1)), KVG_BLOCK, op, st.data(),
-             17u);
-  ctrl_out[0] = ctrl.n_changed;
-  ctrl_out[1] = ctrl.n_alive;
-  return 0;
+  return health_compact(GroupHealthRule{groups, n_groups}, recs, n, state, changed_out, ctrl_out, 17u);
 }
 
 // K5 (kvg_dev_scan_mdev up to the survivor list): type dictionary -> labels -> canonical ids, then the

@@ -1,21 +1,22 @@
 """Latency of the vGPU health re-scan (kvg_health_rescan_mdev) and of the passthrough health re-scan by IOMMU group
-(kvg_health_rescan_groups) in a 1 kHz poll loop, beside the PCI health re-scan of BASELINE.json config 5
-(kvg_health_rescan, 10,000 records) in the same process.
+(kvg_health_rescan_groups) in a 1 kHz poll loop, beside the PCI health re-scan (kvg_health_rescan; --pci-sizes, by
+default 10,000 records as in BASELINE.json config 5 and 65,536, which runs the look-back form) in the same process.
 
 The group leg (--group-sizes) puts 4 functions in each group, gives every group up to the 4,096-handle cap a node,
 flips the driver of 10 records per tick, makes one node vanish every 100 ticks and brings it back 50 ticks later,
 and checks every tick against the numpy state machine of tests/health_groups_ref.py (outside the timed span).  Up to
-32,768 records it runs k_health_small<PciGroupHealthRec>, at 65,536 k_compact<PciGroupHealthOp, 256, 8>.
+32,768 records it runs k_health_small<GroupHealthRule>, at 65,536 k_compact<HealthOp<GroupHealthRule>, 256, 8>.
 
 Each tick flips the type / parent read-error bits of 10 records of a pinned snapshot, and every 100th tick carries one
 XID parent handle.  The host wall time of each call is recorded from "snapshot in the pinned buffer" to "transitions on
 the host" (the call returns with them); 50 warm-up ticks, whose results are also checked against the numpy state
 machine of tests/health_mdev_ref.py, precede the timed ones.  Sizes up to 32,768 records run the one-CTA
-k_health_small<MdevHealthRec>; 65,536 (the config-3 vGPU count) runs k_compact<MdevHealthOp, 256, 8>.  The card's
+k_health_small<MdevHealthRule>; 65,536 (the config-3 vGPU count) runs k_compact<HealthOp<MdevHealthRule>, 256, 8>.
+The PCI leg flips the driver of 10 records per tick and checks its warm-up ticks against numpy.  The card's
 name, power limit and maximum SM clock are read with a read-only nvidia-smi query in the same run.
 
-    python tools/time_health_mdev.py [--sizes 10000,32768,65536] [--group-sizes 10000,32768,65536] [--ticks 10000]
-                                     [--out DIR]
+    python tools/time_health_mdev.py [--sizes 10000,32768,65536] [--group-sizes 10000,32768,65536]
+                                     [--pci-sizes 10000,65536] [--ticks 10000] [--out DIR]
 """
 import argparse
 import ctypes as C
@@ -100,13 +101,12 @@ def mdev_leg(ctx, n, ticks):
         assert r.n_alive == want.n_alive and np.array_equal(got, want.changed), "parity at %d records" % n
 
     out = poll_loop(call, mutate, ticks, check)
-    out["path"] = "k_health_small<MdevHealthRec>" if n <= 32768 else "k_compact<MdevHealthOp, 256, 8>"
+    out["path"] = "k_health_small<MdevHealthRule>" if n <= 32768 else "k_compact<HealthOp<MdevHealthRule>, 256, 8>"
     return out
 
 
-def pci_leg(ctx, ticks, ids):
+def pci_leg(ctx, n, ticks, ids):
     lib = kvgpu.load()
-    n = 10_000
     buf, ptr = pinned(n, 16)
     view = buf.numpy().view(kvgpu.PCI_REC)
     view[:] = O.gen_pci(0, n, ids, 12)
@@ -128,11 +128,12 @@ def pci_leg(ctx, ticks, ids):
         now = util.pci_alive(view)
         idx = np.nonzero(now != prev[0])[0]
         got = np.ctypeslib.as_array(C.cast(r.changed, C.POINTER(C.c_uint32)), (r.n_changed,)) if r.n_changed else np.zeros(0, np.uint32)
-        assert np.array_equal(got, (idx.astype(np.uint32) << 1) | now[idx].astype(np.uint32)), "PCI parity"
+        assert r.n_alive == now.sum(), "PCI parity at %d records" % n
+        assert np.array_equal(got, (idx.astype(np.uint32) << 1) | now[idx].astype(np.uint32)), "PCI parity at %d records" % n
         prev[0] = now
 
     out = poll_loop(call, mutate, ticks, check)
-    out.update(devices=n, path="k_health_small<PciHealthRec>")
+    out["path"] = "k_health_small<PciHealthRule>" if n <= 32768 else "k_compact<HealthOp<PciHealthRule>, 256, 8>"
     return out
 
 
@@ -174,7 +175,7 @@ def groups_leg(ctx, n, ticks, ids):
 
     out = poll_loop(call, mutate, ticks, check, check_all=True)
     out.update(groups_with_node=len(all_nodes),
-               path="k_health_small<PciGroupHealthRec>" if n <= 32768 else "k_compact<PciGroupHealthOp, 256, 8>")
+               path="k_health_small<GroupHealthRule>" if n <= 32768 else "k_compact<HealthOp<GroupHealthRule>, 256, 8>")
     return out
 
 
@@ -182,6 +183,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--sizes", default="10000,32768,65536")
     ap.add_argument("--group-sizes", default="10000,32768,65536")
+    ap.add_argument("--pci-sizes", default="10000,65536")
     ap.add_argument("--ticks", type=int, default=10_000)
     ap.add_argument("--out", default="health_mdev_out", help="directory for health_mdev.json")
     a = ap.parse_args()
@@ -191,7 +193,7 @@ def main():
     ids = O.nv_ids(util.pciids_text())
     out = {"card": card, "poll_hz": 1000, "ticks": a.ticks, "warmup": WARMUP, "flips_per_tick": 10,
            "xid_every": 100, "what": "host wall time from snapshot-in-pinned-buffer to transitions on the host",
-           "mdev": {}, "groups": {}}
+           "mdev": {}, "groups": {}, "pci": {}}
     with kvgpu.Context(0) as ctx:
         for n in [int(s) for s in a.sizes.split(",") if s]:
             out["mdev"][n] = mdev_leg(ctx, n, a.ticks)
@@ -199,8 +201,9 @@ def main():
         for n in [int(s) for s in a.group_sizes.split(",") if s]:
             out["groups"][n] = groups_leg(ctx, n, a.ticks, ids)
             print("groups", n, json.dumps(out["groups"][n]), flush=True)
-        out["pci_config5"] = pci_leg(ctx, a.ticks, ids)
-        print("pci", json.dumps(out["pci_config5"]), flush=True)
+        for n in [int(s) for s in a.pci_sizes.split(",") if s]:
+            out["pci"][n] = pci_leg(ctx, n, a.ticks, ids)
+            print("pci", n, json.dumps(out["pci"][n]), flush=True)
     os.makedirs(a.out, exist_ok=True)
     with open(os.path.join(a.out, "health_mdev.json"), "w") as f:
         json.dump(out, f, indent=1)
