@@ -18,6 +18,9 @@
  *                                            NVML XID critical errors, generic_vgpu_device_plugin.go:280-385
  *   kvg_health_rescan_groups              <- the passthrough health check: Create / Remove / Rename of the IOMMU
  *                                            group's VFIO node, generic_device_plugin.go:611-690
+ *   kvg_health_rescan_*_keyed             <- the same two checks with the state kept per UUID / address, so it
+ *                                            survives re-scans that change the device list (the reference never
+ *                                            re-scans)
  *   kvg_scan_pci_delta                    <- (no reference equivalent: the reference never re-scans)
  *   kvg_scan_mdev_delta                   <- (no reference equivalent: createVgpuIDMap runs once)
  *   kvg_comm_*, kvg_scan_pci_sharded      <- (no reference equivalent; BASELINE.json config 4)
@@ -425,6 +428,40 @@ int kvg_health_mdev_reset(kvg_ctx *ctx);
 int kvg_health_rescan_groups(kvg_ctx *ctx, const kvg_pci_rec *recs, size_t n, const uint32_t *group_nodes,
                              size_t n_nodes, kvg_health_delta **delta);
 int kvg_health_groups_reset(kvg_ctx *ctx);
+
+/* Keyed health re-scans: kvg_health_rescan_mdev and kvg_health_rescan_groups with the state kept per device KEY
+ * instead of per record index, so a device keeps its state while the list of records around it changes (a vGPU
+ * created on another GPU does not clear the XID marks of the vGPUs already listed).
+ *
+ * Key: for mdev records the UUID, compared as 16 big-endian bytes (the order of kvg_scan_mdev_delta); for PCI records
+ * kvg_pci_rec.addr as a uint32.  Within one call the keys must ascend strictly.
+ *
+ * State: each kind keeps a list of (key, state byte) in ascending key order, empty at first.  It is separate from the
+ * index-keyed states and from every scan and delta: none of those calls or their resets touch it, and these calls
+ * touch none of theirs.  For each record i of a call, with key k_i:
+ *
+ *   prior_i = the state byte of k_i in the previous list, or 0 if k_i is absent from it
+ *   s_i     = the next state of the index-keyed rule from record i and prior_i (kvg_health_rescan_mdev with the XID
+ *             parents xid_parents; kvg_health_rescan_groups with the standing node set group_nodes)
+ *   record i is listed iff bit 0 (healthy) of s_i and prior_i differ
+ *
+ * The list then becomes {(k_i, s_i)}: keys missing from this call are forgotten.  So a vGPU keeps its XID mark while
+ * it stays in the list and present; one that leaves the list and returns later starts unmarked.  When every call
+ * carries the same key list, each delta is byte for byte that of the index-keyed call from a fresh state.
+ *
+ * The delta is kvg_health_delta: changed[] holds (i << 1) | healthy_now, i a position in THIS call's records,
+ * ascending; n_alive counts the records healthy now.  n = 0 empties the list and returns an empty delta (the reset).
+ *
+ * Refused with KVG_EINVAL, the list unchanged and nothing handed out: keys not strictly ascending (found on the device;
+ * text in kvg_last_error), n_xid > KVG_HEALTH_MAX_XID or n_nodes > KVG_HEALTH_MAX_GROUPS, a NULL set with a non-zero
+ * count.
+ *
+ * Cost as the index-keyed calls: up to 32,768 records and with kernel timing off, one kernel launch with no driver
+ * synchronisation, pinned `recs` read in place (16-byte aligned, not checked); above that the look-back form. */
+int kvg_health_rescan_mdev_keyed(kvg_ctx *ctx, const kvg_mdev_rec *recs, size_t n, uint32_t n_types,
+                                 const uint32_t *xid_parents, size_t n_xid, kvg_health_delta **delta);
+int kvg_health_rescan_groups_keyed(kvg_ctx *ctx, const kvg_pci_rec *recs, size_t n,
+                                   const uint32_t *group_nodes, size_t n_nodes, kvg_health_delta **delta);
 
 /* Scan `recs` and diff the result against the previous one, keyed by survivor address.
  *

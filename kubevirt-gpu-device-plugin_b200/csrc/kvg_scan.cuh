@@ -10,6 +10,7 @@
 //                            PciHealthRule (alive), MdevHealthRule (present / XID-marked vGPUs),
 //                            GroupHealthRule (alive and the IOMMU group's VFIO node exists)
 //   k_health_small<Rule>   K6 at poll-loop sizes: one CTA, TMA-staged, transitions into mapped host memory
+//                          (Keyed<Rule>, either form: the prior state joined by UUID / address instead of by index)
 //   k_mdev_labels / _canon K5: label rule (:341-342) + merge of equal labels
 //   k_gen_*                counter-based synthetic snapshots (twins of oracle/kvg_oracle.c kvo_gen_*)
 #pragma once
@@ -25,7 +26,8 @@ struct ScanCtrl {
   uint32_t n_own[2];      // sharded scans: records in the owned list of ordering 0 / 1
   uint32_t own_max[2];    // sharded scans: their largest keys (radix plan)
   uint32_t n_gathered;    // sharded scans, NCCL mode: length of the all-gathered survivor list
-  uint32_t reserved[3];
+  uint32_t key_err;       // keyed health, look-back form: the keys do not ascend strictly
+  uint32_t reserved[2];
   uint32_t n_surv;        // survivors of the classify kernel
   uint32_t max_group;     // max iommu group / parent among survivors (radix pass count)
   uint32_t max_devkey;    // max device / type key among survivors
@@ -274,21 +276,99 @@ struct GroupHealthRule {
   }
 };
 
+// ---- where the prior state byte comes from -----------------------------------------------------
+// A rule as it stands is index-keyed: the prior byte of record i is state[i], updated in place.  Keyed<Rule> is the
+// same rule with the prior byte joined by the record's key (kvg_health_rescan_mdev_keyed / _groups_keyed): the
+// previous call's list is (prev_key, prev_state)[0..n_prev), ascending by key; this call writes its own keys to
+// `key` and its state bytes to the kernel's `state` (the other slot), every record, so keys absent now are forgotten.
+// The kernels test KEYED_RULE<Rule>; an index rule compiles exactly the code it compiled before.
+//   HealthKey<Rule>: the key type, the unit of the record holding it, and its order
+template <class Rule>
+struct HealthKey;
+// the UUID (unit 0 of the 32-byte record) as a 128-bit big-endian number: the order of kvg_scan_mdev_delta
+template <>
+struct HealthKey<MdevHealthRule> {
+  using Key = uint4;
+  static constexpr uint32_t UNIT = 0;
+  __device__ __forceinline__ static Key of(const uint4& u) { return u; }
+  __device__ __forceinline__ static bool eq(const Key& a, const Key& b) {
+    return ((a.x ^ b.x) | (a.y ^ b.y) | (a.z ^ b.z) | (a.w ^ b.w)) == 0;
+  }
+  __device__ __forceinline__ static bool lt(const Key& a, const Key& b) {
+    const uint32_t a0 = __byte_perm(a.x, 0, 0x0123), b0 = __byte_perm(b.x, 0, 0x0123);
+    if (a0 != b0) return a0 < b0;
+    const uint32_t a1 = __byte_perm(a.y, 0, 0x0123), b1 = __byte_perm(b.y, 0, 0x0123);
+    if (a1 != b1) return a1 < b1;
+    const uint32_t a2 = __byte_perm(a.z, 0, 0x0123), b2 = __byte_perm(b.z, 0, 0x0123);
+    if (a2 != b2) return a2 < b2;
+    return __byte_perm(a.w, 0, 0x0123) < __byte_perm(b.w, 0, 0x0123);
+  }
+};
+// the address handle (r.x of the 16-byte PCI record)
+template <>
+struct HealthKey<GroupHealthRule> {
+  using Key = uint32_t;
+  static constexpr uint32_t UNIT = 0;
+  __device__ __forceinline__ static Key of(const uint4& u) { return u.x; }
+  __device__ __forceinline__ static bool eq(Key a, Key b) { return a == b; }
+  __device__ __forceinline__ static bool lt(Key a, Key b) { return a < b; }
+};
+
+template <class Rule>
+struct Keyed : Rule {
+  using K = HealthKey<Rule>;
+  using Key = typename K::Key;
+  const Key* prev_key;
+  const uint8_t* prev_state;
+  uint32_t n_prev;
+  Key* key;       // this call's keys, [n]
+  uint32_t* err;  // look-back form: set when a key does not exceed its predecessor's (ScanCtrl::key_err)
+  // the prior byte of `k`, the key of record i: the same position first (the list did not change), else a binary
+  // search of the previous keys (L2-resident at poll-loop sizes); 0 for a key the previous list lacks
+  __device__ __forceinline__ uint32_t search(const Key& k) const {
+    uint32_t lo = 0, hi = n_prev;
+    while (lo < hi) {
+      const uint32_t mid = (lo + hi) >> 1;
+      if (K::lt(__ldg(&prev_key[mid]), k))
+        lo = mid + 1;
+      else
+        hi = mid;
+    }
+    return lo < n_prev && K::eq(__ldg(&prev_key[lo]), k) ? __ldg(&prev_state[lo]) : 0u;
+  }
+  __device__ __forceinline__ uint32_t find(const Key& k, uint32_t i) const {
+    return i < n_prev && K::eq(__ldg(&prev_key[i]), k) ? (uint32_t)__ldg(&prev_state[i]) : search(k);
+  }
+};
+template <class Rule>
+constexpr bool KEYED_RULE = false;
+template <class Rule>
+constexpr bool KEYED_RULE<Keyed<Rule>> = true;
+// dynamic shared memory the small form adds for a keyed rule: the ascent error flag
+template <class Rule>
+constexpr uint32_t KEYED_SMEM = 0;
+template <class Rule>
+constexpr uint32_t KEYED_SMEM<Keyed<Rule>> = 16;
+
 // the look-back form (above HEALTH_SMALL_MAX records, or with kernel timing on): k_compact<HealthOp<Rule>, 256, 8>.
 // Item.x = new state | old state byte << W.  The state byte is written whenever it changes, a transition or not (a
 // marked vGPU that vanishes loses its mark without a health change); a change of bit 0 is listed.  A one-bit state
 // changes only with a transition, so emit writes it, where pred writes a wider one.  That, and reading state[i] as an
 // argument of next() (a rule that ignores it loads it after its own work), keeps the group instantiation at 48
 // registers: with the write in pred for every width, or the byte read first, ptxas takes 53 to 56.
+// A keyed rule joins the prior byte in load (which also reads the key's unit when the rule reads another), checks
+// that the key exceeds the previous record's, and writes the record's key and new byte to this call's slot there:
+// every record, so pred and emit write no state.
 template <class Rule>
 struct HealthOp {
   using Item = uint4;
   static constexpr uint32_t W = Rule::STATE_BITS;
+  static constexpr bool KEYED = KEYED_RULE<Rule>;
   const uint4* recs;  // Rule::UNITS x uint4 per record
   uint32_t n;
   Rule rule;
   const uint32_t* set;  // the rule's set in shared memory (compact_enter); unused without one
-  uint8_t* state;       // one byte per record, updated in place
+  uint8_t* state;       // one byte per record, updated in place (keyed: this call's slot)
   uint32_t* changed;
   ScanCtrl* ctrl;
   uint32_t local_alive;
@@ -296,19 +376,31 @@ struct HealthOp {
   __device__ __forceinline__ Item load(uint32_t i, bool ok) const {
     if (!ok) return make_uint4(0, 0, 0, 0);
     uint4 r = ld_stream(recs + (size_t)i * Rule::UNITS + Rule::UNIT);
-    r.x = rule.next(r, state[i], set) | ((uint32_t)state[i] << W);
+    if constexpr (KEYED) {
+      using K = typename Rule::K;
+      constexpr uint32_t KU = K::UNIT;
+      const typename K::Key key = K::of(KU == Rule::UNIT ? r : ld_stream(recs + (size_t)i * Rule::UNITS + KU));
+      if (i && !K::lt(K::of(__ldg(recs + (size_t)(i - 1) * Rule::UNITS + KU)), key)) *rule.err = 1u;
+      const uint32_t was = rule.find(key, i), s = rule.next(r, was, set);
+      rule.key[i] = key;
+      state[i] = (uint8_t)s;
+      r.x = s | (was << W);
+    } else {
+      r.x = rule.next(r, state[i], set) | ((uint32_t)state[i] << W);
+    }
     return r;
   }
   __device__ __forceinline__ bool pred(const Item& r, uint32_t i) {
     const uint32_t now = r.x & ((1u << W) - 1), was = r.x >> W;
     local_alive += now & 1u;
     if constexpr (W == 1) return now != was;
-    if (now != was) state[i] = (uint8_t)now;
+    if constexpr (!KEYED)
+      if (now != was) state[i] = (uint8_t)now;
     return ((now ^ was) & 1u) != 0;
   }
   __device__ __forceinline__ void emit(uint32_t pos, const Item& r, uint32_t i, uint32_t) {
     changed[pos] = (i << 1) | (r.x & 1u);
-    if constexpr (W == 1) state[i] = (uint8_t)(r.x & 1u);
+    if constexpr (W == 1 && !KEYED) state[i] = (uint8_t)(r.x & 1u);
   }
   __device__ __forceinline__ void tile_epilogue() {
     uint32_t a = warp_sum(local_alive);
@@ -328,18 +420,31 @@ __device__ __forceinline__ void compact_enter(HealthOp<Rule>& op) {
 }
 template <>
 constexpr int COMPACT_MIN_BLOCKS<HealthOp<GroupHealthRule>> = 1;
+template <>
+constexpr int COMPACT_MIN_BLOCKS<HealthOp<Keyed<GroupHealthRule>>> = 1;
 
 // K6 at poll-loop sizes (BASELINE.json config 5: 10,000 devices at 1 kHz): ONE CTA, one launch, one host
 // synchronisation.  The records are read where the host left them (mapped pinned memory: zero-copy over PCIe,
 // every load of a thread in flight at once), the transitions are written — in record order — straight into
 // the host-visible result block, and the two counters follow.  No staging copy, no look-back, no second
 // device-to-host copy.  Dynamic shared memory: the stage, then the rule's set.
+// the key type of a keyed rule (an index rule has none: a placeholder the compiler drops)
+template <class Rule>
+struct KeyOfT {
+  using T = uint32_t;
+};
+template <class Rule>
+struct KeyOfT<Keyed<Rule>> {
+  using T = typename Keyed<Rule>::Key;
+};
+template <class Rule>
+using KeyOf = typename KeyOfT<Rule>::T;
 constexpr uint32_t HEALTH_SMALL_THREADS = 1024;
 constexpr uint32_t HEALTH_SMALL_ROWS = 32;                                        // rows of 1024 records
 constexpr uint32_t HEALTH_SMALL_MAX = HEALTH_SMALL_THREADS * HEALTH_SMALL_ROWS;  // 32,768 records
 constexpr uint32_t HEALTH_STAGE_BYTES = 192u << 10;                               // one TMA round
 template <class Rule>
-constexpr uint32_t HEALTH_SMALL_SMEM = HEALTH_STAGE_BYTES + Rule::SET_CAP * 4;
+constexpr uint32_t HEALTH_SMALL_SMEM = HEALTH_STAGE_BYTES + Rule::SET_CAP * 4 + KEYED_SMEM<Rule>;
 template <class Rule>
 __global__ void __launch_bounds__(HEALTH_SMALL_THREADS) k_health_small(Rule rule, const uint4* __restrict__ recs,
                                                                        uint32_t n, uint8_t* __restrict__ state,
@@ -359,11 +464,15 @@ __global__ void __launch_bounds__(HEALTH_SMALL_THREADS) k_health_small(Rule rule
   __shared__ uint32_t s_scan[NW], s_alv[NW];
   const uint4* stage = reinterpret_cast<const uint4*>(hs_smem);
   uint32_t* set = reinterpret_cast<uint32_t*>(hs_smem + HEALTH_STAGE_BYTES);
+  // keyed: the ascent error flag behind the set; thread 0's copy of the last key of the previous round
+  [[maybe_unused]] uint32_t* keyed_err = reinterpret_cast<uint32_t*>(hs_smem + HEALTH_STAGE_BYTES + Rule::SET_CAP * 4);
+  [[maybe_unused]] KeyOf<Rule> keyed_last{};
   const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const uint32_t rows = (n + HEALTH_SMALL_THREADS - 1) / HEALTH_SMALL_THREADS;
   if (tid == 0) {
     mbar_init(&s_bar, 1);
     mbar_fence_init();
+    if constexpr (KEYED_RULE<Rule>) *keyed_err = 0;
   }
   if constexpr (Rule::SET_CAP > 0) load_sorted_set(set, rule.set, rule.n_set);
   __syncthreads();
@@ -374,16 +483,25 @@ __global__ void __launch_bounds__(HEALTH_SMALL_THREADS) k_health_small(Rule rule
     const uint32_t first = r0 * HEALTH_SMALL_THREADS;
     const uint32_t cnt = min(n - first, SR * HEALTH_SMALL_THREADS);
     if (tid == 0) {
+      if constexpr (KEYED_RULE<Rule>)  // the stage still holds the previous (full) round
+        if (r0) keyed_last = Rule::K::of(stage[(SR * HEALTH_SMALL_THREADS - 1) * U + Rule::K::UNIT]);
       mbar_arrive_expect_tx(&s_bar, cnt * 16 * U);
       for (uint32_t off = 0; off < cnt * 16 * U; off += 16384)
         tma_load_1d(hs_smem + off, reinterpret_cast<const uint8_t*>(recs + first * U) + off,
                     min(16384u, cnt * 16 * U - off), &s_bar);
     }
     uint32_t was[SR];
+    [[maybe_unused]] KeyOf<Rule> pk[SR];
 #pragma unroll
     for (uint32_t k = 0; k < SR; k++) {  // the previous state (device memory) meanwhile
       const uint32_t i = first + k * HEALTH_SMALL_THREADS + tid;
-      was[k] = i < n ? state[i] : 0;
+      if constexpr (KEYED_RULE<Rule>) {  // keyed: the previous list's entry at the same position
+        const bool same = i < n && i < rule.n_prev;
+        pk[k] = same ? __ldg(&rule.prev_key[i]) : KeyOf<Rule>{};
+        was[k] = same ? __ldg(&rule.prev_state[i]) : 0;
+      } else {
+        was[k] = i < n ? state[i] : 0;
+      }
     }
     mbar_wait(&s_bar, phase);
     phase ^= 1;
@@ -392,11 +510,27 @@ __global__ void __launch_bounds__(HEALTH_SMALL_THREADS) k_health_small(Rule rule
       if (r0 + k < rows) {  // uniform
         const uint32_t i = first + k * HEALTH_SMALL_THREADS + tid;
         const bool in = i < n;
+        if constexpr (KEYED_RULE<Rule>) {
+          // the join (a miss at the same position searches the previous keys), the ascent check against the
+          // record before (the stage, or the last key of the previous round), and this call's key
+          using K = typename Rule::K;
+          const uint32_t j = k * HEALTH_SMALL_THREADS + tid;
+          const KeyOf<Rule> key = K::of(stage[j * U + K::UNIT]);
+          if (in) {
+            if (!(i < rule.n_prev && K::eq(pk[k], key))) was[k] = rule.search(key);
+            if (j ? !K::lt(K::of(stage[(j - 1) * U + K::UNIT]), key) : (r0 && !K::lt(keyed_last, key))) *keyed_err = 1u;
+            rule.key[i] = key;
+          }
+        }
         // (lanes past n compute s from stale stage bytes and use none of it)
         const uint32_t s = rule.next(stage[(k * HEALTH_SMALL_THREADS + tid) * U + Rule::UNIT], was[k], set);
         const bool now = in && (s & 1u) != 0;
         const bool chg = in && (now ? 1u : 0u) != (was[k] & 1u);
-        if (in && s != was[k]) state[i] = (uint8_t)s;
+        if constexpr (KEYED_RULE<Rule>) {
+          if (in) state[i] = (uint8_t)s;  // this call's slot: every record
+        } else {
+          if (in && s != was[k]) state[i] = (uint8_t)s;
+        }
         const uint32_t bc = __ballot_sync(KVG_FULL, chg), bn = __ballot_sync(KVG_FULL, now);
         if (lane == 0) {
           s_bal[r0 + k][warp] = bc;
@@ -437,6 +571,7 @@ __global__ void __launch_bounds__(HEALTH_SMALL_THREADS) k_health_small(Rule rule
   if (tid == 0) {
     hdr_host[0] = alive;
     hdr_host[1] = total;
+    if constexpr (KEYED_RULE<Rule>) hdr_host[3] = *keyed_err;
     __threadfence_system();
     *((volatile uint32_t*)&hdr_host[2]) = seq;  // the host polls this word: no driver call on the way back
   }

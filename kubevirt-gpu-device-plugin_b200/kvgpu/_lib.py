@@ -164,6 +164,8 @@ def load() -> C.CDLL:
         "kvg_health_mdev_reset": (C.c_int, [vp]),
         "kvg_health_rescan_groups": (C.c_int, [vp, vp, sz, vp, sz, P(P(HealthDeltaC))]),
         "kvg_health_groups_reset": (C.c_int, [vp]),
+        "kvg_health_rescan_mdev_keyed": (C.c_int, [vp, vp, sz, u32, vp, sz, P(P(HealthDeltaC))]),
+        "kvg_health_rescan_groups_keyed": (C.c_int, [vp, vp, sz, vp, sz, P(P(HealthDeltaC))]),
         "kvg_scan_pci_delta": (C.c_int, [vp, vp, sz, P(P(PciResultC)), P(P(PciDeltaC))]),
         "kvg_scan_pci_delta_reset": (C.c_int, [vp]),
         "kvg_scan_mdev_delta": (C.c_int, [vp, vp, sz, P(TypeDict), P(P(MdevResultC)), P(P(MdevDeltaC))]),

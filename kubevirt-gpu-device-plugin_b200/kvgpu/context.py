@@ -299,6 +299,27 @@ class Context:
     def health_groups_reset(self):
         self._ck(self._lib.kvg_health_groups_reset(self._h))
 
+    def health_rescan_mdev_keyed(self, recs: np.ndarray, n_types: int, xid_parents=()) -> HealthDelta:
+        """health_rescan_mdev with the state kept per UUID (include/kvgpu.h kvg_health_rescan_mdev_keyed): the UUIDs
+        of `recs` must ascend strictly (big-endian bytes); a vGPU keeps its XID mark while it stays in the list,
+        whatever else is added or removed.  `changed` indexes this call's records.  An empty `recs` resets."""
+        recs = np.ascontiguousarray(recs, dtype=L.MDEV_REC)
+        x = np.ascontiguousarray(np.asarray(xid_parents, dtype=np.uint32).reshape(-1))
+        res = C.POINTER(L.HealthDeltaC)()
+        self._ck(self._lib.kvg_health_rescan_mdev_keyed(self._h, recs.ctypes.data, len(recs), int(n_types),
+                                                        x.ctypes.data if len(x) else None, len(x), C.byref(res)))
+        return self._take_health(res)
+
+    def health_rescan_groups_keyed(self, recs: np.ndarray, group_nodes=()) -> HealthDelta:
+        """health_rescan_groups with the state kept per address (include/kvgpu.h kvg_health_rescan_groups_keyed): the
+        addresses of `recs` must ascend strictly.  `changed` indexes this call's records.  An empty `recs` resets."""
+        recs = np.ascontiguousarray(recs, dtype=L.PCI_REC)
+        g = np.ascontiguousarray(np.asarray(group_nodes, dtype=np.uint32).reshape(-1))
+        res = C.POINTER(L.HealthDeltaC)()
+        self._ck(self._lib.kvg_health_rescan_groups_keyed(self._h, recs.ctypes.data, len(recs),
+                                                          g.ctypes.data if len(g) else None, len(g), C.byref(res)))
+        return self._take_health(res)
+
     def _take_pci_delta(self, dl) -> PciDelta:
         d = dl.contents
         delta = PciDelta(int(d.n_prev), L._arr(d.changes, int(d.n_changes), L.PCI_CHANGE),

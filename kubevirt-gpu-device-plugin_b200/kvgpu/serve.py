@@ -16,7 +16,7 @@ Allocate" is testable end to end in an image without a Go toolchain.
 Nothing here computes on the CPU what the scan computes on the GPU: the maps come from
 plugin.DiscoveryScan (libkvgpu.so); the re-validation's classification goes through
 Context.scan_pci (K3); the health feeds through Context.health_rescan, Context.health_rescan_mdev and
-Context.health_rescan_groups (K6); the
+Context.health_rescan_groups and their keyed forms (K6); the
 hot-plug feeds through Context.scan_pci_delta and Context.scan_mdev_delta (K7).
 """
 from __future__ import annotations
@@ -34,7 +34,7 @@ from . import _lib as L
 from . import dpapi
 from .plugin import (DEVICE_NAMESPACE, GPU_PREFIX, VGPU_PREFIX, Maps, PluginSpec, ReferencePanic, _read_id,
                      _read_link, _read_vgpu_raw, _rebuild_mdev_maps, _rebuild_pci_maps, apply_mdev_delta,
-                     apply_pci_delta, plugin_specs_from_maps)
+                     apply_pci_delta, format_uuid, parse_bdf, plugin_specs_from_maps)
 
 VFIO_DEVICE_PATH = "/dev/vfio"      # generic_device_plugin.go:54
 IOMMU_DEVICE_PATH = "/dev/iommu"    # :55
@@ -818,6 +818,98 @@ class GroupHealthFeed(_PollFeed):
             self._bdfs = bdfs
         delta = self.health_rescan_groups(snap.recs, nodes)
         return _send_health(devs, delta, arming)
+
+
+def _uuid_key(s: str) -> bytes:
+    """The UUID bytes of a canonical (lower-case, hyphenated) UUID string; ValueError naming anything else."""
+    h = s.replace("-", "") if isinstance(s, str) else ""
+    if len(s) == 36 and len(h) == 32 and all(c in "0123456789abcdef" for c in h) and format_uuid(bytes.fromhex(h)) == s:
+        return bytes.fromhex(h)
+    raise ValueError("not a canonical vGPU UUID, so it has no stable key: %r" % (s,))
+
+
+def _bdf_key(s: str) -> int:
+    """The packed address of a canonical BDF string; ValueError naming anything else."""
+    p = parse_bdf(s) if isinstance(s, str) else None
+    if p is None:
+        raise ValueError("not a canonical PCI address, so it has no stable key: %r" % (s,))
+    return p
+
+
+def _by_key(plugins, key):
+    """[(device, plugin)] of every advertised device, ascending by key(device ID): the record order of a keyed call."""
+    devs = [(d, p) for p in plugins for d in p.devs]
+    keys = [key(d.ID) for d, _ in devs]
+    return [devs[k] for k in sorted(range(len(devs)), key=keys.__getitem__)]
+
+
+def _send_keyed_health(devs, delta, prev_ids) -> int:
+    """Route a keyed health delta over [(device, plugin)] (record k = devs[k]).  A device whose ID was in the previous
+    tick's list gets each transition; a new one (prior state "nothing", so it is listed iff it is healthy now) is sent
+    only when that differs from what its plugin advertises.  A tick whose list did not change walks the listed
+    records only.  Returns the number of events sent."""
+    sent = 0
+    listed_new = set()
+    for w in delta.changed:
+        k, ok = int(w) >> 1, int(w) & 1
+        d, plugin = devs[k]
+        if d.ID not in prev_ids:
+            listed_new.add(k)
+            if d.health == dpapi.HEALTHY:
+                continue
+        (plugin.healthy if ok else plugin.unhealthy)(d.ID)
+        sent += 1
+    ids = [d.ID for d, _ in devs]
+    if len(ids) != len(prev_ids) or not prev_ids.issuperset(ids):
+        for k, i in enumerate(ids):   # new and not listed: unhealthy now
+            if i not in prev_ids and k not in listed_new and devs[k][0].health == dpapi.HEALTHY:
+                devs[k][1].unhealthy(i)
+                sent += 1
+    return sent
+
+
+class KeyedVgpuHealthFeed(VgpuHealthFeed):
+    """VgpuHealthFeed on Context.health_rescan_mdev_keyed: the state is kept per UUID, so it survives changes of the
+    advertised list (MdevRescanFeed's set_devices).  A vGPU marked by an XID stays unhealthy while it stays advertised,
+    whatever other vGPUs are created or destroyed; only its own path being created again clears the mark.
+
+    Construct it as VgpuHealthFeed, with `health_rescan_mdev` = Context.health_rescan_mdev_keyed.  tick(): order the
+    advertised vGPUs by UUID bytes, snapshot them in that order, one keyed call (never an arming call), then each
+    transition of a UUID that was advertised on the previous tick; a new UUID is sent only when the kernel's health
+    differs from what its plugin advertises.  Every advertised ID must be a canonical UUID (ValueError names the first
+    that is not): a Walk-index handle is not a stable identity, so names that are not UUIDs need VgpuHealthFeed, whose
+    state follows the record index."""
+
+    def tick(self) -> int:
+        devs = _by_key(self.plugins, _uuid_key)
+        uuids = [d.ID for d, _ in devs]
+        snap = self.snapshot(uuids, self.intern)
+        with self._lock:
+            buses, self._queued = self._queued, []
+        xids = [self.intern[b] for b in buses if b in self.intern]
+        delta = self.health_rescan_mdev(snap.recs, len(snap.raw_types), xids)
+        prev, self._uuids = self._uuids or frozenset(), frozenset(uuids)
+        return _send_keyed_health(devs, delta, prev)
+
+
+class KeyedGroupHealthFeed(GroupHealthFeed):
+    """GroupHealthFeed on Context.health_rescan_groups_keyed: the state is kept per address, so a change of the
+    advertised list costs no arming call and no sweep over every device.
+
+    Construct it as GroupHealthFeed, with `health_rescan_groups` = Context.health_rescan_groups_keyed.  tick(): order
+    the advertised devices by packed BDF, snapshot them in that order, list the nodes, one keyed call, then each
+    transition of an address advertised on the previous tick; a new address is sent only when the kernel's health
+    differs from what its plugin advertises.  Every advertised ID must be a canonical BDF (ValueError names the first
+    that is not); other names need GroupHealthFeed."""
+
+    def tick(self) -> int:
+        devs = _by_key(self.plugins, _bdf_key)
+        bdfs = [d.ID for d, _ in devs]
+        snap = self.snapshot(bdfs, self.intern)
+        nodes = self.list_nodes(self.intern)
+        delta = self.health_rescan_groups(snap.recs, nodes)
+        prev, self._bdfs = self._bdfs or frozenset(), frozenset(bdfs)
+        return _send_keyed_health(devs, delta, prev)
 
 
 # ------------------------------------------------------------------------------------------------

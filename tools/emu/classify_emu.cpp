@@ -7,7 +7,8 @@
 #include "../../kubevirt-gpu-device-plugin_b200/csrc/kvg_scan.cuh"
 using namespace kvg;
 
-// K6, both forms of every health rule (kvg_scan.cuh) on the caller's state bytes, transitions in record order.
+// K6, both forms of every health rule (kvg_scan.cuh) on the caller's state bytes, transitions in record order (a keyed
+// rule writes its state bytes to `state`, its keys to the rule's key array).
 // Small form (n <= 32,768): one CTA, transitions + counters written where the host reads them; hdr_out {n_alive,
 // n_changed, seq}.  Look-back form: changed_out has room for n words; ctrl_out {n_changed, n_alive}.  Its grid is one
 // CTA per tile — what compact_grid() picks whenever the tiles fit the GPU, and the only shape a sequential emulation of
@@ -36,11 +37,29 @@ static int health_compact(Rule rule, const uint4* recs, uint32_t n, uint8_t* sta
   op.ctrl = &ctrl;
   op.set = nullptr;
   op.local_alive = 0;
+  if constexpr (KEYED_RULE<Rule>) op.rule.err = &ctrl.key_err;
   emu_launch(k_compact<HealthOp<Rule>, KVG_BLOCK, C_ROWS>, dim3((unsigned)(tiles ? tiles : 1)), KVG_BLOCK, op, st.data(),
              epoch);
   ctrl_out[0] = ctrl.n_changed;
   ctrl_out[1] = ctrl.n_alive;
+  if constexpr (KEYED_RULE<Rule>) ctrl_out[2] = ctrl.key_err;
   return 0;
+}
+
+// Keyed<Rule> over the previous list (prev_key, prev_state)[0..n_prev): this call's keys and state bytes go to key_out /
+// state_out [n]; the caller adopts them as the next previous list only when the ascent flag (hdr_out[3] of the small
+// form, ctrl_out[2] of the look-back form) is 0.
+template <class Rule>
+static Keyed<Rule> keyed(const Rule& base, const void* prev_key, const uint8_t* prev_state, uint32_t n_prev,
+                         void* key_out) {
+  Keyed<Rule> k{};
+  static_cast<Rule&>(k) = base;
+  k.prev_key = (const typename Keyed<Rule>::Key*)prev_key;
+  k.prev_state = prev_state;
+  k.n_prev = n_prev;
+  k.key = (typename Keyed<Rule>::Key*)key_out;
+  k.err = nullptr;
+  return k;
 }
 
 extern "C" {
@@ -105,6 +124,24 @@ int emu_health_mdev_compact(const uint4* recs, uint32_t n, uint32_t n_types, con
   return health_compact(MdevHealthRule{xid, n_xid, n_types}, recs, n, state, changed_out, ctrl_out, 13u);
 }
 
+// The keyed vGPU re-scan (kvg_health_rescan_mdev_keyed): keys = the UUIDs (16 bytes each).  small: hdr_out {n_alive,
+// n_changed, seq, ascent flag}; compact: ctrl_out {n_changed, n_alive, ascent flag}.
+int emu_health_mdev_keyed_small(const uint4* recs, uint32_t n, uint32_t n_types, const uint32_t* xid, uint32_t n_xid,
+                                const uint4* prev_key, const uint8_t* prev_state, uint32_t n_prev, uint4* key_out,
+                                uint8_t* state_out, uint32_t* changed_out, uint32_t* hdr_out) {
+  if (n_xid > KVG_HEALTH_MAX_XID) return -1;
+  return health_small(keyed(MdevHealthRule{xid, n_xid, n_types}, prev_key, prev_state, n_prev, key_out), recs, n,
+                      state_out, changed_out, hdr_out, 19u);
+}
+
+int emu_health_mdev_keyed_compact(const uint4* recs, uint32_t n, uint32_t n_types, const uint32_t* xid, uint32_t n_xid,
+                                  const uint4* prev_key, const uint8_t* prev_state, uint32_t n_prev, uint4* key_out,
+                                  uint8_t* state_out, uint32_t* changed_out, uint32_t* ctrl_out) {
+  if (n_xid > KVG_HEALTH_MAX_XID) return -1;
+  return health_compact(keyed(MdevHealthRule{xid, n_xid, n_types}, prev_key, prev_state, n_prev, key_out), recs, n,
+                        state_out, changed_out, ctrl_out, 23u);
+}
+
 // K6 for passthrough GPUs by IOMMU group (kvg_health_rescan_groups): state = healthy bit.  recs: n x 16 B records;
 // groups: the sorted, deduplicated handles of the groups whose node exists.
 int emu_health_groups_small(const uint4* recs, uint32_t n, const uint32_t* groups, uint32_t n_groups, uint8_t* state,
@@ -117,6 +154,23 @@ int emu_health_groups_compact(const uint4* recs, uint32_t n, const uint32_t* gro
                               uint32_t* changed_out, uint32_t* ctrl_out) {
   if (n_groups > KVG_HEALTH_MAX_GROUPS) return -1;
   return health_compact(GroupHealthRule{groups, n_groups}, recs, n, state, changed_out, ctrl_out, 17u);
+}
+
+// The keyed group re-scan (kvg_health_rescan_groups_keyed): keys = the addresses.  Outputs as the keyed vGPU form's.
+int emu_health_groups_keyed_small(const uint4* recs, uint32_t n, const uint32_t* groups, uint32_t n_groups,
+                                  const uint32_t* prev_key, const uint8_t* prev_state, uint32_t n_prev, uint32_t* key_out,
+                                  uint8_t* state_out, uint32_t* changed_out, uint32_t* hdr_out) {
+  if (n_groups > KVG_HEALTH_MAX_GROUPS) return -1;
+  return health_small(keyed(GroupHealthRule{groups, n_groups}, prev_key, prev_state, n_prev, key_out), recs, n,
+                      state_out, changed_out, hdr_out, 29u);
+}
+
+int emu_health_groups_keyed_compact(const uint4* recs, uint32_t n, const uint32_t* groups, uint32_t n_groups,
+                                    const uint32_t* prev_key, const uint8_t* prev_state, uint32_t n_prev,
+                                    uint32_t* key_out, uint8_t* state_out, uint32_t* changed_out, uint32_t* ctrl_out) {
+  if (n_groups > KVG_HEALTH_MAX_GROUPS) return -1;
+  return health_compact(keyed(GroupHealthRule{groups, n_groups}, prev_key, prev_state, n_prev, key_out), recs, n,
+                        state_out, changed_out, ctrl_out, 31u);
 }
 
 // K5 (kvg_dev_scan_mdev up to the survivor list): type dictionary -> labels -> canonical ids, then the

@@ -15,8 +15,12 @@ k_health_small<MdevHealthRule>; 65,536 (the config-3 vGPU count) runs k_compact<
 The PCI leg flips the driver of 10 records per tick and checks its warm-up ticks against numpy.  The card's
 name, power limit and maximum SM clock are read with a read-only nvidia-smi query in the same run.
 
+--keyed adds the keyed legs (kvg_health_rescan_mdev_keyed / _groups_keyed) in the same process: the same event
+patterns plus one key inserted near the front every 100 ticks, every tick checked; the ticks with an edit are also
+reported on their own.
+
     python tools/time_health_mdev.py [--sizes 10000,32768,65536] [--group-sizes 10000,32768,65536]
-                                     [--pci-sizes 10000,65536] [--ticks 10000] [--out DIR]
+                                     [--pci-sizes 10000,65536] [--ticks 10000] [--keyed] [--out DIR]
 """
 import argparse
 import ctypes as C
@@ -50,10 +54,16 @@ def pinned(n, itemsize):
     return t, t.data_ptr()
 
 
-def poll_loop(call, mutate, ticks, check=None, check_all=False):
+def stats(lat):
+    lat = np.array(lat) * 1e6
+    return {"p50_us": float(np.percentile(lat, 50)), "p99_us": float(np.percentile(lat, 99)), "max_us": float(lat.max())}
+
+
+def poll_loop(call, mutate, ticks, check=None, check_all=False, edit=None):
     """1 kHz loop: mutate the pinned snapshot, time one call; -> latencies in us of the timed ticks.  `check` runs on
-    the warm-up ticks, or on every tick with check_all (outside the timed span, before the wait for the next tick)."""
-    lat = []
+    the warm-up ticks, or on every tick with check_all (outside the timed span, before the wait for the next tick).
+    edit(tick) -> True marks the ticks whose list changed; they are also reported on their own ("edit")."""
+    lat, lat_edit = [], []
     t_next = time.perf_counter()
     for tick in range(ticks + WARMUP):
         xids = mutate(tick)
@@ -65,11 +75,15 @@ def poll_loop(call, mutate, ticks, check=None, check_all=False):
         kvgpu.load().kvg_result_free(res)
         if tick >= WARMUP:
             lat.append(dt)
+            if edit is not None and edit(tick):
+                lat_edit.append(dt)
         t_next += PERIOD
         while time.perf_counter() < t_next:
             pass
-    lat = np.array(lat) * 1e6
-    return {"p50_us": float(np.percentile(lat, 50)), "p99_us": float(np.percentile(lat, 99)), "max_us": float(lat.max())}
+    out = stats(lat)
+    if lat_edit:
+        out["edit"] = dict(stats(lat_edit), ticks=len(lat_edit))
+    return out
 
 
 def mdev_leg(ctx, n, ticks):
@@ -179,12 +193,99 @@ def groups_leg(ctx, n, ticks, ids):
     return out
 
 
+def keyed_leg(ctx, kind, n, ticks, ids, per_group=4):
+    """kvg_health_rescan_mdev_keyed / _groups_keyed on the event pattern of the index-keyed leg of the same kind, plus
+    a list edit every 100 ticks: one key inserted near the front (the records after it move down one place, so every
+    later record misses its same-position hint on that tick).  Keys are spaced two apart so that there is room.  Every
+    tick is checked against the rules of tests/health_mdev_ref.py / health_groups_ref.py with the prior state kept per
+    key (a new key starts at 0): the vectorised form of tests/health_keyed_ref.py for a list that only grows."""
+    lib = kvgpu.load()
+    cap = n + (ticks + WARMUP) // 100 + 1
+    mdev = kind == "mdev"
+    size = 32 if mdev else 16
+    buf, ptr = pinned(cap, size)
+    view = buf.numpy().view(kvgpu.MDEV_REC if mdev else kvgpu.PCI_REC)
+    if mdev:
+        univ = O.gen_mdev(0, 2 * cap)                   # uuid bytes 0..3 = BE32(index): ascending
+        parents = np.unique(univ["parent"])
+    else:
+        univ = O.gen_pci(0, 2 * cap, ids, 12)
+        univ["addr"] = np.arange(2 * cap, dtype=np.uint32)
+        univ["iommu_group"] = 1 + np.arange(2 * cap, dtype=np.uint32) // (2 * per_group)
+        all_nodes = np.arange(1, min(-(-n // per_group), GROUP_CAP) + 1, dtype=np.uint32)
+        nodes = [all_nodes]
+    m = [n]
+    view[:n] = univ[0:2 * n:2]
+    st = {"p": np.zeros(n, bool), "m": np.zeros(n, bool), "h": np.zeros(n, bool)}
+    rng = np.random.default_rng(n + 11)
+    edits = [0]
+    if mdev:                                            # n = 0: the reset
+        ctx.health_rescan_mdev_keyed(view[:0], N_TYPES)
+    else:
+        ctx.health_rescan_groups_keyed(view[:0])
+
+    def is_edit(tick):
+        return tick % 100 == 77
+
+    def mutate(tick):
+        k = m[0]
+        if is_edit(tick):                               # key 2e+1 goes behind key 2e, at position 2e+1
+            e = edits[0]
+            edits[0] += 1
+            at = 2 * e + 1
+            view[at + 1:k + 1] = view[at:k].copy()
+            view[at] = univ[2 * e + 1]
+            for a in st:
+                st[a] = np.insert(st[a], at, False)
+            m[0] = k = k + 1
+        idx = rng.integers(0, k, 10)
+        if mdev:
+            view["flags"][idx] ^= rng.integers(1, 4, 10).astype(np.uint8)
+            return [int(parents[rng.integers(0, len(parents))])] if tick % 100 == 99 else []
+        view["driver"][idx] = rng.integers(0, 5, 10)
+        if tick % 100 == 0:
+            nodes[0] = np.setdiff1d(all_nodes, [int(rng.integers(1, len(all_nodes) + 1))])
+        elif tick % 100 == 50:
+            nodes[0] = all_nodes
+        return nodes[0]
+
+    def call(xs):
+        x = np.asarray(xs, dtype=np.uint32)
+        res = C.POINTER(kvgpu._lib.HealthDeltaC)()
+        if mdev:
+            rc = lib.kvg_health_rescan_mdev_keyed(ctx.handle, ptr, m[0], N_TYPES, x.ctypes.data if len(x) else None,
+                                                  len(x), C.byref(res))
+        else:
+            rc = lib.kvg_health_rescan_groups_keyed(ctx.handle, ptr, m[0], x.ctypes.data if len(x) else None, len(x),
+                                                    C.byref(res))
+        assert rc == 0, ctx._lib.kvg_last_error(ctx.handle)
+        return res
+
+    def check(res, xs):
+        r = res.contents
+        got = np.ctypeslib.as_array(C.cast(r.changed, C.POINTER(C.c_uint32)), (r.n_changed,)) if r.n_changed else np.zeros(0, np.uint32)
+        if mdev:
+            want, alive, st["p"], st["m"] = health_mdev_ref.step(view[:m[0]], N_TYPES, xs, st["p"], st["m"])
+        else:
+            want, alive, st["h"] = health_groups_ref.step(view[:m[0]], xs, st["h"])
+        assert r.n_alive == alive and np.array_equal(got, want), "keyed parity at %d records" % m[0]
+
+    out = poll_loop(call, mutate, ticks, check, check_all=True, edit=is_edit)
+    out["path"] = "k_health_small<Keyed<%s>>" % ("MdevHealthRule" if mdev else "GroupHealthRule") if n + ticks // 100 < 32768 \
+        else "k_compact<HealthOp<Keyed<%s>>, 256, 8>" % ("MdevHealthRule" if mdev else "GroupHealthRule")
+    if not mdev:
+        out["groups"] = int(-(-n // per_group))
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--sizes", default="10000,32768,65536")
     ap.add_argument("--group-sizes", default="10000,32768,65536")
     ap.add_argument("--pci-sizes", default="10000,65536")
     ap.add_argument("--ticks", type=int, default=10_000)
+    ap.add_argument("--keyed", action="store_true", help="also the keyed legs: 10,000 and 65,536 vGPUs; 10,000 PCI "
+                    "functions in 2,500 groups and 65,536 in 4,096")
     ap.add_argument("--out", default="health_mdev_out", help="directory for health_mdev.json")
     a = ap.parse_args()
     card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
@@ -193,7 +294,7 @@ def main():
     ids = O.nv_ids(util.pciids_text())
     out = {"card": card, "poll_hz": 1000, "ticks": a.ticks, "warmup": WARMUP, "flips_per_tick": 10,
            "xid_every": 100, "what": "host wall time from snapshot-in-pinned-buffer to transitions on the host",
-           "mdev": {}, "groups": {}, "pci": {}}
+           "mdev": {}, "groups": {}, "pci": {}, "mdev_keyed": {}, "groups_keyed": {}}
     with kvgpu.Context(0) as ctx:
         for n in [int(s) for s in a.sizes.split(",") if s]:
             out["mdev"][n] = mdev_leg(ctx, n, a.ticks)
@@ -204,6 +305,13 @@ def main():
         for n in [int(s) for s in a.pci_sizes.split(",") if s]:
             out["pci"][n] = pci_leg(ctx, n, a.ticks, ids)
             print("pci", n, json.dumps(out["pci"][n]), flush=True)
+        if a.keyed:
+            for n in (10_000, 65_536):
+                out["mdev_keyed"][n] = keyed_leg(ctx, "mdev", n, a.ticks, ids)
+                print("mdev_keyed", n, json.dumps(out["mdev_keyed"][n]), flush=True)
+            for n, per in ((10_000, 4), (65_536, 16)):
+                out["groups_keyed"][n] = keyed_leg(ctx, "groups", n, a.ticks, ids, per)
+                print("groups_keyed", n, json.dumps(out["groups_keyed"][n]), flush=True)
     os.makedirs(a.out, exist_ok=True)
     with open(os.path.join(a.out, "health_mdev.json"), "w") as f:
         json.dump(out, f, indent=1)
