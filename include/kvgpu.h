@@ -359,6 +359,17 @@ int kvg_scan_pci(kvg_ctx *ctx, const kvg_pci_rec *recs, size_t n, kvg_pci_result
  *  chunk by chunk on separate copy streams; results are identical.  KVG_PIPELINE=0 disables.) */
 int kvg_scan_mdev(kvg_ctx *ctx, const kvg_mdev_rec *recs, size_t n, const kvg_type_dict *types,
                   kvg_mdev_result **res);
+/* Allocate-time re-check of the vGPU plugin (generic_vgpu_device_plugin.go:216-221): match[i] = 1 iff the label of
+ * file i -- Trim(raw, "\n") then every RE2 \s+ run ([\t\n\f\r ]) -> "_" (device_plugin.go:341-342) -- equals the
+ * name_len bytes at `name`, else 0.  `files` uses the layout of kvg_type_dict, one entry per file that WAS read; a
+ * failed read never reaches the rule (the reference's `err != nil ||` short-circuits), so the caller skips it.
+ * `match` is caller memory of files->n_types bytes.  One launch per call with n_types > 0, none for n_types = 0 or a
+ * refused call.  Files of any length, up to the uint32 offsets.  The call uses buffers of its own: no scan, fetch,
+ * delta or health state changes, so it may run between kvg_dev_scan_mdev and kvg_dev_scan_mdev_fetch.
+ * KVG_EINVAL: ctx, files or match NULL; off or bytes NULL with n_types > 0; name NULL with name_len > 0; off[0] != 0
+ * or decreasing offsets. */
+int kvg_mdev_label_match(kvg_ctx *ctx, const kvg_type_dict *files, const uint8_t *name, size_t name_len,
+                         uint8_t *match);
 /* Classify `recs`, diff against the alive-set of the previous call on this context (first call:
  * against "nothing alive").  A call with a different n re-arms the same way, as does
  * kvg_health_reset(); n = 0 returns an empty delta.  Pinned (cudaHostAlloc / registered) `recs` of

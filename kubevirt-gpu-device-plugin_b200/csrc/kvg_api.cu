@@ -42,5 +42,6 @@ using namespace kvg;
 #include "api/kvg_api_health.inc"
 #include "api/kvg_api_delta.inc"
 #include "api/kvg_api_mdev.inc"
+#include "api/kvg_api_alloc.inc"
 #include "api/kvg_api_util.inc"
 #include "api/kvg_api_shard.inc"

@@ -12,6 +12,7 @@
 //   k_health_small<Rule>   K6 at poll-loop sizes: one CTA, TMA-staged, transitions into mapped host memory
 //                          (Keyed<Rule>, either form: the prior state joined by UUID / address instead of by index)
 //   k_mdev_labels / _canon K5: label rule (:341-342) + merge of equal labels
+//   k_mdev_label_match     the same label rule against one name: the vGPU plugin's Allocate-time re-check
 //   k_gen_*                counter-based synthetic snapshots (twins of oracle/kvg_oracle.c kvo_gen_*)
 #pragma once
 #include "../../include/kvgpu.h"
@@ -581,18 +582,17 @@ __global__ void __launch_bounds__(HEALTH_SMALL_THREADS) k_health_small(Rule rule
 // mdev type dictionary: label = Trim(raw, "\n") then \s+ -> "_"  (device_plugin.go:341-342);
 // canonical id = smallest raw index with an identical label (they are ONE vGpuMap key).
 // ------------------------------------------------------------------------------------------------
-__global__ void k_mdev_labels(const uint8_t* __restrict__ raw, const uint32_t* __restrict__ raw_off,
-                              uint32_t n_types, uint8_t* __restrict__ label,
-                              uint32_t* __restrict__ label_len, uint64_t* __restrict__ label_hash) {
-  pdl_enter();
-  uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
-  if (k >= n_types) return;
-  uint32_t a = raw_off[k], b = raw_off[k + 1];
+// The label rule, the one definition the scan's dictionary and the Allocate-time check share, in the reference's two
+// steps: mdev_label_trim narrows raw[a, b) to Trim(raw, "\n"); mdev_label_emit feeds the label of that span -- every
+// RE2 \s+ run as one '_' -- to emit(c) byte by byte, and stops early (returns false) when emit returns false.
+// mdev_label_rule is the two in order.  k_mdev_labels calls them one by one and sets up its outputs in between: set up
+// before the trim, they make nvcc lay out its loops differently.
+__device__ __forceinline__ void mdev_label_trim(const uint8_t* __restrict__ raw, uint32_t& a, uint32_t& b) {
   while (a < b && raw[a] == '\n') a++;
   while (b > a && raw[b - 1] == '\n') b--;
-  uint8_t* out = label + raw_off[k];  // sanitised text is never longer than the raw text
-  uint32_t o = 0;
-  uint64_t h = 1469598103934665603ull;  // FNV-1a of the label: cheap first-level equality test
+}
+template <class Emit>
+__device__ __forceinline__ bool mdev_label_emit(const uint8_t* __restrict__ raw, uint32_t a, uint32_t b, Emit&& emit) {
   for (uint32_t i = a; i < b;) {
     uint8_t c;
     if (d_re2_space(raw[i])) {
@@ -601,11 +601,58 @@ __global__ void k_mdev_labels(const uint8_t* __restrict__ raw, const uint32_t* _
     } else {
       c = raw[i++];
     }
+    if (!emit(c)) return false;
+  }
+  return true;
+}
+template <class Emit>
+__device__ __forceinline__ bool mdev_label_rule(const uint8_t* __restrict__ raw, uint32_t a, uint32_t b, Emit&& emit) {
+  mdev_label_trim(raw, a, b);
+  return mdev_label_emit(raw, a, b, emit);
+}
+
+__global__ void k_mdev_labels(const uint8_t* __restrict__ raw, const uint32_t* __restrict__ raw_off,
+                              uint32_t n_types, uint8_t* __restrict__ label,
+                              uint32_t* __restrict__ label_len, uint64_t* __restrict__ label_hash) {
+  pdl_enter();
+  uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= n_types) return;
+  uint32_t a = raw_off[k], b = raw_off[k + 1];
+  mdev_label_trim(raw, a, b);
+  uint8_t* out = label + raw_off[k];  // sanitised text is never longer than the raw text
+  uint32_t o = 0;
+  uint64_t h = 1469598103934665603ull;  // FNV-1a of the label: cheap first-level equality test
+  mdev_label_emit(raw, a, b, [&](uint8_t c) {
     out[o++] = c;
     h = (h ^ c) * 1099511628211ull;
-  }
+    return true;
+  });
   label_len[k] = o;
   label_hash[k] = h;
+}
+
+// Allocate-time re-check (generic_vgpu_device_plugin.go:216-221): match[k] = 1 iff the label of file k is the name
+// (name_len bytes; `name` holds min(name_len, raw_off[n]) of them, all a label can reach).  One CTA, one thread per
+// file, striding; the bytes go straight to mapped host memory, then the sequence word the host polls.
+static constexpr int LABEL_MATCH_THREADS = 1024;
+__global__ void __launch_bounds__(LABEL_MATCH_THREADS) k_mdev_label_match(const uint8_t* __restrict__ raw,
+                                                                           const uint32_t* __restrict__ raw_off,
+                                                                           uint32_t n, const uint8_t* __restrict__ name,
+                                                                           uint64_t name_len, uint8_t* match_host,
+                                                                           uint32_t* seq_host, uint32_t seq) {
+  pdl_enter();
+  for (uint32_t k = threadIdx.x; k < n; k += blockDim.x) {
+    uint32_t o = 0;
+    const bool same = mdev_label_rule(raw, raw_off[k], raw_off[k + 1],
+                                      [&](uint8_t c) { return o < name_len && name[o++] == c; });
+    match_host[k] = same && o == name_len;
+  }
+  __threadfence_system();  // every thread's bytes are on their way before the sequence word
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    __threadfence_system();
+    *((volatile uint32_t*)seq_host) = seq;
+  }
 }
 // canonical id = smallest raw index with an identical label: hash + length first (independent,
 // pipelined loads), bytes only on a hash match

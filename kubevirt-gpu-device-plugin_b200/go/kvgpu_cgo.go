@@ -299,26 +299,8 @@ func createVgpuIDMapGPU() {
 		log.Printf("Error: %v", err)
 		return
 	}
-	// The dictionary struct holds two pointers: they must not be Go pointers (cgo rule: a Go pointer passed to
-	// C may not point at memory that itself holds Go pointers), so both arrays live in C memory for the call.
-	total := 0
-	for _, t := range rawTypes {
-		total += len(t)
-	}
-	cOff := (*C.uint32_t)(C.malloc(C.size_t(4 * (len(rawTypes) + 1))))
-	cBlob := (*C.uint8_t)(C.malloc(C.size_t(total + 1)))
-	defer C.free(unsafe.Pointer(cOff))
-	defer C.free(unsafe.Pointer(cBlob))
-	off := unsafe.Slice(cOff, len(rawTypes)+1)
-	blob := unsafe.Slice((*byte)(unsafe.Pointer(cBlob)), total+1)
-	off[0] = 0
-	pos := 0
-	for i, t := range rawTypes {
-		pos += copy(blob[pos:], t)
-		off[i+1] = C.uint32_t(pos)
-	}
-	blob[total] = 0
-	dict := C.kvg_type_dict{n_types: C.uint32_t(len(rawTypes)), off: cOff, bytes: cBlob}
+	dict, freeDict := cTypeDict(rawTypes)
+	defer freeDict()
 	var res *C.kvg_mdev_result
 	var p *C.kvg_mdev_rec
 	if len(recs) > 0 {
@@ -353,6 +335,31 @@ func createVgpuIDMapGPU() {
 		}
 	}
 	_ = sort.Strings // (kept: callers that want deterministic logs sort the keys)
+}
+
+// cTypeDict lays raw out as a kvg_type_dict.  The dictionary struct holds two pointers: they must not be Go pointers
+// (cgo rule: a Go pointer passed to C may not point at memory that itself holds Go pointers), so both arrays live in
+// C memory; free releases them after the call.
+func cTypeDict(raw [][]byte) (dict C.kvg_type_dict, free func()) {
+	total := 0
+	for _, t := range raw {
+		total += len(t)
+	}
+	cOff := (*C.uint32_t)(C.malloc(C.size_t(4 * (len(raw) + 1))))
+	cBlob := (*C.uint8_t)(C.malloc(C.size_t(total + 1)))
+	off := unsafe.Slice(cOff, len(raw)+1)
+	blob := unsafe.Slice((*byte)(unsafe.Pointer(cBlob)), total+1)
+	off[0] = 0
+	pos := 0
+	for i, t := range raw {
+		pos += copy(blob[pos:], t)
+		off[i+1] = C.uint32_t(pos)
+	}
+	blob[total] = 0
+	return C.kvg_type_dict{n_types: C.uint32_t(len(raw)), off: cOff, bytes: cBlob}, func() {
+		C.free(unsafe.Pointer(cOff))
+		C.free(unsafe.Pointer(cBlob))
+	}
 }
 
 // revalidateBatchGPU is the Allocate-time re-check of generic_device_plugin.go:387-399 for ALL devices
@@ -420,4 +427,52 @@ func revalidateBatchGPU(devs []string, want []string) (first int, err error) {
 		}
 	}
 	return -1, nil
+}
+
+// revalidateVgpuBatchGPU is the Allocate-time re-check of generic_vgpu_device_plugin.go:216-228 for ALL IDs of an
+// AllocateRequest in one launch (Python twin: kvgpu/serve.py MdevLabelCheck, pinned by
+// tests/test_serve_vgpu_allocate.py).  Each ID's mdev_type/name is read raw, as readVgpuIDFromFile reads it, and no
+// regexp runs here: the GPU applies Trim(raw, "\n") and \s+ -> "_" (device_plugin.go:341-342) and compares the label
+// with deviceName.  keep[i] is false for an ID whose read failed; such a file never reaches the rule.
+//
+// Call site (generic_vgpu_device_plugin.go:208-245): collect the DevicesIDs of every ContainerRequest in order, call
+// this once, then walk the requests again and append each devID whose keep entry is true to that container's env
+// list, replacing the per-ID readVgpuIDFromFile call and its regexp.MustCompile.
+func revalidateVgpuBatchGPU(ids []string, deviceName string) ([]bool, error) {
+	keep := make([]bool, len(ids))
+	var raw [][]byte
+	var at []int
+	for i, id := range ids {
+		data, err := os.ReadFile(filepath.Join(vGpuBasePath, id, "mdev_type/name"))
+		if err != nil {
+			continue
+		}
+		raw = append(raw, data)
+		at = append(at, i)
+	}
+	if len(raw) == 0 {
+		return keep, nil
+	}
+	kvgMu.Lock()
+	defer kvgMu.Unlock()
+	if err := kvgEnsure(); err != nil {
+		return nil, err
+	}
+	dict, freeDict := cTypeDict(raw)
+	defer freeDict()
+	match := (*C.uint8_t)(C.malloc(C.size_t(len(raw))))
+	defer C.free(unsafe.Pointer(match))
+	var name *C.uint8_t
+	if len(deviceName) > 0 {
+		cname := C.CString(deviceName)
+		defer C.free(unsafe.Pointer(cname))
+		name = (*C.uint8_t)(unsafe.Pointer(cname))
+	}
+	if rc := C.kvg_mdev_label_match(kvgCtx, &dict, name, C.size_t(len(deviceName)), match); rc != C.KVG_OK {
+		return nil, fmt.Errorf("kvg_mdev_label_match: %s", C.GoString(C.kvg_last_error(kvgCtx)))
+	}
+	for k, m := range unsafe.Slice(match, len(raw)) {
+		keep[at[k]] = m != 0
+	}
+	return keep, nil
 }

@@ -50,8 +50,10 @@ def main(argv=None) -> int:
         from . import dpapi, serve
         sockdir = args.socket_dir or dpapi.DEVICE_PLUGIN_PATH
         reval = serve.BatchRevalidator(ds.ctx.scan_pci, args.base_path)
-        plugins = serve.plugins_from_specs(specs, ds.maps, reval, socket_dir=sockdir, base_path=args.base_path,
-                                           root_path=args.root_path, vgpu_base_path=args.vgpu_base_path)
+        vgpu_check = serve.MdevLabelCheck(ds.ctx.mdev_label_match, args.vgpu_base_path)
+        plugins = serve.plugins_from_specs(specs, ds.maps, reval, vgpu_check=vgpu_check, socket_dir=sockdir,
+                                           base_path=args.base_path, root_path=args.root_path,
+                                           vgpu_base_path=args.vgpu_base_path)
         watchers, started = [], []
         for p in plugins:                 # createDevicePlugins :131-137, :158-165: a failed start is logged, the rest go on
             try:

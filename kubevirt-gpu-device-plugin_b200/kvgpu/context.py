@@ -255,6 +255,18 @@ class Context:
         del keep
         return self._take_mdev(res)
 
+    def mdev_label_match(self, raw_files: list, name) -> np.ndarray:
+        r"""The vGPU plugin's Allocate-time re-check (include/kvgpu.h kvg_mdev_label_match), one launch: element i is
+        True iff the label of raw_files[i] (Trim "\n", then every \s+ run -> "_") equals `name`.  A str name is
+        encoded as latin-1, the decoding the plugin's labels use."""
+        if isinstance(name, str):
+            name = name.encode("latin-1")
+        td, keep = self._type_dict(raw_files)
+        match = np.zeros(max(len(raw_files), 1), dtype=np.uint8)
+        self._ck(self._lib.kvg_mdev_label_match(self._h, C.byref(td), name, len(name), match.ctypes.data))
+        del keep
+        return match[:len(raw_files)].astype(bool)
+
     def _take_health(self, res) -> HealthDelta:
         r = res.contents
         out = HealthDelta(int(r.n_records), int(r.n_alive),

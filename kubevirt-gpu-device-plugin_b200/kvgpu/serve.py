@@ -14,8 +14,10 @@ reference's generic_device_plugin_test.go.  In a deployment these servers stay i
 Allocate" is testable end to end in an image without a Go toolchain.
 
 Nothing here computes on the CPU what the scan computes on the GPU: the maps come from
-plugin.DiscoveryScan (libkvgpu.so); the re-validation's classification goes through
-Context.scan_pci (K3); the health feeds through Context.health_rescan, Context.health_rescan_mdev and
+plugin.DiscoveryScan (libkvgpu.so); the passthrough re-validation's classification goes through
+Context.scan_pci (K3), the vGPU plugin's label check through Context.mdev_label_match (MdevLabelCheck;
+a vGPU plugin built without a check keeps the reference's CPU rule, the path the GPU check is tested
+against); the health feeds through Context.health_rescan, Context.health_rescan_mdev and
 Context.health_rescan_groups and their keyed forms (K6); the
 hot-plug feeds through Context.scan_pci_delta and Context.scan_mdev_delta (K7).
 """
@@ -467,33 +469,68 @@ class GenericDevicePlugin(_PluginBase):
 
 
 class GenericVGpuDevicePlugin(_PluginBase):
-    """The vGPU plugin (generic_vgpu_device_plugin.go)."""
+    """The vGPU plugin (generic_vgpu_device_plugin.go).  `check` is the Allocate-time re-check of the type labels
+    (MdevLabelCheck: one GPU call per AllocateRequest); without it each ID is read and its label built on the CPU."""
     vgpu = True
 
     def __init__(self, device_name, device_path, devs, *, vgpu_base_path="/sys/bus/mdev/devices",
-                 read_vgpu_id=None, **kw):
+                 read_vgpu_id=None, check=None, **kw):
         super().__init__(device_name, devs, **kw)
         self.device_path, self.vgpu_base_path = device_path, vgpu_base_path
         self.read_vgpu_id = read_vgpu_id or _read_vgpu_label
+        self.check = check
 
     def GetPreferredAllocation(self, request, context):
         # "has not been implemented" in the reference: returns (nil, nil) (:262-271) -> empty message
         return dpapi.PreferredAllocationResponse()
 
     def Allocate(self, request, context):
-        """:208-245 — ids whose type label no longer equals the plugin's name are skipped, not errors."""
+        """:208-245 — ids whose type label no longer equals the plugin's name are skipped, not errors.  With a check,
+        the IDs of all container requests go to it in one call, in request order."""
+        reqs = list(request.container_requests)
+        if self.check is not None:
+            ok = iter(self.check(self.device_name, [dev_id for req in reqs for dev_id in req.devices_ids]))
+
+            def keep(dev_id):
+                return bool(next(ok))
+        else:
+            def keep(dev_id):
+                label, err = self.read_vgpu_id(self.vgpu_base_path, dev_id, "mdev_type/name")
+                return not err and label == self.device_name
         responses = dpapi.AllocateResponse()
-        for req in request.container_requests:
+        for req in reqs:
             env_list = {}
             for dev_id in req.devices_ids:
-                label, err = self.read_vgpu_id(self.vgpu_base_path, dev_id, "mdev_type/name")
-                if err or label != self.device_name:
+                if not keep(dev_id):
                     continue
                 env_list.setdefault("%s_%s" % (VGPU_PREFIX, self.device_name.upper()), []).append(dev_id)
             spec = dpapi.DeviceSpec(host_path=VFIO_DEVICE_PATH, container_path=VFIO_DEVICE_PATH, permissions="mrw")
             responses.container_responses.append(dpapi.ContainerAllocateResponse(
                 envs={k: ",".join(v) for k, v in env_list.items()}, devices=[spec]))
         return responses
+
+
+class MdevLabelCheck:
+    """The vGPU plugin's Allocate-time re-check (generic_vgpu_device_plugin.go:216-228) with the label rule on the
+    GPU.  Every ID's mdev_type/name is read with the reference's raw reader, in request order; the files that were
+    read go to ONE `label_match` call (Context.mdev_label_match), which builds each label and compares it with the
+    plugin's name.  An ID whose read failed never reaches the rule and is not kept."""
+
+    def __init__(self, label_match, vgpu_base_path: str = "/sys/bus/mdev/devices", read_raw=_read_vgpu_raw):
+        self.label_match, self.vgpu_base_path, self.read_raw = label_match, vgpu_base_path, read_raw
+
+    def __call__(self, device_name, ids) -> list:
+        """One bool per ID: its label equals device_name."""
+        out, files, at = [False] * len(ids), [], []
+        for i, dev_id in enumerate(ids):
+            raw, err = self.read_raw(self.vgpu_base_path, dev_id, "mdev_type/name")
+            if not err:
+                files.append(raw)
+                at.append(i)
+        if files:
+            for i, m in zip(at, self.label_match(files, device_name)):
+                out[i] = bool(m)
+        return out
 
 
 def _read_vgpu_label(base, addr, prop):
@@ -505,13 +542,14 @@ def _read_vgpu_label(base, addr, prop):
     return re.sub(rb"[\t\n\f\r ]+", b"_", raw.strip(b"\n")).decode("latin-1"), False
 
 
-def plugins_from_specs(specs, maps: Maps, revalidate, **kw) -> list:
-    """createDevicePlugins' server half (device_plugin.go:99-157): one plugin object per spec."""
+def plugins_from_specs(specs, maps: Maps, revalidate, vgpu_check=None, **kw) -> list:
+    """createDevicePlugins' server half (device_plugin.go:99-157): one plugin object per spec.  `revalidate` is the
+    passthrough plugins' Allocate-time re-check, `vgpu_check` the vGPU plugins' (None: the CPU rule)."""
     out = []
     for spec in specs:
         devs = devices_from_spec(spec)
         if spec.vgpu:
-            out.append(GenericVGpuDevicePlugin(spec.device_name, "vgpu", devs,
+            out.append(GenericVGpuDevicePlugin(spec.device_name, "vgpu", devs, check=vgpu_check,
                                                **{k: v for k, v in kw.items() if k in ("socket_dir", "kubelet_socket",
                                                                                           "vgpu_base_path")}))
         else:

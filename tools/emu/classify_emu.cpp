@@ -215,4 +215,13 @@ int emu_scan_mdev(const uint4* recs, uint32_t n, const uint8_t* raw, const uint3
   return 0;
 }
 
+// kvg_mdev_label_match's kernel in its launch shape (one CTA of LABEL_MATCH_THREADS): raw / raw_off: n files with n+1
+// offsets; name: min(name_len, raw_off[n]) bytes.  match_out: n bytes; seq_out: the sequence word (7 when done).
+int emu_mdev_label_match(const uint8_t* raw, const uint32_t* raw_off, uint32_t n, const uint8_t* name, uint64_t name_len,
+                         uint8_t* match_out, uint32_t* seq_out) {
+  if (n == 0) return -1;
+  emu_launch(k_mdev_label_match, dim3(1), LABEL_MATCH_THREADS, raw, raw_off, n, name, name_len, match_out, seq_out, 7u);
+  return 0;
+}
+
 }  // extern "C"

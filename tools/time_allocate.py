@@ -1,0 +1,122 @@
+"""Latency of the vGPU plugin's Allocate-time label check on the GPU (kvg_mdev_label_match), beside the passthrough
+plugin's re-validation batch (kvg_scan_pci, the figure bench.py reports as allocate_revalidation) and the CPU rule of
+serve._read_vgpu_label, in one process.
+
+  (a) kvg_mdev_label_match at 1, 2, 4, 8 and 16 files, and at 4 containers x 4 files (one call per AllocateRequest:
+      the 16 files of the four containers in request order);
+  (b) kvg_scan_pci on a pinned batch of 16 records, as bench.py builds it;
+  (c) on the CPU, the rule inside _read_vgpu_label (strip, re.sub, decode, compare) on the same bytes in memory.
+
+Each size: 50 warm-up calls, then the p50 and p99 of the host wall time of 1,000 calls; every result is checked
+against the CPU rule.  The file contents are those of a live mdev_type/name ("GRID A100-4C\\n"), with one in four of
+another type.  The card's name, power limit and maximum SM clock are read with a read-only nvidia-smi query in the
+same run.
+
+    python tools/time_allocate.py [--calls 1000] [--out DIR]
+"""
+import argparse
+import ctypes as C
+import gzip
+import json
+import os
+import re
+import subprocess
+import sys
+import time
+
+import numpy as np
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, os.path.join(ROOT, "kubevirt-gpu-device-plugin_b200"))
+import kvgpu  # noqa: E402
+
+WARMUP = 50
+NAME = b"GRID_A100-4C"
+
+
+def stats(lat):
+    lat = np.array(lat) * 1e6
+    return {"p50_us": round(float(np.percentile(lat, 50)), 2), "p99_us": round(float(np.percentile(lat, 99)), 2)}
+
+
+def timed(fn, calls):
+    lat = []
+    for it in range(WARMUP + calls):
+        t0 = time.perf_counter()
+        fn()
+        dt = time.perf_counter() - t0
+        if it >= WARMUP:
+            lat.append(dt)
+    return stats(lat)
+
+
+def cpu_rule(raw):
+    return re.sub(rb"[\t\n\f\r ]+", b"_", raw.strip(b"\n")).decode("latin-1")
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--calls", type=int, default=1000)
+    ap.add_argument("--out", default=None)
+    a = ap.parse_args()
+    card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                          capture_output=True, text=True, check=True).stdout.strip().splitlines()[0]
+    print(card, flush=True)
+    lib = kvgpu.load()
+    out = {"card": card, "calls": a.calls, "warmup": WARMUP, "what": "host wall time of one call", "label_match": {},
+           "scan_pci_16": None, "cpu_rule": {}}
+    legs = [("%d" % k, k) for k in (1, 2, 4, 8, 16)] + [("4x4", 16)]
+    with kvgpu.Context(0) as ctx:
+        with gzip.open(os.path.join(ROOT, "tests", "golden", "pci.ids.gz"), "rb") as f:
+            ctx.pciids_load(f.read())                                  # a scan joins names: it needs the table
+        for label, k in legs:
+            files = [b"GRID A100-4C\n" if i % 4 != 3 else b"GRID A100-8C\n" for i in range(k)]
+            want = np.array([cpu_rule(f) == NAME.decode() for f in files], dtype=np.uint8)
+            td, keep = ctx._type_dict(files)
+            match = np.zeros(k, dtype=np.uint8)
+
+            def gpu():
+                assert lib.kvg_mdev_label_match(ctx.handle, C.byref(td), NAME, len(NAME), match.ctypes.data) == 0
+            before = ctx.launch_count
+            out["label_match"][label] = timed(gpu, a.calls)
+            assert ctx.launch_count - before == WARMUP + a.calls      # one launch per call
+            assert np.array_equal(match, want)
+            assert np.array_equal(ctx.mdev_label_match(files, NAME), want.astype(bool))
+
+            def cpu():
+                return [cpu_rule(f) == "GRID_A100-4C" for f in files]
+            out["cpu_rule"][label] = timed(cpu, a.calls)
+            assert np.array_equal(np.array(cpu(), dtype=np.uint8), want)
+            del keep
+
+        import torch
+        rr = np.zeros(16, dtype=kvgpu.PCI_REC)
+        for i in range(16):
+            rr[i] = (i, 0x10de, 0, i // 2, 1, 0, 0)                    # what BatchRevalidator builds (bench.py)
+        hr = torch.from_numpy(np.frombuffer(rr.tobytes(), dtype=np.uint8).copy()).pin_memory()
+
+        def scan():
+            res = C.POINTER(kvgpu._lib.PciResultC)()
+            assert lib.kvg_scan_pci(ctx.handle, hr.data_ptr(), 16, C.byref(res)) == 0
+            assert res.contents.n_survivors == 16
+            lib.kvg_result_free(res)
+        out["scan_pci_16"] = timed(scan, a.calls)
+
+    print("%-28s %10s %10s" % ("call", "p50 us", "p99 us"))
+    for label, _ in legs:
+        s = out["label_match"][label]
+        print("%-28s %10.1f %10.1f" % ("kvg_mdev_label_match " + label, s["p50_us"], s["p99_us"]))
+    s = out["scan_pci_16"]
+    print("%-28s %10.1f %10.1f" % ("kvg_scan_pci 16 records", s["p50_us"], s["p99_us"]))
+    for label, _ in legs:
+        s = out["cpu_rule"][label]
+        print("%-28s %10.1f %10.1f" % ("CPU rule " + label, s["p50_us"], s["p99_us"]))
+    if a.out:
+        os.makedirs(a.out, exist_ok=True)
+        with open(os.path.join(a.out, "time_allocate.json"), "w") as f:
+            json.dump(out, f, indent=1)
+    print(json.dumps(out))
+
+
+if __name__ == "__main__":
+    main()
