@@ -330,6 +330,31 @@ __global__ void __launch_bounds__(DELTA_THREADS) k_delta_merge(DeltaMergeOp<Tr> 
   lookback_tile<DeltaMergeOp<Tr>, DELTA_THREADS, DELTA_ROWS>(o, tile, n_tiles, tile_state, o.tag, s_wtot, s_woff, s_base);
 }
 
+// The launch arguments below are built on the host, by kvg_api_delta.inc and by the CPU emulator alike.
+
+// k_delta_merge's operator over prev[0, n_prev) and now[0, n_now) (Tr::Rec in 16-byte units): entries to out, counts
+// to ctrl.  keys / n_keys: the distinct keys of the first map now and before, then those of the second map; flag:
+// their tag words in the same order; xlate: the first map's cross-map (mdev type ids) or NULL; tag: never repeated.
+template <class Tr>
+inline DeltaMergeOp<Tr> delta_merge_op(const uint4* prev, uint32_t n_prev, const uint4* now, uint32_t n_now, uint4* out,
+                                       ScanCtrl* ctrl, const uint32_t* const* keys, const uint32_t* n_keys,
+                                       uint32_t* const* flag, const uint32_t* xlate, uint32_t tag) {
+  DeltaMergeOp<Tr> op = {};
+  op.prev = reinterpret_cast<const typename Tr::Rec*>(prev);
+  op.n_prev = n_prev;
+  op.now = reinterpret_cast<const typename Tr::Rec*>(now);
+  op.n_now = n_now;
+  op.n = n_prev + n_now;
+  op.out = out;
+  op.ctrl = ctrl;
+  op.k0 = {keys[0], n_keys[0], flag[0], keys[1], n_keys[1], flag[1], xlate};
+  op.k1 = {keys[2], n_keys[2], flag[2], keys[3], n_keys[3], flag[3], nullptr};
+  op.tag = tag;
+  return op;
+}
+// k_delta_merge's grid over n merged positions: at least one CTA, which writes the zero count
+inline uint32_t delta_merge_tiles(uint32_t n) { return n ? (n + DELTA_TILE - 1) / DELTA_TILE : 1; }
+
 // The sharded forms (kvg_dev_scan_pci_shard_fetch_delta, kvg_dev_scan_mdev_shard_fetch_delta): one merge per
 // blockIdx.y over one pair of this rank's lists, all three checked for strict ascent.
 //   y = 0  the local survivors: change entries through the look-back tile body; its DeltaKeys hold no keys, so it
@@ -368,6 +393,33 @@ __global__ void __launch_bounds__(DELTA_THREADS) k_delta_merge_shard(DeltaShardA
     const typename DeltaMergeOp<Tr>::Item it = o.load(o.d0 + k, true);
     if (it.what) o.template apply<false>(0, it, o.d0 + k);
   }
+}
+// The three rows from op, the merge of the local survivors: row 0 is op without keys, its k0 keeping only the
+// cross-map; rows 1 and 2 merge prev[y - 1] and now[y - 1], the previous and the new members of the owned keys of the
+// first / second map, keep that map's keys and write no entries.  Returns the grid's columns: the longest row's tiles.
+template <class Tr>
+inline uint32_t delta_shard_args(DeltaShardArgs<Tr>& a, const DeltaMergeOp<Tr>& op, const uint4* const (&prev)[2],
+                                 const uint32_t (&n_prev)[2], const uint4* const (&now)[2],
+                                 const uint32_t (&n_now)[2]) {
+  const DeltaKeys none = {}, xlate_only = {nullptr, 0, nullptr, nullptr, 0, nullptr, op.k0.xlate};
+  uint32_t cols = 1;
+  for (int y = 0; y < 3; y++) {
+    DeltaMergeOp<Tr>& o = a.o[y];
+    o = op;
+    if (y > 0) {
+      o.prev = reinterpret_cast<const typename Tr::Rec*>(prev[y - 1]);
+      o.n_prev = n_prev[y - 1];
+      o.now = reinterpret_cast<const typename Tr::Rec*>(now[y - 1]);
+      o.n_now = n_now[y - 1];
+      o.n = o.n_prev + o.n_now;
+      o.out = nullptr;
+    }
+    if (y != 1) o.k0 = xlate_only;
+    if (y != 2) o.k1 = none;
+    const uint32_t t = delta_merge_tiles(o.n);
+    if (t > cols) cols = t;
+  }
+  return cols;
 }
 
 // One of the four key lists: keys whose tag word holds this call's tag, ascending.  Dirty lists give the key's
@@ -416,6 +468,25 @@ __global__ void __launch_bounds__(KVG_BLOCK) k_delta_lists(DeltaListArgs args, u
   lookback_tile<DeltaListOp, KVG_BLOCK, C_ROWS>(op, tile, n_tiles, tile_state + (size_t)blockIdx.y * state_stride, epoch,
                                                 s_wtot, s_woff, s_base);
 }
+// The four lists of op's two maps, counted into ctrl->reserved2[DELTA_W_LISTS ..]; out: where they go, the first gone
+// list as u16 when gone0_u16 (PCI device ids).  Returns the grid's columns: the longest list's tiles.
+template <class Tr>
+inline uint32_t delta_list_args(DeltaListArgs& la, const DeltaMergeOp<Tr>& op, void* const (&out)[4], bool gone0_u16) {
+  uint32_t* cnt = &op.ctrl->reserved2[DELTA_W_LISTS];
+  uint32_t cols = 1;
+  for (int m = 0; m < 2; m++) {
+    const DeltaKeys& k = m ? op.k1 : op.k0;
+    const bool u16 = m == 0 && gone0_u16;
+    la.o[2 * m] = {k.flag_now, k.n_now, op.tag, nullptr, (uint32_t*)out[2 * m], nullptr, cnt + 2 * m};
+    la.o[2 * m + 1] = {k.flag_prev, k.n_prev, op.tag, k.keys_prev, u16 ? nullptr : (uint32_t*)out[2 * m + 1],
+                       u16 ? (uint16_t*)out[2 * m + 1] : nullptr, cnt + 2 * m + 1};
+    for (const uint32_t n : {k.n_now, k.n_prev}) {
+      const uint32_t t = (n + C_TILE - 1) / C_TILE;
+      if (t > cols) cols = t;
+    }
+  }
+  return cols;
+}
 
 // The previous result's type keys in the new key space.  The canonical ids of two scans are not comparable (each
 // numbers its own dictionary), labels are: xlate[c] for every previous type key c is the new type key with a
@@ -428,6 +499,12 @@ __global__ void __launch_bounds__(KVG_BLOCK) k_delta_lists(DeltaListArgs args, u
 // O(KT_prev + KT_now) expected probes.
 constexpr uint32_t XMAP_THREADS = 1024;
 constexpr uint32_t XMAP_SLOTS = 1u << 17;  // >= 2 x 65,535 type keys
+// the table's probe mask for n_keys new keys: at least 64 slots and twice the keys, a power of two
+inline uint32_t delta_xmap_mask(uint32_t n_keys) {
+  uint32_t slots = 64;
+  while (slots < 2 * n_keys) slots <<= 1;
+  return slots - 1;
+}
 struct MdevTypeLabels {  // one dictionary: labels indexed by canonical id, and the ids that are keys
   const uint32_t* keys;  // the canonical ids to translate (from) / to look up (into), ascending
   uint32_t n_keys;

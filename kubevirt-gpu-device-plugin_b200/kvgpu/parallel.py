@@ -126,12 +126,12 @@ def shard_delta_part(res: PciShardResult, delta) -> PciShardDelta:
                          res.grp.grp_keys[delta.grp_dirty].astype(np.uint32), delta.grp_gone)
 
 
-def merge_pci_shard_deltas(parts: list) -> PciShardDelta:
-    """The delta of the whole snapshot from the ranks' shard_delta_part summaries (rank order): equal to
-    kvg_scan_pci_delta on the concatenated snapshot (changes byte for byte, dirty keys as values).  Changes are
-    sorted by address; an address that crossed a shard boundary is REMOVED on one rank and ADDED on another, and
-    the pair fuses into one entry whose bits compare the two survivors (none: no entry).  Local indices become
-    global through prefix sums of the per-rank counts; the key lists are unions (ranks own disjoint keys)."""
+def _merge_shard_changes(parts: list, dtype, key_name: str, key, bits) -> tuple:
+    """The ranks' changes (rank order) as those of the whole snapshot -> (changes, n_prev, n_now).  Local indices
+    become global through prefix sums of the per-rank counts, and the changes are sorted by key(changes), an (n, w)
+    array of unsigned words, most significant first.  A key seen twice must be REMOVED on one rank and ADDED on
+    another (it crossed a shard boundary): the pair fuses into one entry with the previous side of the REMOVED one and
+    the new side of the ADDED one, whose bits(fused) compare the two survivors (none: no entry)."""
     none = np.uint32(0xFFFFFFFF)
     prev_off = np.cumsum([0] + [p.n_prev for p in parts])
     now_off = np.cumsum([0] + [p.n_now for p in parts])
@@ -141,26 +141,39 @@ def merge_pci_shard_deltas(parts: list) -> PciShardDelta:
         c["prev_index"] = np.where(c["prev_index"] == none, none, c["prev_index"] + np.uint32(prev_off[r]))
         c["now_index"] = np.where(c["now_index"] == none, none, c["now_index"] + np.uint32(now_off[r]))
         chs.append(c)
-    ch = np.concatenate(chs) if chs else np.zeros(0, L.PCI_CHANGE)
-    ch = ch[np.argsort(ch["addr"], kind="stable")]
-    dup = np.nonzero(ch["addr"][1:] == ch["addr"][:-1])[0]      # pairs: i (one side), i + 1 (the other)
+    ch = np.concatenate(chs) if chs else np.zeros(0, dtype)
+    k = key(ch)
+    order = np.lexsort(k.T[::-1])
+    ch, k = ch[order], k[order]
+    dup = np.nonzero((k[1:] == k[:-1]).all(axis=1))[0]          # pairs: i (one side), i + 1 (the other)
     if len(dup):
         rem = (ch["what"][dup] & L.CH_REMOVED) != 0             # which of the two is the REMOVED entry
         gone_, new_ = ch[np.where(rem, dup, dup + 1)], ch[np.where(rem, dup + 1, dup)]
         if not ((gone_["what"] == L.CH_REMOVED) & (new_["what"] == L.CH_ADDED)).all():
-            raise ValueError("one address twice, not as REMOVED + ADDED: the shards overlap")
+            raise ValueError("one %s twice, not as REMOVED + ADDED: the shards overlap" % key_name)
         f = new_.copy()
-        for side in ("prev_group", "prev_device", "prev_numa", "prev_index"):
+        for side in (name for name in dtype.names if name.startswith("prev_")):
             f[side] = gone_[side]
-        f["what"] = ((f["prev_group"] != f["now_group"]) * L.CH_GROUP | (f["prev_device"] != f["now_device"]) * L.CH_DEVICE
-                     | (f["prev_numa"] != f["now_numa"]) * L.CH_NUMA).astype(np.uint32)
+        f["what"] = bits(f).astype(np.uint32)
         keep = np.ones(len(ch), dtype=bool)
         keep[dup + 1] = False
         ch[dup] = f
         keep[dup[f["what"] == 0]] = False
         ch = ch[keep]
+    return np.ascontiguousarray(ch), int(prev_off[-1]), int(now_off[-1])
+
+
+def merge_pci_shard_deltas(parts: list) -> PciShardDelta:
+    """The delta of the whole snapshot from the ranks' shard_delta_part summaries (rank order): equal to
+    kvg_scan_pci_delta on the concatenated snapshot (changes byte for byte, dirty keys as values).  Changes are
+    sorted by address; an address that crossed a shard boundary is REMOVED on one rank and ADDED on another, and
+    the pair fuses into one entry whose bits compare the two survivors (none: no entry).  Local indices become
+    global through prefix sums of the per-rank counts; the key lists are unions (ranks own disjoint keys)."""
+    bits = lambda f: ((f["prev_group"] != f["now_group"]) * L.CH_GROUP
+                      | (f["prev_device"] != f["now_device"]) * L.CH_DEVICE | (f["prev_numa"] != f["now_numa"]) * L.CH_NUMA)
+    ch, n_prev, n_now = _merge_shard_changes(parts, L.PCI_CHANGE, "address", lambda ch: ch["addr"][:, None], bits)
     cat = lambda name, dt: np.unique(np.concatenate([getattr(p, name) for p in parts] + [np.zeros(0, dt)])).astype(dt)
-    return PciShardDelta(int(prev_off[-1]), int(now_off[-1]), np.ascontiguousarray(ch), cat("dev_dirty", np.uint16),
+    return PciShardDelta(n_prev, n_now, ch, cat("dev_dirty", np.uint16),
                          cat("dev_gone", np.uint16), cat("grp_dirty", np.uint32), cat("grp_gone", np.uint32))
 
 
@@ -227,44 +240,20 @@ def merge_mdev_shard_deltas(parts: list, prev_labels: list, now_labels: list) ->
     are not the union of the ranks' lists: a label that moved between ranks with unchanged members is gone on one rank
     and dirty on the other, yet neither in the whole snapshot's delta.  Parent handles never change owner, so the
     gpuVgpuMap lists are unions."""
-    none = np.uint32(0xFFFFFFFF)
-    prev_off = np.cumsum([0] + [p.n_prev for p in parts])
-    now_off = np.cumsum([0] + [p.n_now for p in parts])
-    chs = []
-    for r, p in enumerate(parts):
-        c = p.changes.copy()
-        c["prev_index"] = np.where(c["prev_index"] == none, none, c["prev_index"] + np.uint32(prev_off[r]))
-        c["now_index"] = np.where(c["now_index"] == none, none, c["now_index"] + np.uint32(now_off[r]))
-        chs.append(c)
-    ch = np.concatenate(chs) if chs else np.zeros(0, L.MDEV_CHANGE)
-    words = np.ascontiguousarray(ch["uuid"]).reshape(-1, 16).view(">u8").astype(np.uint64)
-    ch = ch[np.lexsort((words[:, 1], words[:, 0]))]
-    u = np.ascontiguousarray(ch["uuid"]).reshape(-1, 16)
-    dup = np.nonzero((u[1:] == u[:-1]).all(axis=1))[0]          # pairs: i (one side), i + 1 (the other)
     prev_lab = [bytes(b) for b in prev_labels]
     now_lab = [bytes(b) for b in now_labels]
-    if len(dup):
-        rem = (ch["what"][dup] & L.CH_REMOVED) != 0
-        gone_, new_ = ch[np.where(rem, dup, dup + 1)], ch[np.where(rem, dup + 1, dup)]
-        if not ((gone_["what"] == L.CH_REMOVED) & (new_["what"] == L.CH_ADDED)).all():
-            raise ValueError("one UUID twice, not as REMOVED + ADDED: the shards overlap")
-        f = new_.copy()
-        for side in ("prev_parent", "prev_type", "prev_numa", "prev_index"):
-            f[side] = gone_[side]
-        relabel = np.array([prev_lab[int(a)] != now_lab[int(b)] for a, b in zip(f["prev_type"], f["now_type"])], bool)
-        f["what"] = (relabel * L.CH_TYPE | (f["prev_parent"] != f["now_parent"]) * L.CH_PARENT
-                     | (f["prev_numa"] != f["now_numa"]) * L.CH_NUMA).astype(np.uint32)
-        keep = np.ones(len(ch), dtype=bool)
-        keep[dup + 1] = False
-        ch[dup] = f
-        keep[dup[f["what"] == 0]] = False
-        ch = ch[keep]
+    key = lambda ch: np.ascontiguousarray(ch["uuid"]).reshape(-1, 16).view(">u8").astype(np.uint64)
+    relabel = lambda f: np.array([prev_lab[int(a)] != now_lab[int(b)] for a, b in zip(f["prev_type"], f["now_type"])],
+                                 bool)
+    bits = lambda f: (relabel(f) * L.CH_TYPE | (f["prev_parent"] != f["now_parent"]) * L.CH_PARENT
+                      | (f["prev_numa"] != f["now_numa"]) * L.CH_NUMA)
+    ch, n_prev, n_now = _merge_shard_changes(parts, L.MDEV_CHANGE, "UUID", key, bits)
     type_keys = np.unique(np.concatenate([p.type_keys for p in parts] + [np.zeros(0, np.uint16)])).astype(np.uint16)
     now_id = _canonical_ids(now_lab)
     live = set(type_keys.tolist())
     dirty, gone = set(), set()
     for c in ch[(ch["what"] & (L.CH_ADDED | L.CH_REMOVED | L.CH_TYPE | L.CH_NUMA)) != 0]:
-        has_now, has_prev = c["now_index"] != none, c["prev_index"] != none
+        has_now, has_prev = c["now_index"] != L.NO_INDEX, c["prev_index"] != L.NO_INDEX
         if has_now:
             dirty.add(int(c["now_type"]))
         if has_prev:
@@ -277,7 +266,7 @@ def merge_mdev_shard_deltas(parts: list, prev_labels: list, now_labels: list) ->
             else:
                 gone.add(int(c["prev_type"]))
     cat = lambda name: np.unique(np.concatenate([getattr(p, name) for p in parts] + [np.zeros(0, np.uint32)]))
-    return MdevShardDelta(int(prev_off[-1]), int(now_off[-1]), np.ascontiguousarray(ch), type_keys,
+    return MdevShardDelta(n_prev, n_now, ch, type_keys,
                           np.array(sorted(dirty), np.uint16), [prev_lab[c] for c in sorted(gone)],
                           cat("par_dirty").astype(np.uint32), cat("par_gone").astype(np.uint32))
 
@@ -341,21 +330,27 @@ class ShardedScan:
         rank's status.  If any rank's call failed, EVERY rank resets its previous result and raises KvgError, so that
         the ranks never diff against previous results of different steps; the next step then reports everything as
         added on every rank."""
-        err, out = None, None
-        try:
-            out = self.ctx.dev_scan_pci_shard_fetch_delta()
-        except L.KvgError as e:
-            err = e
-        if all(s[:1] == b"\1" for s in self._statuses(b"\0" if err else b"\1")):
-            return out
-        self.ctx.dev_scan_pci_shard_delta_reset()
-        if err is not None:
-            raise err
-        raise L.KvgError(L.KVG_ESTATE, "fetch_delta failed on another rank; every rank's previous result is reset")
+        return self._collective(self.ctx.dev_scan_pci_shard_fetch_delta, self.ctx.dev_scan_pci_shard_delta_reset,
+                                "fetch_delta")
 
     def delta_reset(self):
         """Forget this rank's previous result (call it on every rank)."""
         self.ctx.dev_scan_pci_shard_delta_reset()
+
+    def _collective(self, call, reset, name: str):
+        """call() on this rank.  If it raised KvgError on any rank, every rank calls reset() and raises: the rank's own
+        error, or KVG_ESTATE for a failure elsewhere."""
+        err, out = None, None
+        try:
+            out = call()
+        except L.KvgError as e:
+            err = e
+        if all(s[:1] == b"\1" for s in self._statuses(b"\0" if err else b"\1")):
+            return out
+        reset()
+        if err is not None:
+            raise err
+        raise L.KvgError(L.KVG_ESTATE, "%s failed on another rank; every rank's previous result is reset" % name)
 
     def _statuses(self, mine: bytes) -> list:
         """every rank's status byte, in rank order"""
@@ -374,18 +369,9 @@ class ShardedScan:
         Context.dev_scan_mdev_shard_fetch_delta.  Collective here exactly like fetch_delta: if any rank's call failed,
         EVERY rank resets its previous result and raises KvgError.  The labels of the dictionary the delta was taken
         against are kept, so that merge_mdev_deltas needs only the ranks' parts."""
-        err, out = None, None
-        try:
-            out = self.ctx.dev_scan_mdev_shard_fetch_delta()
-        except L.KvgError as e:
-            err = e
-        if all(s[:1] == b"\1" for s in self._statuses(b"\0" if err else b"\1")):
-            self.mdev_prev_labels, self.mdev_labels = self.mdev_labels, list(out[0].by_type.labels)
-            return out
-        self.mdev_delta_reset()
-        if err is not None:
-            raise err
-        raise L.KvgError(L.KVG_ESTATE, "fetch_mdev_delta failed on another rank; every rank's previous result is reset")
+        out = self._collective(self.ctx.dev_scan_mdev_shard_fetch_delta, self.mdev_delta_reset, "fetch_mdev_delta")
+        self.mdev_prev_labels, self.mdev_labels = self.mdev_labels, list(out[0].by_type.labels)
+        return out
 
     def mdev_delta_reset(self):
         """Forget this rank's previous mdev result (call it on every rank)."""

@@ -1,11 +1,36 @@
 // delta_emu.cpp — K7, the re-scan deltas of csrc/kvg_delta.cuh, compiled for the CPU from their real source on top
-// of warp_emu.h, with the launch shapes of kvg_api_delta.inc: k_delta_merge<PciDeltaRec> then k_delta_lists
-// (kvg_scan_pci_delta), k_mdev_delta_types, k_delta_merge<MdevDeltaRec>, k_delta_lists (kvg_scan_mdev_delta), and the
-// sharded forms through k_delta_merge_shard<PciDeltaRec> / <MdevDeltaRec>.
+// of warp_emu.h.  The launch arguments come from the builders of kvg_delta.cuh that kvg_api_delta.inc uses, in its
+// launch order: k_delta_merge<PciDeltaRec> then k_delta_lists (kvg_scan_pci_delta), k_mdev_delta_types,
+// k_delta_merge<MdevDeltaRec>, k_delta_lists (kvg_scan_mdev_delta), and the sharded forms through
+// k_delta_merge_shard<PciDeltaRec> / <MdevDeltaRec>.
 #define KVG_HOST_EMU 1
 #include "warp_emu.h"
 #include "../../kubevirt-gpu-device-plugin_b200/csrc/kvg_delta.cuh"
 using namespace kvg;
+
+namespace {
+// one call: its control block and the caller's four arrays of tag words
+struct Call {
+  ScanCtrl ctrl{};
+  uint32_t* flag[4];
+  Call(uint32_t* flags, uint32_t flag_cap) {
+    for (int k = 0; k < 4; k++) flag[k] = flags + (size_t)k * flag_cap;
+  }
+  // the merge (merge(tile_state) launches it), the lists behind it, then counts: {n_changes, error, the list lengths}
+  template <class Tr, class Merge>
+  void run(const DeltaMergeOp<Tr>& op, void* const (&lists)[4], bool gone0_u16, uint32_t* counts, Merge&& merge) {
+    DeltaListArgs la;
+    const uint32_t merge_tiles = delta_merge_tiles(op.n), list_tiles = delta_list_args(la, op, lists, gone0_u16);
+    std::vector<uint64_t> state(merge_tiles + 1 + 4 * (list_tiles + 1), 0);
+    merge(state.data());
+    emu_launch(k_delta_lists, dim3(list_tiles, 4), KVG_BLOCK, la, state.data() + merge_tiles + 1, list_tiles + 1,
+               op.tag + 1);
+    counts[0] = ctrl.reserved2[DELTA_W_CHANGES];
+    counts[1] = ctrl.reserved2[DELTA_W_ERROR];
+    for (int k = 0; k < 4; k++) counts[2 + k] = ctrl.reserved2[DELTA_W_LISTS + k];
+  }
+};
+}  // namespace
 
 extern "C" {
 
@@ -17,37 +42,12 @@ extern "C" {
 int emu_delta(const uint4* prev, uint32_t n_prev, const uint4* now, uint32_t n_now, const uint32_t* const* keys,
               const uint32_t* n_keys, uint32_t* flags, uint32_t flag_cap, uint32_t tag, uint4* changes, uint32_t* dev_dirty,
               uint16_t* dev_gone, uint32_t* grp_dirty, uint32_t* grp_gone, uint32_t* counts) {
-  ScanCtrl ctrl;
-  memset(&ctrl, 0, sizeof ctrl);
-  const uint32_t M = n_prev + n_now;
-  const uint32_t merge_tiles = M ? (M + DELTA_TILE - 1) / DELTA_TILE : 1;
-  uint32_t list_tiles = 1;
-  for (int k = 0; k < 4; k++) list_tiles = max(list_tiles, (n_keys[k] + C_TILE - 1) / C_TILE);
-  std::vector<uint64_t> state(merge_tiles + 1 + 4 * (list_tiles + 1), 0);
-  uint32_t* f[4];
-  for (int k = 0; k < 4; k++) f[k] = flags + (size_t)k * flag_cap;
-  DeltaMergeOp<PciDeltaRec> op = {};
-  op.prev = prev;
-  op.n_prev = n_prev;
-  op.now = now;
-  op.n_now = n_now;
-  op.n = M;
-  op.out = changes;
-  op.ctrl = &ctrl;
-  op.k0 = {keys[0], n_keys[0], f[0], keys[1], n_keys[1], f[1], nullptr};
-  op.k1 = {keys[2], n_keys[2], f[2], keys[3], n_keys[3], f[3], nullptr};
-  op.tag = tag;
-  emu_launch(k_delta_merge<PciDeltaRec>, dim3(merge_tiles), DELTA_THREADS, op, state.data());
-  DeltaListArgs la;
-  uint32_t* cnt = &ctrl.reserved2[DELTA_W_LISTS];
-  la.o[0] = {f[0], n_keys[0], tag, nullptr, dev_dirty, nullptr, cnt + 0};
-  la.o[1] = {f[1], n_keys[1], tag, keys[1], nullptr, dev_gone, cnt + 1};
-  la.o[2] = {f[2], n_keys[2], tag, nullptr, grp_dirty, nullptr, cnt + 2};
-  la.o[3] = {f[3], n_keys[3], tag, keys[3], grp_gone, nullptr, cnt + 3};
-  emu_launch(k_delta_lists, dim3(list_tiles, 4), KVG_BLOCK, la, state.data() + merge_tiles + 1, list_tiles + 1, tag + 1);
-  counts[0] = ctrl.reserved2[DELTA_W_CHANGES];
-  counts[1] = ctrl.reserved2[DELTA_W_ERROR];
-  for (int k = 0; k < 4; k++) counts[2 + k] = cnt[k];
+  Call c(flags, flag_cap);
+  const auto op = delta_merge_op<PciDeltaRec>(prev, n_prev, now, n_now, changes, &c.ctrl, keys, n_keys, c.flag, nullptr,
+                                              tag);
+  c.run(op, {dev_dirty, dev_gone, grp_dirty, grp_gone}, true, counts, [&](uint64_t* state) {
+    emu_launch(k_delta_merge<PciDeltaRec>, dim3(delta_merge_tiles(op.n)), DELTA_THREADS, op, state);
+  });
   return 0;
 }
 
@@ -59,43 +59,15 @@ int emu_shard_delta(const uint4* const* prev, const uint32_t* n_prev, const uint
                     const uint32_t* const* keys, const uint32_t* n_keys, uint32_t* flags, uint32_t flag_cap,
                     uint32_t tag, uint4* changes, uint32_t* dev_dirty, uint16_t* dev_gone, uint32_t* grp_dirty,
                     uint32_t* grp_gone, uint32_t* counts) {
-  ScanCtrl ctrl;
-  memset(&ctrl, 0, sizeof ctrl);
-  const uint32_t M = n_prev[0] + n_now[0];
-  const uint32_t merge_tiles = M ? (M + DELTA_TILE - 1) / DELTA_TILE : 1;
-  uint32_t list_tiles = 1;
-  for (int k = 0; k < 4; k++) list_tiles = max(list_tiles, (n_keys[k] + C_TILE - 1) / C_TILE);
-  std::vector<uint64_t> state(merge_tiles + 1 + 4 * (list_tiles + 1), 0);
-  uint32_t* f[4];
-  for (int k = 0; k < 4; k++) f[k] = flags + (size_t)k * flag_cap;
-  DeltaShardArgs<PciDeltaRec> a;
-  uint32_t cols = merge_tiles;
-  for (int y = 0; y < 3; y++) {
-    DeltaMergeOp<PciDeltaRec>& o = a.o[y];
-    o = {};
-    o.prev = prev[y];
-    o.n_prev = n_prev[y];
-    o.now = now[y];
-    o.n_now = n_now[y];
-    o.n = n_prev[y] + n_now[y];
-    o.out = y == 0 ? changes : nullptr;
-    o.ctrl = &ctrl;
-    if (y == 1) o.k0 = {keys[0], n_keys[0], f[0], keys[1], n_keys[1], f[1], nullptr};
-    if (y == 2) o.k1 = {keys[2], n_keys[2], f[2], keys[3], n_keys[3], f[3], nullptr};
-    o.tag = tag;
-    cols = max(cols, (o.n + DELTA_TILE - 1) / DELTA_TILE);
-  }
-  emu_launch(k_delta_merge_shard<PciDeltaRec>, dim3(cols, 3), DELTA_THREADS, a, state.data());
-  DeltaListArgs la;
-  uint32_t* cnt = &ctrl.reserved2[DELTA_W_LISTS];
-  la.o[0] = {f[0], n_keys[0], tag, nullptr, dev_dirty, nullptr, cnt + 0};
-  la.o[1] = {f[1], n_keys[1], tag, keys[1], nullptr, dev_gone, cnt + 1};
-  la.o[2] = {f[2], n_keys[2], tag, nullptr, grp_dirty, nullptr, cnt + 2};
-  la.o[3] = {f[3], n_keys[3], tag, keys[3], grp_gone, nullptr, cnt + 3};
-  emu_launch(k_delta_lists, dim3(list_tiles, 4), KVG_BLOCK, la, state.data() + merge_tiles + 1, list_tiles + 1, tag + 1);
-  counts[0] = ctrl.reserved2[DELTA_W_CHANGES];
-  counts[1] = ctrl.reserved2[DELTA_W_ERROR];
-  for (int k = 0; k < 4; k++) counts[2 + k] = cnt[k];
+  Call c(flags, flag_cap);
+  const auto op = delta_merge_op<PciDeltaRec>(prev[0], n_prev[0], now[0], n_now[0], changes, &c.ctrl, keys, n_keys,
+                                              c.flag, nullptr, tag);
+  c.run(op, {dev_dirty, dev_gone, grp_dirty, grp_gone}, true, counts, [&](uint64_t* state) {
+    DeltaShardArgs<PciDeltaRec> a;
+    const uint32_t cols = delta_shard_args(a, op, {prev[1], prev[2]}, {n_prev[1], n_prev[2]}, {now[1], now[2]},
+                                           {n_now[1], n_now[2]});
+    emu_launch(k_delta_merge_shard<PciDeltaRec>, dim3(cols, 3), DELTA_THREADS, a, state);
+  });
   return 0;
 }
 
@@ -114,42 +86,15 @@ int emu_mdev_delta(const uint4* prev, uint32_t n_prev, const uint4* now, uint32_
                    const uint32_t* n_keys, const EmuLabels* labels, uint64_t* table, uint32_t* xlate, uint32_t* flags,
                    uint32_t flag_cap, uint32_t tag, uint4* changes, uint32_t* type_dirty, uint32_t* type_gone,
                    uint32_t* par_dirty, uint32_t* par_gone, uint32_t* counts) {
-  ScanCtrl ctrl;
-  memset(&ctrl, 0, sizeof ctrl);
-  uint32_t slots = 64;
-  while (slots < 2 * n_keys[0]) slots <<= 1;
+  Call c(flags, flag_cap);
   const MdevTypeLabels ln = {keys[0], n_keys[0], labels[0].bytes, labels[0].off, labels[0].len, labels[0].hash};
   const MdevTypeLabels lp = {keys[1], n_keys[1], labels[1].bytes, labels[1].off, labels[1].len, labels[1].hash};
-  emu_launch(k_mdev_delta_types, dim3(1), XMAP_THREADS, ln, lp, table, slots - 1, tag, xlate);
-  const uint32_t M = n_prev + n_now;
-  const uint32_t merge_tiles = M ? (M + DELTA_TILE - 1) / DELTA_TILE : 1;
-  uint32_t list_tiles = 1;
-  for (int k = 0; k < 4; k++) list_tiles = max(list_tiles, (n_keys[k] + C_TILE - 1) / C_TILE);
-  std::vector<uint64_t> state(merge_tiles + 1 + 4 * (list_tiles + 1), 0);
-  uint32_t* f[4];
-  for (int k = 0; k < 4; k++) f[k] = flags + (size_t)k * flag_cap;
-  DeltaMergeOp<MdevDeltaRec> op = {};
-  op.prev = reinterpret_cast<const MdevItem*>(prev);
-  op.n_prev = n_prev;
-  op.now = reinterpret_cast<const MdevItem*>(now);
-  op.n_now = n_now;
-  op.n = M;
-  op.out = changes;
-  op.ctrl = &ctrl;
-  op.k0 = {keys[0], n_keys[0], f[0], keys[1], n_keys[1], f[1], xlate};
-  op.k1 = {keys[2], n_keys[2], f[2], keys[3], n_keys[3], f[3], nullptr};
-  op.tag = tag;
-  emu_launch(k_delta_merge<MdevDeltaRec>, dim3(merge_tiles), DELTA_THREADS, op, state.data());
-  DeltaListArgs la;
-  uint32_t* cnt = &ctrl.reserved2[DELTA_W_LISTS];
-  la.o[0] = {f[0], n_keys[0], tag, nullptr, type_dirty, nullptr, cnt + 0};
-  la.o[1] = {f[1], n_keys[1], tag, keys[1], type_gone, nullptr, cnt + 1};
-  la.o[2] = {f[2], n_keys[2], tag, nullptr, par_dirty, nullptr, cnt + 2};
-  la.o[3] = {f[3], n_keys[3], tag, keys[3], par_gone, nullptr, cnt + 3};
-  emu_launch(k_delta_lists, dim3(list_tiles, 4), KVG_BLOCK, la, state.data() + merge_tiles + 1, list_tiles + 1, tag + 1);
-  counts[0] = ctrl.reserved2[DELTA_W_CHANGES];
-  counts[1] = ctrl.reserved2[DELTA_W_ERROR];
-  for (int k = 0; k < 4; k++) counts[2 + k] = cnt[k];
+  emu_launch(k_mdev_delta_types, dim3(1), XMAP_THREADS, ln, lp, table, delta_xmap_mask(n_keys[0]), tag, xlate);
+  const auto op = delta_merge_op<MdevDeltaRec>(prev, n_prev, now, n_now, changes, &c.ctrl, keys, n_keys, c.flag, xlate,
+                                               tag);
+  c.run(op, {type_dirty, type_gone, par_dirty, par_gone}, false, counts, [&](uint64_t* state) {
+    emu_launch(k_delta_merge<MdevDeltaRec>, dim3(delta_merge_tiles(op.n)), DELTA_THREADS, op, state);
+  });
   return 0;
 }
 
@@ -165,49 +110,18 @@ int emu_mdev_shard_delta(const uint4* const* prev, const uint32_t* n_prev, const
                          uint64_t* table, uint32_t* xlate, uint32_t* flags, uint32_t flag_cap, uint32_t tag,
                          uint4* changes, uint32_t* type_dirty, uint32_t* type_gone, uint32_t* par_dirty,
                          uint32_t* par_gone, uint32_t* counts) {
-  ScanCtrl ctrl;
-  memset(&ctrl, 0, sizeof ctrl);
-  uint32_t slots = 64;
-  while (slots < 2 * n_canon[0]) slots <<= 1;
+  Call c(flags, flag_cap);
   const MdevTypeLabels ln = {canon[0], n_canon[0], labels[0].bytes, labels[0].off, labels[0].len, labels[0].hash};
   const MdevTypeLabels lp = {canon[1], n_canon[1], labels[1].bytes, labels[1].off, labels[1].len, labels[1].hash};
-  emu_launch(k_mdev_delta_types, dim3(1), XMAP_THREADS, ln, lp, table, slots - 1, tag, xlate);
-  const uint32_t M = n_prev[0] + n_now[0];
-  const uint32_t merge_tiles = M ? (M + DELTA_TILE - 1) / DELTA_TILE : 1;
-  uint32_t list_tiles = 1;
-  for (int k = 0; k < 4; k++) list_tiles = max(list_tiles, (n_keys[k] + C_TILE - 1) / C_TILE);
-  std::vector<uint64_t> state(merge_tiles + 1 + 4 * (list_tiles + 1), 0);
-  uint32_t* f[4];
-  for (int k = 0; k < 4; k++) f[k] = flags + (size_t)k * flag_cap;
-  const DeltaKeys xlate_only = {nullptr, 0, nullptr, nullptr, 0, nullptr, xlate};
-  DeltaShardArgs<MdevDeltaRec> a;
-  uint32_t cols = merge_tiles;
-  for (int y = 0; y < 3; y++) {
-    DeltaMergeOp<MdevDeltaRec>& o = a.o[y];
-    o = {};
-    o.prev = reinterpret_cast<const MdevItem*>(prev[y]);
-    o.n_prev = n_prev[y];
-    o.now = reinterpret_cast<const MdevItem*>(now[y]);
-    o.n_now = n_now[y];
-    o.n = n_prev[y] + n_now[y];
-    o.out = y == 0 ? changes : nullptr;
-    o.ctrl = &ctrl;
-    o.k0 = y == 1 ? DeltaKeys{keys[0], n_keys[0], f[0], keys[1], n_keys[1], f[1], xlate} : xlate_only;
-    if (y == 2) o.k1 = {keys[2], n_keys[2], f[2], keys[3], n_keys[3], f[3], nullptr};
-    o.tag = tag;
-    cols = max(cols, (o.n + DELTA_TILE - 1) / DELTA_TILE);
-  }
-  emu_launch(k_delta_merge_shard<MdevDeltaRec>, dim3(cols, 3), DELTA_THREADS, a, state.data());
-  DeltaListArgs la;
-  uint32_t* cnt = &ctrl.reserved2[DELTA_W_LISTS];
-  la.o[0] = {f[0], n_keys[0], tag, nullptr, type_dirty, nullptr, cnt + 0};
-  la.o[1] = {f[1], n_keys[1], tag, keys[1], type_gone, nullptr, cnt + 1};
-  la.o[2] = {f[2], n_keys[2], tag, nullptr, par_dirty, nullptr, cnt + 2};
-  la.o[3] = {f[3], n_keys[3], tag, keys[3], par_gone, nullptr, cnt + 3};
-  emu_launch(k_delta_lists, dim3(list_tiles, 4), KVG_BLOCK, la, state.data() + merge_tiles + 1, list_tiles + 1, tag + 1);
-  counts[0] = ctrl.reserved2[DELTA_W_CHANGES];
-  counts[1] = ctrl.reserved2[DELTA_W_ERROR];
-  for (int k = 0; k < 4; k++) counts[2 + k] = cnt[k];
+  emu_launch(k_mdev_delta_types, dim3(1), XMAP_THREADS, ln, lp, table, delta_xmap_mask(n_canon[0]), tag, xlate);
+  const auto op = delta_merge_op<MdevDeltaRec>(prev[0], n_prev[0], now[0], n_now[0], changes, &c.ctrl, keys, n_keys,
+                                               c.flag, xlate, tag);
+  c.run(op, {type_dirty, type_gone, par_dirty, par_gone}, false, counts, [&](uint64_t* state) {
+    DeltaShardArgs<MdevDeltaRec> a;
+    const uint32_t cols = delta_shard_args(a, op, {prev[1], prev[2]}, {n_prev[1], n_prev[2]}, {now[1], now[2]},
+                                           {n_now[1], n_now[2]});
+    emu_launch(k_delta_merge_shard<MdevDeltaRec>, dim3(cols, 3), DELTA_THREADS, a, state);
+  });
   return 0;
 }
 
