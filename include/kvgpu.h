@@ -370,6 +370,21 @@ int kvg_scan_mdev(kvg_ctx *ctx, const kvg_mdev_rec *recs, size_t n, const kvg_ty
  * or decreasing offsets. */
 int kvg_mdev_label_match(kvg_ctx *ctx, const kvg_type_dict *files, const uint8_t *name, size_t name_len,
                          uint8_t *match);
+/* Allocate-time re-check of the passthrough plugin (generic_device_plugin.go:387-399) for every member of every
+ * requested IOMMU group, in the order the reference visits them.  Record i passes iff KVG_PF_IOMMU_ERR is clear,
+ * recs[i].iommu_group == want_group[i], KVG_PF_VENDOR_ERR is clear and recs[i].vendor == 0x10de; addr, device, driver,
+ * numa and every other flag are ignored.  *first_bad = the smallest failing index, or n when all pass.
+ * Handles: intern the group strings per call, one handle per distinct string, and use the same table for the link
+ * just read (recs[i].iommu_group) and the group the maps hold (want_group[i]), so equal handles mean equal strings.
+ * Never parse the strings as numbers: the reference compares strings, so "042" is not "42".  The vendor is 0x10de
+ * iff the vendor file read back as exactly "10de" (any other value, e.g. 0xffff, fails).
+ * One launch per call with n > 0, none for n = 0 (*first_bad = 0) or a refused call.  The call uses buffers of its
+ * own: no scan, fetch, delta, health or name-table state changes, and it does not wait for a pci.ids parse, so it
+ * may run between kvg_dev_scan_pci and kvg_dev_scan_pci_fetch.
+ * KVG_EINVAL (nothing launched, *first_bad unwritten): ctx or first_bad NULL; recs or want_group NULL with n > 0;
+ * n > UINT32_MAX. */
+int kvg_pci_group_check(kvg_ctx *ctx, const kvg_pci_rec *recs, const uint32_t *want_group, size_t n,
+                        size_t *first_bad);
 /* Classify `recs`, diff against the alive-set of the previous call on this context (first call:
  * against "nothing alive").  A call with a different n re-arms the same way, as does
  * kvg_health_reset(); n = 0 returns an empty delta.  Pinned (cudaHostAlloc / registered) `recs` of

@@ -13,6 +13,7 @@
 //                          (Keyed<Rule>, either form: the prior state joined by UUID / address instead of by index)
 //   k_mdev_labels / _canon K5: label rule (:341-342) + merge of equal labels
 //   k_mdev_label_match     the same label rule against one name: the vGPU plugin's Allocate-time re-check
+//   k_pci_group_check      the passthrough plugin's Allocate-time re-check: group link and vendor per group member
 //   k_gen_*                counter-based synthetic snapshots (twins of oracle/kvg_oracle.c kvo_gen_*)
 #pragma once
 #include "../../include/kvgpu.h"
@@ -78,6 +79,14 @@ __device__ __forceinline__ bool pci_record_alive(const uint4& r) {
   static_assert(KVG_DRV_VFIO_PCI == 1 && KVG_DRV_NVGRACE == 2, "driver codes");
   static_assert((KVG_PF_VENDOR_ERR | KVG_PF_DRIVER_ERR | KVG_PF_IOMMU_ERR | KVG_PF_DEVICE_ERR) == 0xf, "flags");
   return (r.y & 0xffffu) == 0x10deu && ((r.w & 0x0fffu) - 1u) < 2u;
+}
+// The passthrough plugin's Allocate-time re-check of one group member (generic_device_plugin.go:388-397): its
+// iommu_group link reads back as the group the maps hold for it (`want`, the same interned handle), and its vendor
+// reads back as "10de".  Nothing else of the record counts: not the driver, the device id, the NUMA node or any other
+// read error, so the rule stays the reference's whatever pci_record_alive comes to require.
+__device__ __forceinline__ bool pci_group_check_pass(const uint4& r, uint32_t want) {
+  const uint32_t flags = (r.w >> 8) & 0xffu;
+  return !(flags & KVG_PF_IOMMU_ERR) && r.z == want && !(flags & KVG_PF_VENDOR_ERR) && (r.y & 0xffffu) == 0x10deu;
 }
 // What the PCI and mdev classify operators share: a survivor goes out as Self::UNITS 16-byte streaming stores of
 // Self::make, and the largest Self::keys of the survivors a thread wrote bound the radix passes of the two
@@ -651,6 +660,35 @@ __global__ void __launch_bounds__(LABEL_MATCH_THREADS) k_mdev_label_match(const 
   __syncthreads();
   if (threadIdx.x == 0) {
     __threadfence_system();
+    *((volatile uint32_t*)seq_host) = seq;
+  }
+}
+
+// Allocate-time re-check of the passthrough plugin (generic_device_plugin.go:387-399): the smallest i whose record
+// fails pci_group_check_pass against want[i], or n when every record passes.  One CTA, striding; each thread stops at
+// its first failure (its indices ascend), the warps reduce with one REDUX each and the block through one shared word.
+// The index goes straight to mapped host memory, then the sequence word the host polls.
+static constexpr int GROUP_CHECK_THREADS = 1024;
+__global__ void __launch_bounds__(GROUP_CHECK_THREADS) k_pci_group_check(const uint4* __restrict__ recs,
+                                                                         const uint32_t* __restrict__ want, uint32_t n,
+                                                                         uint32_t* first_bad_host, uint32_t* seq_host,
+                                                                         uint32_t seq) {
+  pdl_enter();
+  __shared__ uint32_t block_min;
+  if (threadIdx.x == 0) block_min = n;
+  uint32_t m = n;
+  for (uint32_t i = threadIdx.x; i < n; i += blockDim.x)
+    if (!pci_group_check_pass(recs[i], want[i])) {
+      m = i;
+      break;
+    }
+  m = warp_min(m);
+  __syncthreads();  // block_min is initialised
+  if (lane_id() == 0) atomicMin(&block_min, m);
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    *((volatile uint32_t*)first_bad_host) = block_min;
+    __threadfence_system();  // the index is on its way before the sequence word
     *((volatile uint32_t*)seq_host) = seq;
   }
 }

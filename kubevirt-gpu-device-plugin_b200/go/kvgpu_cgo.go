@@ -43,7 +43,7 @@ var kvgCtx *C.kvg_ctx
 var kvgLoadedPath string
 
 // A kvg_ctx is single-threaded (include/kvgpu.h).  The scans run on the main goroutine before any server
-// starts, but getDeviceNameGPU and revalidateBatchGPU are reached from gRPC handler goroutines (grpc-go runs
+// starts, but getDeviceNameGPU and the revalidate*GPU functions are reached from gRPC handler goroutines (grpc-go runs
 // one goroutine per stream) and from healthCheck goroutines: every entry into the library takes kvgMu.
 var kvgMu sync.Mutex
 
@@ -427,6 +427,60 @@ func revalidateBatchGPU(devs []string, want []string) (first int, err error) {
 		}
 	}
 	return -1, nil
+}
+
+// revalidateGroupsGPU is the same re-check as revalidateBatchGPU, with the same contract and call site, as its own
+// rule in one launch of kvg_pci_group_check (Python twin: kvgpu/serve.py GroupCheck, tested against BatchRevalidator
+// by tests/test_serve_group_check.py).  A device passes iff its iommu_group link read back as want[i] and its vendor
+// as "10de" (generic_device_plugin.go:388-397); no driver or device id is pinned, because the rule reads neither.
+// The group strings are interned per call and never parsed as numbers: the reference compares strings, so "042" is
+// not "42".  It touches no scan state, so it may run while a scan's result is still to be fetched.
+func revalidateGroupsGPU(devs []string, want []string) (first int, err error) {
+	if len(devs) == 0 {
+		return -1, nil
+	}
+	kvgMu.Lock()
+	defer kvgMu.Unlock()
+	if err := kvgEnsure(); err != nil {
+		return 0, err
+	}
+	intern := map[string]uint32{}
+	id := func(s string) uint32 {
+		if v, ok := intern[s]; ok {
+			return v
+		}
+		v := uint32(len(intern))
+		intern[s] = v
+		return v
+	}
+	recs := make([]C.kvg_pci_rec, len(devs))
+	wantGroup := make([]C.uint32_t, len(devs))
+	for i, addr := range devs {
+		r := &recs[i]
+		r.addr = C.uint32_t(i)
+		r.vendor = 0xffff
+		wantGroup[i] = C.uint32_t(id(want[i]))
+		group, err := readLink(basePath, addr, "iommu_group")
+		if err != nil {
+			r.flags |= C.KVG_PF_IOMMU_ERR
+		} else {
+			r.iommu_group = C.uint32_t(id(group))
+		}
+		vendorID, err := readIDFromFile(basePath, addr, "vendor")
+		if err != nil {
+			r.flags |= C.KVG_PF_VENDOR_ERR
+		} else if vendorID == nvidiaVendorID {
+			r.vendor = 0x10de
+		}
+	}
+	var bad C.size_t
+	if rc := C.kvg_pci_group_check(kvgCtx, &recs[0], &wantGroup[0], C.size_t(len(recs)), &bad); rc != C.KVG_OK {
+		return 0, fmt.Errorf("kvg_pci_group_check: %s", C.GoString(C.kvg_last_error(kvgCtx)))
+	}
+	if int(bad) == len(devs) {
+		return -1, nil
+	}
+	return int(bad), nil
 }
 
 // revalidateVgpuBatchGPU is the Allocate-time re-check of generic_vgpu_device_plugin.go:216-228 for ALL IDs of an

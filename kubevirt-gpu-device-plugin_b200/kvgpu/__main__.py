@@ -49,7 +49,7 @@ def main(argv=None) -> int:
             return 0
         from . import dpapi, serve
         sockdir = args.socket_dir or dpapi.DEVICE_PLUGIN_PATH
-        reval = serve.BatchRevalidator(ds.ctx.scan_pci, args.base_path)
+        reval = serve.GroupCheck(ds.ctx.pci_group_check, args.base_path)
         vgpu_check = serve.MdevLabelCheck(ds.ctx.mdev_label_match, args.vgpu_base_path)
         plugins = serve.plugins_from_specs(specs, ds.maps, reval, vgpu_check=vgpu_check, socket_dir=sockdir,
                                            base_path=args.base_path, root_path=args.root_path,

@@ -159,6 +159,7 @@ def load() -> C.CDLL:
         "kvg_scan_pci": (C.c_int, [vp, vp, sz, P(P(PciResultC))]),
         "kvg_scan_mdev": (C.c_int, [vp, vp, sz, P(TypeDict), P(P(MdevResultC))]),
         "kvg_mdev_label_match": (C.c_int, [vp, P(TypeDict), vp, sz, vp]),
+        "kvg_pci_group_check": (C.c_int, [vp, vp, vp, sz, P(sz)]),
         "kvg_health_rescan": (C.c_int, [vp, vp, sz, P(P(HealthDeltaC))]),
         "kvg_health_reset": (C.c_int, [vp]),
         "kvg_health_rescan_mdev": (C.c_int, [vp, vp, sz, u32, vp, sz, P(P(HealthDeltaC))]),

@@ -267,6 +267,19 @@ class Context:
         del keep
         return match[:len(raw_files)].astype(bool)
 
+    def pci_group_check(self, recs: np.ndarray, want) -> int | None:
+        """The passthrough plugin's Allocate-time re-check (include/kvgpu.h kvg_pci_group_check), one launch: the
+        index of the first record whose iommu_group is not want[i] or whose vendor is not 10de (or whose read of
+        either failed), or None when every record passes.  Group handles are interned strings, never numbers."""
+        recs = np.ascontiguousarray(recs, dtype=L.PCI_REC)
+        want = np.ascontiguousarray(want, dtype=np.uint32)
+        if len(want) != len(recs):
+            raise ValueError("pci_group_check: %d records but %d wanted groups" % (len(recs), len(want)))
+        first = C.c_size_t()
+        self._ck(self._lib.kvg_pci_group_check(self._h, recs.ctypes.data, want.ctypes.data, len(recs),
+                                               C.byref(first)))
+        return None if first.value == len(recs) else first.value
+
     def _take_health(self, res) -> HealthDelta:
         r = res.contents
         out = HealthDelta(int(r.n_records), int(r.n_alive),

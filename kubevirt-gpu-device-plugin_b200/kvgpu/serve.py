@@ -14,8 +14,9 @@ reference's generic_device_plugin_test.go.  In a deployment these servers stay i
 Allocate" is testable end to end in an image without a Go toolchain.
 
 Nothing here computes on the CPU what the scan computes on the GPU: the maps come from
-plugin.DiscoveryScan (libkvgpu.so); the passthrough re-validation's classification goes through
-Context.scan_pci (K3), the vGPU plugin's label check through Context.mdev_label_match (MdevLabelCheck;
+plugin.DiscoveryScan (libkvgpu.so); the passthrough re-validation's group and vendor rule goes through
+Context.pci_group_check (GroupCheck; BatchRevalidator, the same check through Context.scan_pci (K3), is the
+reference it is tested against), the vGPU plugin's label check through Context.mdev_label_match (MdevLabelCheck;
 a vGPU plugin built without a check keeps the reference's CPU rule, the path the GPU check is tested
 against); the health feeds through Context.health_rescan, Context.health_rescan_mdev and
 Context.health_rescan_groups and their keyed forms (K6); the
@@ -234,6 +235,57 @@ class BatchRevalidator:
         return None
 
 
+class GroupCheck:
+    """The passthrough plugin's Allocate-time re-check (generic_device_plugin.go:387-399) as its own rule in one
+    launch: a drop-in `revalidate` for GenericDevicePlugin with BatchRevalidator's contract, which stays as the
+    reference this check is tested against.
+
+    Every device's iommu_group link and vendor are read with the reference's readers, in the reference's order.  What
+    they returned goes to ONE `group_check` call (Context.pci_group_check): per device a record with the read errors,
+    the link's group and the vendor (0x10de iff it read "10de"), and the group the maps hold for it.  The group
+    strings are interned per call, so equal handles mean equal strings ("042" is not "42").  Nothing in the record
+    but those reads matters to the rule, so no driver or device id is pinned."""
+
+    def __init__(self, group_check, base_path: str = "/sys/bus/pci/devices", read_link=_read_link, read_id=_read_id):
+        self.group_check, self.base_path = group_check, base_path
+        self.read_link, self.read_id = read_link, read_id
+
+    def __call__(self, pairs):
+        """pairs: [(addr, expected iommu group)] in the order the reference would visit them.
+        Returns the index of the first device the reference would reject, or None.  A reader panic
+        (short vendor file) is re-raised only if the reference would have reached that read."""
+        n = len(pairs)
+        if n == 0:
+            return None
+        recs, want = np.zeros(n, dtype=L.PCI_REC), np.zeros(n, dtype=np.uint32)
+        intern, link_ok, panics = {}, [False] * n, {}
+        for i, (addr, expect) in enumerate(pairs):
+            want[i] = intern.setdefault(expect, len(intern))
+            flags, vendor, group = 0, 0xFFFF, 0
+            got, err = self.read_link(self.base_path, addr, "iommu_group")
+            if err:
+                flags |= L.PF_IOMMU_ERR
+            else:
+                group = intern.setdefault(got, len(intern))
+                link_ok[i] = got == expect
+            try:
+                v, err = self.read_id(self.base_path, addr, "vendor")
+            except ReferencePanic as e:
+                panics[i] = e
+                v, err = "", True
+            if err:
+                flags |= L.PF_VENDOR_ERR
+            elif v == NVIDIA_VENDOR_ID:
+                vendor = 0x10de
+            recs[i] = (i, vendor, 0, group, 0, flags, 0)
+        bad = self.group_check(recs, want)
+        # a panicking read fails its record, so the only one the reference can reach is the first rejected device,
+        # and only when its link check passed (the vendor is read after it)
+        if bad is not None and bad in panics and link_ok[bad]:
+            raise panics[bad]
+        return bad
+
+
 # ------------------------------------------------------------------------------------------------
 # the plugins
 # ------------------------------------------------------------------------------------------------
@@ -385,7 +437,7 @@ class _PluginBase:
 class GenericDevicePlugin(_PluginBase):
     """The passthrough plugin (generic_device_plugin.go).  `maps` supplies what returnIommuMap /
     returnBdfToIommuMap supply in the reference; `revalidate` is the Allocate-time re-check
-    (default: BatchRevalidator over the given scan function)."""
+    (GroupCheck, or BatchRevalidator over a scan function)."""
 
     def __init__(self, device_name, device_path, devs, maps: Maps, *, revalidate=None,
                  base_path="/sys/bus/pci/devices", root_path="/", discover_egm=None, **kw):

@@ -224,4 +224,13 @@ int emu_mdev_label_match(const uint8_t* raw, const uint32_t* raw_off, uint32_t n
   return 0;
 }
 
+// kvg_pci_group_check's kernel in its launch shape (one CTA of GROUP_CHECK_THREADS): recs: n x 16 B records; want: n
+// group handles.  first_bad_out: the smallest failing index, or n; seq_out: the sequence word (7 when done).
+int emu_pci_group_check(const uint4* recs, const uint32_t* want, uint32_t n, uint32_t* first_bad_out,
+                        uint32_t* seq_out) {
+  if (n == 0) return -1;
+  emu_launch(k_pci_group_check, dim3(1), GROUP_CHECK_THREADS, recs, want, n, first_bad_out, seq_out, 7u);
+  return 0;
+}
+
 }  // extern "C"

@@ -1,16 +1,19 @@
-"""Latency of the vGPU plugin's Allocate-time label check on the GPU (kvg_mdev_label_match), beside the passthrough
-plugin's re-validation batch (kvg_scan_pci, the figure bench.py reports as allocate_revalidation) and the CPU rule of
-serve._read_vgpu_label, in one process.
+"""Latency of the Allocate-time re-checks on the GPU: the vGPU plugin's label check (kvg_mdev_label_match) and the
+passthrough plugin's group check (kvg_pci_group_check), beside the passthrough plugin's older re-validation batch
+(kvg_scan_pci, the figure bench.py reports as allocate_revalidation) and the CPU rule of serve._read_vgpu_label, in
+one process.
 
   (a) kvg_mdev_label_match at 1, 2, 4, 8 and 16 files, and at 4 containers x 4 files (one call per AllocateRequest:
       the 16 files of the four containers in request order);
   (b) kvg_scan_pci on a pinned batch of 16 records, as bench.py builds it;
-  (c) on the CPU, the rule inside _read_vgpu_label (strip, re.sub, decode, compare) on the same bytes in memory.
+  (c) on the CPU, the rule inside _read_vgpu_label (strip, re.sub, decode, compare) on the same bytes in memory;
+  (d) kvg_pci_group_check at 1, 2, 4, 8 and 16 records, as serve.GroupCheck builds them: the group members of (b)
+      with the groups the maps hold for them, one in three with a driver or device id the check must ignore.
 
 Each size: 50 warm-up calls, then the p50 and p99 of the host wall time of 1,000 calls; every result is checked
-against the CPU rule.  The file contents are those of a live mdev_type/name ("GRID A100-4C\\n"), with one in four of
-another type.  The card's name, power limit and maximum SM clock are read with a read-only nvidia-smi query in the
-same run.
+against the CPU rule, the group check's against its numpy restatement.  The file contents are those of a live
+mdev_type/name ("GRID A100-4C\\n"), with one in four of another type.  The card's name, power limit and maximum SM
+clock are read with a read-only nvidia-smi query in the same run.
 
     python tools/time_allocate.py [--calls 1000] [--out DIR]
 """
@@ -32,6 +35,7 @@ import kvgpu  # noqa: E402
 
 WARMUP = 50
 NAME = b"GRID_A100-4C"
+GROUP_SIZES = (1, 2, 4, 8, 16)
 
 
 def stats(lat):
@@ -54,6 +58,14 @@ def cpu_rule(raw):
     return re.sub(rb"[\t\n\f\r ]+", b"_", raw.strip(b"\n")).decode("latin-1")
 
 
+def group_rule(recs, want):
+    """generic_device_plugin.go:388-397 on kvg_pci_rec: the smallest failing index, or len(recs)."""
+    ok = (((recs["flags"] & (kvgpu._lib.PF_IOMMU_ERR | kvgpu._lib.PF_VENDOR_ERR)) == 0)
+          & (recs["iommu_group"] == want) & (recs["vendor"] == 0x10de))
+    bad = np.flatnonzero(~ok)
+    return int(bad[0]) if len(bad) else len(recs)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--calls", type=int, default=1000)
@@ -64,7 +76,7 @@ def main():
     print(card, flush=True)
     lib = kvgpu.load()
     out = {"card": card, "calls": a.calls, "warmup": WARMUP, "what": "host wall time of one call", "label_match": {},
-           "scan_pci_16": None, "cpu_rule": {}}
+           "scan_pci_16": None, "cpu_rule": {}, "group_check": {}}
     legs = [("%d" % k, k) for k in (1, 2, 4, 8, 16)] + [("4x4", 16)]
     with kvgpu.Context(0) as ctx:
         with gzip.open(os.path.join(ROOT, "tests", "golden", "pci.ids.gz"), "rb") as f:
@@ -102,12 +114,32 @@ def main():
             lib.kvg_result_free(res)
         out["scan_pci_16"] = timed(scan, a.calls)
 
+        for k in GROUP_SIZES:
+            recs = rr[:k].copy()
+            recs["driver"][::3] = kvgpu._lib.DRV_OTHER                 # ignored by the rule
+            recs["device"][1::3] = 0x1b38
+            want = np.ascontiguousarray(recs["iommu_group"], dtype=np.uint32)
+            first, expect = C.c_size_t(), group_rule(recs, want)
+
+            def check():
+                assert lib.kvg_pci_group_check(ctx.handle, recs.ctypes.data, want.ctypes.data, k, C.byref(first)) == 0
+                assert first.value == expect
+            before = ctx.launch_count
+            out["group_check"]["%d" % k] = timed(check, a.calls)
+            assert ctx.launch_count - before == WARMUP + a.calls      # one launch per call
+            bad = want.copy()
+            bad[k - 1] += 1                                            # the last member's link moved
+            assert ctx.pci_group_check(recs, bad) == group_rule(recs, bad) == k - 1
+
     print("%-28s %10s %10s" % ("call", "p50 us", "p99 us"))
     for label, _ in legs:
         s = out["label_match"][label]
         print("%-28s %10.1f %10.1f" % ("kvg_mdev_label_match " + label, s["p50_us"], s["p99_us"]))
     s = out["scan_pci_16"]
     print("%-28s %10.1f %10.1f" % ("kvg_scan_pci 16 records", s["p50_us"], s["p99_us"]))
+    for k in GROUP_SIZES:
+        s = out["group_check"]["%d" % k]
+        print("%-28s %10.1f %10.1f" % ("kvg_pci_group_check %d" % k, s["p50_us"], s["p99_us"]))
     for label, _ in legs:
         s = out["cpu_rule"][label]
         print("%-28s %10.1f %10.1f" % ("CPU rule " + label, s["p50_us"], s["p99_us"]))
