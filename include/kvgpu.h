@@ -385,6 +385,44 @@ int kvg_mdev_label_match(kvg_ctx *ctx, const kvg_type_dict *files, const uint8_t
  * n > UINT32_MAX. */
 int kvg_pci_group_check(kvg_ctx *ctx, const kvg_pci_rec *recs, const uint32_t *want_group, size_t n,
                         size_t *first_bad);
+/* GetPreferredAllocation of the passthrough plugin (generic_device_plugin.go:470-608): the NUMA packing of every
+ * container request of one PreferredAllocationRequest, in one launch.
+ * Entries: request r's entries follow those of requests 0..r-1 in `ids`, its n_must must-include IDs first, then its
+ * n_avail available IDs, each list in kubelet order (duplicates and IDs the plugin does not know included).
+ * Interning, per request: handle = one index per distinct ID string (< n_must + n_avail), so equal handles mean equal
+ * strings; node = one index per distinct NUMA node value (< n_must + n_avail), or KVG_PREF_NODE_NONE for an ID that
+ * is not a device of the plugin, a device without topology, or a device whose node is -1.  Equal handles carry equal
+ * nodes.  The device's node is that of its last entry in the plugin's device list that has topology.  Nodes are only
+ * compared for equality, so any other value (e.g. -2) is an ordinary node.
+ * Rule, with P = the number of distinct must-include IDs: P > size (size may be 0 or negative) fails with
+ * res[r].n_out = -1.  Otherwise the picks are the must-include IDs in order, then -- when P < size -- the IDs of the
+ * first candidate node (must-include nodes in order of first appearance, then the nodes of `available` in order of
+ * first appearance) whose must-include IDs plus available entries of other IDs (duplicates counted) reach size,
+ * unless that node is KVG_PREF_NODE_NONE, then available IDs in order until size; an ID is never picked twice.
+ * Output: res[r] = {n_out, P}; out_pos[first entry of r ..] holds r's n_out picks as entry positions within r
+ * (0 = its first must-include entry), in the order the reference appends them.  out_pos has room for n_ids positions;
+ * a failed request writes none.  The reference's error text is
+ * "number of MustIncludeDeviceIDs (P) exceeds allocation size (size)" for the first failing request.
+ * One launch per call with n_reqs > 0 (requests with empty lists included: they still take the size test), none for
+ * n_reqs = 0 or a refused call.  The call uses buffers of its own: no scan, fetch, delta, health or name-table state
+ * changes, and it does not wait for a pci.ids parse.
+ * KVG_EINVAL (nothing launched, res unwritten): ctx NULL; reqs or res NULL with n_reqs > 0; ids or out_pos NULL with
+ * n_ids > 0; n_ids > UINT32_MAX; sum of n_must + n_avail != n_ids; a handle or node out of its request's range. */
+#define KVG_PREF_NODE_NONE 0xffffffffu /* the reference's -1: no topology, node -1, or not a device of the plugin */
+typedef struct kvg_pref_id {
+  uint32_t handle, node;
+} kvg_pref_id;
+typedef struct kvg_pref_req {
+  uint32_t n_must, n_avail;
+  int32_t size; /* allocation_size */
+  uint32_t pad;
+} kvg_pref_req;
+typedef struct kvg_pref_res {
+  int32_t n_out; /* -1: more distinct must-include IDs than size */
+  uint32_t n_must_distinct;
+} kvg_pref_res;
+int kvg_preferred_allocation(kvg_ctx *ctx, const kvg_pref_req *reqs, uint32_t n_reqs, const kvg_pref_id *ids,
+                             size_t n_ids, kvg_pref_res *res, uint32_t *out_pos);
 /* Classify `recs`, diff against the alive-set of the previous call on this context (first call:
  * against "nothing alive").  A call with a different n re-arms the same way, as does
  * kvg_health_reset(); n = 0 returns an empty delta.  Pinned (cudaHostAlloc / registered) `recs` of

@@ -32,6 +32,7 @@
 #include "kvg_order.cuh"
 #include "kvg_shard.cuh"
 #include "kvg_delta.cuh"
+#include "kvg_alloc.cuh"
 
 using namespace kvg;
 

@@ -37,14 +37,17 @@ import (
 	"strings"
 	"sync"
 	"unsafe"
+
+	pluginapi "k8s.io/kubelet/pkg/apis/deviceplugin/v1beta1"
 )
 
 var kvgCtx *C.kvg_ctx
 var kvgLoadedPath string
 
 // A kvg_ctx is single-threaded (include/kvgpu.h).  The scans run on the main goroutine before any server
-// starts, but getDeviceNameGPU and the revalidate*GPU functions are reached from gRPC handler goroutines (grpc-go runs
-// one goroutine per stream) and from healthCheck goroutines: every entry into the library takes kvgMu.
+// starts, but getDeviceNameGPU, preferredAllocationGPU and the revalidate*GPU functions are reached from gRPC handler
+// goroutines (grpc-go runs one goroutine per stream) and from healthCheck goroutines: every entry into the library
+// takes kvgMu.
 var kvgMu sync.Mutex
 
 // kvgEnsure creates the context once and (re)loads the pci.ids table when the path changed.
@@ -481,6 +484,82 @@ func revalidateGroupsGPU(devs []string, want []string) (first int, err error) {
 		return -1, nil
 	}
 	return int(bad), nil
+}
+
+// preferredAllocationGPU is GetPreferredAllocation's NUMA packing (generic_device_plugin.go:470-608) for every container
+// request of one PreferredAllocationRequest, in one launch of kvg_preferred_allocation (Python twin: kvgpu/serve.py
+// NumaPacker, tested against serve.preferred_allocation by tests/test_serve_preferred_alloc.py).  devs is the plugin's
+// device list: the last entry with topology gives a device its node, and a node of -1, a device without topology and
+// an ID the plugin does not know share the reference's -1 group (KVG_PREF_NODE_NONE).  Per request the ID strings,
+// must-include first, are interned into handles and the node values into dense indices; the kernel decides, and this
+// function only maps the positions it returns back to IDs.  The error is the reference's text for the first failing
+// request.  It touches no scan state, so it may run while a scan's result is still to be fetched.
+func preferredAllocationGPU(devs []*pluginapi.Device, reqs []*pluginapi.ContainerPreferredAllocationRequest) ([][]string, error) {
+	if len(reqs) == 0 {
+		return nil, nil
+	}
+	nodeOf := map[string]int64{}
+	for _, d := range devs {
+		if d.Topology != nil && len(d.Topology.Nodes) > 0 {
+			nodeOf[d.ID] = d.Topology.Nodes[0].ID
+		}
+	}
+	creqs := make([]C.kvg_pref_req, len(reqs))
+	ids := []C.kvg_pref_id{}
+	entries := make([][]string, len(reqs))
+	for r, req := range reqs {
+		ent := append(append([]string{}, req.MustIncludeDeviceIDs...), req.AvailableDeviceIDs...)
+		handles, nodes := map[string]uint32{}, map[int64]uint32{}
+		for _, id := range ent {
+			h, ok := handles[id]
+			if !ok {
+				h = uint32(len(handles))
+				handles[id] = h
+			}
+			node := uint32(C.KVG_PREF_NODE_NONE)
+			if n, ok := nodeOf[id]; ok && n != -1 {
+				v, ok := nodes[n]
+				if !ok {
+					v = uint32(len(nodes))
+					nodes[n] = v
+				}
+				node = v
+			}
+			ids = append(ids, C.kvg_pref_id{handle: C.uint32_t(h), node: C.uint32_t(node)})
+		}
+		creqs[r] = C.kvg_pref_req{n_must: C.uint32_t(len(req.MustIncludeDeviceIDs)),
+			n_avail: C.uint32_t(len(req.AvailableDeviceIDs)), size: C.int32_t(req.AllocationSize)}
+		entries[r] = ent
+	}
+	res := make([]C.kvg_pref_res, len(reqs))
+	pos := make([]C.uint32_t, len(ids)+1)
+	var idp *C.kvg_pref_id
+	if len(ids) > 0 {
+		idp = &ids[0]
+	}
+	kvgMu.Lock()
+	defer kvgMu.Unlock()
+	if err := kvgEnsure(); err != nil {
+		return nil, err
+	}
+	if rc := C.kvg_preferred_allocation(kvgCtx, &creqs[0], C.uint32_t(len(creqs)), idp, C.size_t(len(ids)), &res[0],
+		&pos[0]); rc != C.KVG_OK {
+		return nil, fmt.Errorf("kvg_preferred_allocation: %s", C.GoString(C.kvg_last_error(kvgCtx)))
+	}
+	out := make([][]string, len(reqs))
+	at := 0
+	for r, ent := range entries {
+		if res[r].n_out < 0 {
+			return nil, fmt.Errorf("number of MustIncludeDeviceIDs (%d) exceeds allocation size (%d)",
+				int(res[r].n_must_distinct), reqs[r].AllocationSize)
+		}
+		out[r] = make([]string, int(res[r].n_out))
+		for k := range out[r] {
+			out[r][k] = ent[pos[at+k]]
+		}
+		at += len(ent)
+	}
+	return out, nil
 }
 
 // revalidateVgpuBatchGPU is the Allocate-time re-check of generic_vgpu_device_plugin.go:216-228 for ALL IDs of an

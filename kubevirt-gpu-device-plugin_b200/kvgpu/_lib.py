@@ -41,8 +41,13 @@ MDEV_CHANGE = np.dtype([("uuid", "u1", (16,)), ("what", "<u4"), ("prev_parent", 
 CH_ADDED, CH_REMOVED, CH_GROUP, CH_DEVICE, CH_NUMA = 1, 2, 4, 8, 16
 CH_TYPE, CH_PARENT = 32, 64
 NO_INDEX = 0xFFFFFFFF
+PREF_ID = np.dtype([("handle", "<u4"), ("node", "<u4")])
+PREF_REQ = np.dtype([("n_must", "<u4"), ("n_avail", "<u4"), ("size", "<i4"), ("pad", "<u4")])
+PREF_RES = np.dtype([("n_out", "<i4"), ("n_must_distinct", "<u4")])
+PREF_NODE_NONE = 0xFFFFFFFF
 assert PCI_REC.itemsize == 16 and PCI_SURV.itemsize == 16 and PCI_CHANGE.itemsize == 32
 assert MDEV_REC.itemsize == 32 and MDEV_SURV.itemsize == 32 and MDEV_CHANGE.itemsize == 48
+assert PREF_ID.itemsize == 8 and PREF_REQ.itemsize == 16 and PREF_RES.itemsize == 8
 
 
 class KvgError(RuntimeError):
@@ -160,6 +165,7 @@ def load() -> C.CDLL:
         "kvg_scan_mdev": (C.c_int, [vp, vp, sz, P(TypeDict), P(P(MdevResultC))]),
         "kvg_mdev_label_match": (C.c_int, [vp, P(TypeDict), vp, sz, vp]),
         "kvg_pci_group_check": (C.c_int, [vp, vp, vp, sz, P(sz)]),
+        "kvg_preferred_allocation": (C.c_int, [vp, vp, u32, vp, sz, vp, vp]),
         "kvg_health_rescan": (C.c_int, [vp, vp, sz, P(P(HealthDeltaC))]),
         "kvg_health_reset": (C.c_int, [vp]),
         "kvg_health_rescan_mdev": (C.c_int, [vp, vp, sz, u32, vp, sz, P(P(HealthDeltaC))]),

@@ -280,6 +280,31 @@ class Context:
                                                C.byref(first)))
         return None if first.value == len(recs) else first.value
 
+    def preferred_allocation(self, ids, n_must, n_avail, sizes) -> list:
+        """GetPreferredAllocation's NUMA packing for every container request of one call, one launch
+        (include/kvgpu.h kvg_preferred_allocation).  ids: PREF_ID entries, request after request, each request's
+        must-include entries first; n_must, n_avail, sizes: one value per request.  Returns (n_out, n_must_distinct,
+        positions) per request: n_out = -1 when the must-include IDs outnumber the size, else the picks as entry
+        positions within the request, in the order the reference appends them."""
+        ids = np.ascontiguousarray(ids, dtype=L.PREF_ID)
+        n_must, n_avail = np.asarray(n_must, dtype=np.int64), np.asarray(n_avail, dtype=np.int64)
+        sizes = np.asarray(sizes, dtype=np.int64)
+        if not (len(n_must) == len(n_avail) == len(sizes)):
+            raise ValueError("preferred_allocation: %d / %d / %d per-request values"
+                             % (len(n_must), len(n_avail), len(sizes)))
+        reqs = np.zeros(len(sizes), dtype=L.PREF_REQ)
+        reqs["n_must"], reqs["n_avail"], reqs["size"] = n_must, n_avail, sizes
+        res = np.zeros(len(reqs), dtype=L.PREF_RES)
+        pos = np.zeros(len(ids), dtype=np.uint32)
+        self._ck(self._lib.kvg_preferred_allocation(self._h, reqs.ctypes.data, len(reqs), ids.ctypes.data, len(ids),
+                                                    res.ctypes.data, pos.ctypes.data))
+        out, at = [], 0
+        for r in range(len(reqs)):
+            n = int(res["n_out"][r])
+            out.append((n, int(res["n_must_distinct"][r]), pos[at:at + max(n, 0)].astype(np.int64)))
+            at += int(n_must[r] + n_avail[r])
+        return out
+
     def _take_health(self, res) -> HealthDelta:
         r = res.contents
         out = HealthDelta(int(r.n_records), int(r.n_alive),

@@ -2,8 +2,8 @@
 
 SURVEY.md 8(f): (1) host glue + a mock kubelet to replay Register -> ListAndWatch -> Allocate,
 (2) Allocate-time re-validation as ONE batched re-scan, (3) a health feed driven by the K6 delta
-kernel, (4) GetPreferredAllocation NUMA packing and EGM path selection (host logic, pinned by the
-reference's own tests).  Function by function this mirrors
+kernel, (4) GetPreferredAllocation NUMA packing (on the GPU through NumaPacker) and EGM path
+selection (host logic), both pinned by the reference's own tests.  Function by function this mirrors
 
     pkg/device_plugin/generic_device_plugin.go       (passthrough plugin)
     pkg/device_plugin/generic_vgpu_device_plugin.go  (vGPU plugin)
@@ -18,7 +18,8 @@ plugin.DiscoveryScan (libkvgpu.so); the passthrough re-validation's group and ve
 Context.pci_group_check (GroupCheck; BatchRevalidator, the same check through Context.scan_pci (K3), is the
 reference it is tested against), the vGPU plugin's label check through Context.mdev_label_match (MdevLabelCheck;
 a vGPU plugin built without a check keeps the reference's CPU rule, the path the GPU check is tested
-against); the health feeds through Context.health_rescan, Context.health_rescan_mdev and
+against), the passthrough plugin's GetPreferredAllocation through Context.preferred_allocation (NumaPacker;
+preferred_allocation below stays the reference it is tested against); the health feeds through Context.health_rescan, Context.health_rescan_mdev and
 Context.health_rescan_groups and their keyed forms (K6); the
 hot-plug feeds through Context.scan_pci_delta and Context.scan_mdev_delta (K7).
 """
@@ -437,19 +438,26 @@ class _PluginBase:
 class GenericDevicePlugin(_PluginBase):
     """The passthrough plugin (generic_device_plugin.go).  `maps` supplies what returnIommuMap /
     returnBdfToIommuMap supply in the reference; `revalidate` is the Allocate-time re-check
-    (GroupCheck, or BatchRevalidator over a scan function)."""
+    (GroupCheck, or BatchRevalidator over a scan function); `prefer` answers GetPreferredAllocation
+    (NumaPacker: every container request in one GPU call; None: preferred_allocation per request on the CPU)."""
 
     def __init__(self, device_name, device_path, devs, maps: Maps, *, revalidate=None,
-                 base_path="/sys/bus/pci/devices", root_path="/", discover_egm=None, **kw):
+                 base_path="/sys/bus/pci/devices", root_path="/", discover_egm=None, prefer=None, **kw):
         super().__init__(device_name, devs, **kw)
         self.device_path, self.maps = device_path, maps
         self.base_path, self.root_path = base_path, root_path
-        self.revalidate = revalidate
+        self.revalidate, self.prefer = revalidate, prefer
         self.discover_egm = discover_egm or (lambda: discover_egm_devices(self.root_path))
 
     def GetPreferredAllocation(self, request, context):
         resp = dpapi.PreferredAllocationResponse()
         devs = [(d.ID, d.topology.nodes[0].ID if len(d.topology.nodes) else None) for d in self.devs]
+        if self.prefer is not None:
+            reqs = [(list(r.available_deviceIDs), list(r.must_include_deviceIDs), int(r.allocation_size))
+                    for r in request.container_requests]
+            for ids in self.prefer(devs, reqs):
+                resp.container_responses.append(dpapi.ContainerPreferredAllocationResponse(deviceIDs=ids))
+            return resp
         for req in request.container_requests:
             ids = preferred_allocation(devs, list(req.available_deviceIDs), list(req.must_include_deviceIDs),
                                        int(req.allocation_size))
@@ -585,6 +593,43 @@ class MdevLabelCheck:
         return out
 
 
+class NumaPacker:
+    """GetPreferredAllocation's NUMA packing (generic_device_plugin.go:470-608) on the GPU: a drop-in `prefer` for
+    GenericDevicePlugin, with preferred_allocation, which stays, as the reference it is tested against.
+
+    `call` is Context.preferred_allocation.  From the plugin's devices it builds ID -> NUMA node, where the last entry
+    with topology wins; a node of -1, a device without topology and an ID the plugin does not know all become
+    PREF_NODE_NONE, the reference's -1.  Per container request the ID strings (must-include first, then available)
+    are interned into handles and the node values into dense indices.  ONE call covers every container request of a
+    PreferredAllocationRequest; the positions it returns map back to the ID strings.  Which device is preferred is
+    decided by the kernel alone."""
+
+    def __init__(self, call):
+        self.call = call
+
+    def __call__(self, devs, requests) -> list:
+        """devs: [(device id, numa node or None)]; requests: [(available, must_include, size)] in request order.
+        Returns the preferred IDs per request, or raises AllocateError with the reference's text for the first
+        request that fails."""
+        node_of = {d: n for d, n in devs if n is not None}
+        ids, n_must, n_avail, sizes, entries = [], [], [], [], []
+        for available, must, size in requests:
+            handles, nodes, ent = {}, {}, list(must) + list(available)
+            for dev_id in ent:
+                node = node_of.get(dev_id, -1)
+                ids.append((handles.setdefault(dev_id, len(handles)),
+                            L.PREF_NODE_NONE if node == -1 else nodes.setdefault(node, len(nodes))))
+            n_must.append(len(must))
+            n_avail.append(len(available))
+            sizes.append(size)
+            entries.append(ent)
+        out = self.call(np.array(ids, dtype=L.PREF_ID), n_must, n_avail, sizes)
+        for (n, p, _), size in zip(out, sizes):
+            if n < 0:
+                raise AllocateError("number of MustIncludeDeviceIDs (%d) exceeds allocation size (%d)" % (p, size))
+        return [[ent[k] for k in pos] for ent, (_, _, pos) in zip(entries, out)]
+
+
 def _read_vgpu_label(base, addr, prop):
     """readVgpuIDFromFileFunc :334-344 for ONE id at Allocate time: trim '\\n', \\s+ -> '_'."""
     import re
@@ -594,9 +639,10 @@ def _read_vgpu_label(base, addr, prop):
     return re.sub(rb"[\t\n\f\r ]+", b"_", raw.strip(b"\n")).decode("latin-1"), False
 
 
-def plugins_from_specs(specs, maps: Maps, revalidate, vgpu_check=None, **kw) -> list:
+def plugins_from_specs(specs, maps: Maps, revalidate, vgpu_check=None, prefer=None, **kw) -> list:
     """createDevicePlugins' server half (device_plugin.go:99-157): one plugin object per spec.  `revalidate` is the
-    passthrough plugins' Allocate-time re-check, `vgpu_check` the vGPU plugins' (None: the CPU rule)."""
+    passthrough plugins' Allocate-time re-check, `vgpu_check` the vGPU plugins' (None: the CPU rule), `prefer` the
+    passthrough plugins' GetPreferredAllocation (None: the CPU rule)."""
     out = []
     for spec in specs:
         devs = devices_from_spec(spec)
@@ -606,7 +652,7 @@ def plugins_from_specs(specs, maps: Maps, revalidate, vgpu_check=None, **kw) -> 
                                                                                           "vgpu_base_path")}))
         else:
             out.append(GenericDevicePlugin(spec.device_name, VFIO_DEVICE_PATH, devs, maps, revalidate=revalidate,
-                                           **{k: v for k, v in kw.items() if k != "vgpu_base_path"}))
+                                           prefer=prefer, **{k: v for k, v in kw.items() if k != "vgpu_base_path"}))
     return out
 
 

@@ -5,6 +5,7 @@
 #define KVG_HOST_EMU 1
 #include "warp_emu.h"
 #include "../../kubevirt-gpu-device-plugin_b200/csrc/kvg_scan.cuh"
+#include "../../kubevirt-gpu-device-plugin_b200/csrc/kvg_alloc.cuh"
 using namespace kvg;
 
 // K6, both forms of every health rule (kvg_scan.cuh) on the caller's state bytes, transitions in record order (a keyed
@@ -231,6 +232,25 @@ int emu_pci_group_check(const uint4* recs, const uint32_t* want, uint32_t n, uin
   if (n == 0) return -1;
   emu_launch(k_pci_group_check, dim3(1), GROUP_CHECK_THREADS, recs, want, n, first_bad_out, seq_out, 7u);
   return 0;
+}
+
+// kvg_preferred_allocation's kernel in its launch shape (min(n_reqs, PREF_MAX_GRID) CTAs of PREF_THREADS): reqs: n_reqs x
+// {n_must, n_avail, size, pad}; ids: n_ids x {handle, node}, the requests' entries one after another.  res_out: n_out,
+// P per request; pos_out: room for n_ids picks, request r's from its first entry; seq_out: the sequence word (7 when
+// done).  The scratch, the CTA counter and the request offsets are the harness's, as the library's are its own.
+int emu_preferred_allocation(const uint4* reqs, uint32_t n_reqs, const uint2* ids, uint32_t n_ids, uint32_t* res_out,
+                             uint32_t* pos_out, uint32_t* seq_out) {
+  if (n_reqs == 0) return -1;
+  std::vector<uint32_t> off(n_reqs);
+  for (uint32_t r = 0, a = 0; r < n_reqs; r++) {
+    off[r] = a;
+    a += reqs[r].x + reqs[r].y;
+  }
+  std::vector<uint32_t> scratch(pref_scratch_words(n_ids, n_reqs), 0xa5a5a5a5u);  // every CTA initialises its slice
+  uint32_t done = 0;
+  emu_launch(k_preferred_alloc, dim3(std::min(n_reqs, PREF_MAX_GRID)), PREF_THREADS, reqs, (const uint32_t*)off.data(),
+             ids, n_reqs, n_ids, scratch.data(), &done, res_out, pos_out, seq_out, 7u);
+  return done == std::min(n_reqs, PREF_MAX_GRID) ? 0 : -2;
 }
 
 }  // extern "C"

@@ -1,17 +1,23 @@
-"""Latency of the Allocate-time re-checks on the GPU: the vGPU plugin's label check (kvg_mdev_label_match) and the
-passthrough plugin's group check (kvg_pci_group_check), beside the passthrough plugin's older re-validation batch
-(kvg_scan_pci, the figure bench.py reports as allocate_revalidation) and the CPU rule of serve._read_vgpu_label, in
-one process.
+"""Latency of the request-path rules on the GPU: the vGPU plugin's label check (kvg_mdev_label_match), the passthrough
+plugin's group check (kvg_pci_group_check) and its GetPreferredAllocation packing (kvg_preferred_allocation), beside
+the passthrough plugin's older re-validation batch (kvg_scan_pci, the figure bench.py reports as
+allocate_revalidation) and the CPU rules of serve._read_vgpu_label and serve.preferred_allocation, in one process.
 
   (a) kvg_mdev_label_match at 1, 2, 4, 8 and 16 files, and at 4 containers x 4 files (one call per AllocateRequest:
       the 16 files of the four containers in request order);
   (b) kvg_scan_pci on a pinned batch of 16 records, as bench.py builds it;
   (c) on the CPU, the rule inside _read_vgpu_label (strip, re.sub, decode, compare) on the same bytes in memory;
   (d) kvg_pci_group_check at 1, 2, 4, 8 and 16 records, as serve.GroupCheck builds them: the group members of (b)
-      with the groups the maps hold for them, one in three with a driver or device id the check must ignore.
+      with the groups the maps hold for them, one in three with a driver or device id the check must ignore;
+  (e) kvg_preferred_allocation on requests as serve.NumaPacker interns them, beside serve.NumaPacker around it
+      (interning, the call, the IDs mapped back) and serve.preferred_allocation, the CPU rule, on the same requests:
+      1 request of 4, 8 and 16 available devices over two NUMA nodes, with 0 and 2 must-include IDs; 4 requests of 8
+      in one call; 1 request of 10,000 and 1 of 100,000 available devices over eight nodes.  The two large legs take
+      min(--calls, 100) timed calls.
 
 Each size: 50 warm-up calls, then the p50 and p99 of the host wall time of 1,000 calls; every result is checked
-against the CPU rule, the group check's against its numpy restatement.  The file contents are those of a live
+against the CPU rule, the group check's against its numpy restatement, the packing's against
+serve.preferred_allocation.  The file contents are those of a live
 mdev_type/name ("GRID A100-4C\\n"), with one in four of another type.  The card's name, power limit and maximum SM
 clock are read with a read-only nvidia-smi query in the same run.
 
@@ -36,6 +42,10 @@ import kvgpu  # noqa: E402
 WARMUP = 50
 NAME = b"GRID_A100-4C"
 GROUP_SIZES = (1, 2, 4, 8, 16)
+# (label, requests, available devices per request, must-include IDs per request, NUMA nodes)
+PREF_LEGS = [("1x4 must0", 1, 4, 0, 2), ("1x4 must2", 1, 4, 2, 2), ("1x8 must0", 1, 8, 0, 2), ("1x8 must2", 1, 8, 2, 2),
+             ("1x16 must0", 1, 16, 0, 2), ("1x16 must2", 1, 16, 2, 2), ("4x8", 4, 8, 0, 2),
+             ("1x10000", 1, 10_000, 2, 8), ("1x100000", 1, 100_000, 2, 8)]
 
 
 def stats(lat):
@@ -66,6 +76,16 @@ def group_rule(recs, want):
     return int(bad[0]) if len(bad) else len(recs)
 
 
+def pref_call(n_reqs, n_avail, n_must, n_nodes):
+    """(devs, requests): n_avail devices spread over n_nodes nodes in runs, each request listing them all in kubelet
+    order; the must-include IDs sit on the last node and the size is half a node's devices plus one, so the packing
+    fills from one node: the must-include node when there is one."""
+    devs = [("0000:%02x:%02x.0" % (i >> 8, i & 0xff), i * n_nodes // n_avail) for i in range(n_avail)]
+    ids = [d for d, _ in devs]
+    reqs = [(ids, ids[n_avail - n_must:], n_avail // n_nodes // 2 + 1) for _ in range(n_reqs)]
+    return devs, reqs
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--calls", type=int, default=1000)
@@ -76,7 +96,8 @@ def main():
     print(card, flush=True)
     lib = kvgpu.load()
     out = {"card": card, "calls": a.calls, "warmup": WARMUP, "what": "host wall time of one call", "label_match": {},
-           "scan_pci_16": None, "cpu_rule": {}, "group_check": {}}
+           "scan_pci_16": None, "cpu_rule": {}, "group_check": {}, "preferred_allocation": {}, "numa_packer": {},
+           "preferred_cpu_rule": {}}
     legs = [("%d" % k, k) for k in (1, 2, 4, 8, 16)] + [("4x4", 16)]
     with kvgpu.Context(0) as ctx:
         with gzip.open(os.path.join(ROOT, "tests", "golden", "pci.ids.gz"), "rb") as f:
@@ -131,6 +152,36 @@ def main():
             bad[k - 1] += 1                                            # the last member's link moved
             assert ctx.pci_group_check(recs, bad) == group_rule(recs, bad) == k - 1
 
+        from kvgpu import serve
+        for label, n_reqs, n_avail, n_must, n_nodes in PREF_LEGS:
+            devs, reqs = pref_call(n_reqs, n_avail, n_must, n_nodes)
+            calls = a.calls if n_avail <= 1000 else min(a.calls, 100)
+            want = [serve.preferred_allocation(devs, av, m, sz) for av, m, sz in reqs]
+            seen = []
+
+            def keep(ids, n_m, n_a, sizes):                         # the arrays NumaPacker builds, for the raw leg
+                seen.append((ids, np.zeros(len(sizes), dtype=kvgpu._lib.PREF_REQ)))
+                seen[-1][1]["n_must"], seen[-1][1]["n_avail"], seen[-1][1]["size"] = n_m, n_a, sizes
+                return ctx.preferred_allocation(ids, n_m, n_a, sizes)
+            packer = serve.NumaPacker(keep)
+            assert packer(devs, reqs) == want
+            ids, rq = seen[0]
+            res = np.zeros(n_reqs, dtype=kvgpu._lib.PREF_RES)
+            pos = np.zeros(len(ids), dtype=np.uint32)
+
+            def gpu():
+                assert lib.kvg_preferred_allocation(ctx.handle, rq.ctypes.data, n_reqs, ids.ctypes.data, len(ids),
+                                                    res.ctypes.data, pos.ctypes.data) == 0
+            before = ctx.launch_count
+            out["preferred_allocation"][label] = timed(gpu, calls)
+            assert ctx.launch_count - before == WARMUP + calls         # one launch per call
+            assert list(res["n_out"]) == [len(w) for w in want]
+            packer = serve.NumaPacker(ctx.preferred_allocation)
+            out["numa_packer"][label] = timed(lambda: packer(devs, reqs), calls)
+            assert packer(devs, reqs) == want
+            out["preferred_cpu_rule"][label] = timed(
+                lambda: [serve.preferred_allocation(devs, av, m, sz) for av, m, sz in reqs], calls)
+
     print("%-28s %10s %10s" % ("call", "p50 us", "p99 us"))
     for label, _ in legs:
         s = out["label_match"][label]
@@ -143,6 +194,11 @@ def main():
     for label, _ in legs:
         s = out["cpu_rule"][label]
         print("%-28s %10.1f %10.1f" % ("CPU rule " + label, s["p50_us"], s["p99_us"]))
+    for key, what in (("preferred_allocation", "kvg_preferred_allocation"), ("numa_packer", "NumaPacker"),
+                      ("preferred_cpu_rule", "CPU preferred_allocation")):
+        for label, *_ in PREF_LEGS:
+            s = out[key][label]
+            print("%-40s %10.1f %10.1f" % ("%s %s" % (what, label), s["p50_us"], s["p99_us"]))
     if a.out:
         os.makedirs(a.out, exist_ok=True)
         with open(os.path.join(a.out, "time_allocate.json"), "w") as f:
