@@ -382,9 +382,40 @@ int kvg_mdev_label_match(kvg_ctx *ctx, const kvg_type_dict *files, const uint8_t
  * own: no scan, fetch, delta, health or name-table state changes, and it does not wait for a pci.ids parse, so it
  * may run between kvg_dev_scan_pci and kvg_dev_scan_pci_fetch.
  * KVG_EINVAL (nothing launched, *first_bad unwritten): ctx or first_bad NULL; recs or want_group NULL with n > 0;
- * n > UINT32_MAX. */
+ * n > UINT32_MAX.  It is kvg_pci_allocate_check with one request and no EGM device. */
 int kvg_pci_group_check(kvg_ctx *ctx, const kvg_pci_rec *recs, const uint32_t *want_group, size_t n,
                         size_t *first_bad);
+/* The passthrough plugin's Allocate decisions (generic_device_plugin.go:352-444) for every container request of one
+ * AllocateRequest, in one launch: the re-check of kvg_pci_group_check and the EGM match of egmPathsForAllocatedGPUs
+ * (:159-184).
+ * Re-check: request r's records are recs / want_group from the end of request r-1's, reqs[r].n_members of them: every
+ * member of every requested group, in the order the reference visits them.  Each is judged by kvg_pci_group_check's
+ * rule.  first_bad[r] = the smallest failing position within the request, or reqs[r].n_members when every member
+ * passes.  Group handles come from one intern table per call, as for kvg_pci_group_check ("042" is not "42").
+ * EGM: intern the EGM devices' GPU strings first, into handles [0, n_egm_gpus), keyed by the reference's normalised
+ * string (strings.ToLower(strings.TrimSpace(s))).  EGM device e lists its handles in egm_gpu[egm_off[e] ..
+ * egm_off[e + 1]).  Request r's reqs[r].n_ids DevicesIDs follow those of requests 0..r-1 in `ids`, each the handle of
+ * its normalised string if some EGM device lists that string, else any value >= n_egm_gpus.
+ * egm_take[r * n_egm + e] = 1 iff every handle of device e is among request r's IDs, else 0; a device with an empty
+ * list is taken, as the reference's loop takes it.  Duplicates on either side do not matter.  The reference mounts
+ * the taken devices' paths, sorted.
+ * One launch per call with n_reqs > 0 (requests with empty lists included), none for n_reqs = 0 or a refused call.
+ * The call uses buffers of its own: no scan, fetch, delta, health or name-table state changes, and it does not wait
+ * for a pci.ids parse.  egm_off (n_egm + 1 entries) may be NULL when n_egm = 0.
+ * KVG_EINVAL (nothing launched, first_bad and egm_take unwritten): ctx NULL; reqs or first_bad NULL with n_reqs > 0;
+ * recs or want_group NULL with n_recs > 0; ids NULL with n_ids > 0; egm_off NULL with n_egm > 0; egm_gpu NULL with a
+ * non-empty list; egm_take NULL with n_reqs * n_egm > 0; member or ID counts that do not add up to n_recs / n_ids;
+ * n_recs or n_ids > UINT32_MAX; egm_off[0] != 0 or decreasing offsets; an egm_gpu value >= n_egm_gpus;
+ * n_egm_gpus > KVG_ALLOC_MAX_EGM_GPUS. */
+#define KVG_ALLOC_MAX_EGM_GPUS 65536 /* distinct EGM GPU strings per call: one bit each in shared memory (8 KiB) */
+typedef struct kvg_alloc_req {
+  uint32_t n_members; /* records of this request: every member of every requested group, in the reference's order */
+  uint32_t n_ids;     /* this request's DevicesIDs, as EGM handles */
+} kvg_alloc_req;
+int kvg_pci_allocate_check(kvg_ctx *ctx, const kvg_alloc_req *reqs, uint32_t n_reqs, const kvg_pci_rec *recs,
+                           const uint32_t *want_group, size_t n_recs, const uint32_t *ids, size_t n_ids,
+                           const uint32_t *egm_off, const uint32_t *egm_gpu, uint32_t n_egm, uint32_t n_egm_gpus,
+                           uint32_t *first_bad, uint8_t *egm_take);
 /* GetPreferredAllocation of the passthrough plugin (generic_device_plugin.go:470-608): the NUMA packing of every
  * container request of one PreferredAllocationRequest, in one launch.
  * Entries: request r's entries follow those of requests 0..r-1 in `ids`, its n_must must-include IDs first, then its

@@ -13,7 +13,8 @@
 //                          (Keyed<Rule>, either form: the prior state joined by UUID / address instead of by index)
 //   k_mdev_labels / _canon K5: label rule (:341-342) + merge of equal labels
 //   k_mdev_label_match     the same label rule against one name: the vGPU plugin's Allocate-time re-check
-//   k_pci_group_check      the passthrough plugin's Allocate-time re-check: group link and vendor per group member
+//   k_pci_allocate_check   the passthrough plugin's Allocate decisions: group link and vendor per group member, and
+//                          the EGM all-GPUs match, for every container request of one call
 //   k_gen_*                counter-based synthetic snapshots (twins of oracle/kvg_oracle.c kvo_gen_*)
 #pragma once
 #include "../../include/kvgpu.h"
@@ -664,31 +665,63 @@ __global__ void __launch_bounds__(LABEL_MATCH_THREADS) k_mdev_label_match(const 
   }
 }
 
-// Allocate-time re-check of the passthrough plugin (generic_device_plugin.go:387-399): the smallest i whose record
-// fails pci_group_check_pass against want[i], or n when every record passes.  One CTA, striding; each thread stops at
-// its first failure (its indices ascend), the warps reduce with one REDUX each and the block through one shared word.
-// The index goes straight to mapped host memory, then the sequence word the host polls.
+// The passthrough plugin's Allocate decisions for every container request of one AllocateRequest
+// (generic_device_plugin.go:352-444): the re-check of each requested group's members (:387-399) and the EGM match
+// (egmPathsForAllocatedGPUs :159-184).  One CTA per request, striding over the requests when there are more than the
+// grid; req[r] = {first member, members, first ID, IDs}.
+//   re-check: first_bad_host[r] = the smallest position within the request whose record fails pci_group_check_pass
+//     against its wanted group, or its member count.  Each thread stops at its first failure (its positions ascend);
+//     the warps reduce with one REDUX each and the block through one shared word.
+//   EGM (n_egm > 0): the request's ID handles below n_egm_gpus set their bits of a shared bitmap; then device e is
+//     taken (take_host[r * n_egm + e] = 1) iff every handle it lists, egm_gpu[egm_off[e] .. egm_off[e + 1]), has its
+//     bit set.  An empty list is taken, as the reference's loop takes it.
+// Results go straight to mapped host memory; the last CTA to finish (done counts them; the host zeroes it) writes the
+// sequence word the host polls.
 static constexpr int GROUP_CHECK_THREADS = 1024;
-__global__ void __launch_bounds__(GROUP_CHECK_THREADS) k_pci_group_check(const uint4* __restrict__ recs,
-                                                                         const uint32_t* __restrict__ want, uint32_t n,
-                                                                         uint32_t* first_bad_host, uint32_t* seq_host,
-                                                                         uint32_t seq) {
+static constexpr uint32_t ALLOC_CHECK_MAX_GRID = 65535;  // more requests than this: each CTA takes several in turn
+__global__ void __launch_bounds__(GROUP_CHECK_THREADS) k_pci_allocate_check(
+    const uint4* __restrict__ req, const uint4* __restrict__ recs, const uint32_t* __restrict__ want,
+    const uint32_t* __restrict__ ids, const uint32_t* __restrict__ egm_off, const uint32_t* __restrict__ egm_gpu,
+    uint32_t n_reqs, uint32_t n_egm, uint32_t n_egm_gpus, uint32_t* done, uint32_t* first_bad_host,
+    uint8_t* take_host, uint32_t* seq_host, uint32_t seq) {
   pdl_enter();
   __shared__ uint32_t block_min;
-  if (threadIdx.x == 0) block_min = n;
-  uint32_t m = n;
-  for (uint32_t i = threadIdx.x; i < n; i += blockDim.x)
-    if (!pci_group_check_pass(recs[i], want[i])) {
-      m = i;
-      break;
+  __shared__ uint32_t present[KVG_ALLOC_MAX_EGM_GPUS / 32];
+  const uint32_t n_words = (n_egm_gpus + 31) / 32;
+  for (uint32_t r = blockIdx.x; r < n_reqs; r += gridDim.x) {
+    const uint4 q = req[r];
+    const uint32_t n = q.y;
+    if (threadIdx.x == 0) block_min = n;
+    if (n_egm)
+      for (uint32_t w = threadIdx.x; w < n_words; w += blockDim.x) present[w] = 0;
+    uint32_t m = n;
+    for (uint32_t i = threadIdx.x; i < n; i += blockDim.x)
+      if (!pci_group_check_pass(recs[q.x + i], want[q.x + i])) {
+        m = i;
+        break;
+      }
+    m = warp_min(m);
+    __syncthreads();  // block_min and the bitmap are initialised
+    if (lane_id() == 0) atomicMin(&block_min, m);
+    if (n_egm)
+      for (uint32_t j = threadIdx.x; j < q.w; j += blockDim.x) {
+        const uint32_t h = ids[q.z + j];
+        if (h < n_egm_gpus) atomicOr(&present[h / 32], 1u << (h % 32));
+      }
+    __syncthreads();
+    if (threadIdx.x == 0) ((volatile uint32_t*)first_bad_host)[r] = block_min;
+    for (uint32_t e = threadIdx.x; e < n_egm; e += blockDim.x) {
+      uint32_t k = egm_off[e];
+      const uint32_t end = egm_off[e + 1];
+      while (k < end && (present[egm_gpu[k] / 32] >> (egm_gpu[k] % 32) & 1u)) k++;
+      ((volatile uint8_t*)take_host)[(size_t)r * n_egm + e] = k == end;
     }
-  m = warp_min(m);
-  __syncthreads();  // block_min is initialised
-  if (lane_id() == 0) atomicMin(&block_min, m);
+    __syncthreads();  // block_min and the bitmap are read before the next request resets them
+  }
+  __threadfence_system();  // this thread's results are on their way before the CTA counts itself done
   __syncthreads();
-  if (threadIdx.x == 0) {
-    *((volatile uint32_t*)first_bad_host) = block_min;
-    __threadfence_system();  // the index is on its way before the sequence word
+  if (threadIdx.x == 0 && atomicAdd(done, 1u) == gridDim.x - 1) {
+    __threadfence_system();
     *((volatile uint32_t*)seq_host) = seq;
   }
 }

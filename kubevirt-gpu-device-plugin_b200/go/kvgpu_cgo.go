@@ -45,7 +45,7 @@ var kvgCtx *C.kvg_ctx
 var kvgLoadedPath string
 
 // A kvg_ctx is single-threaded (include/kvgpu.h).  The scans run on the main goroutine before any server
-// starts, but getDeviceNameGPU, preferredAllocationGPU and the revalidate*GPU functions are reached from gRPC handler
+// starts, but getDeviceNameGPU, preferredAllocationGPU, allocateCheckGPU and the revalidate*GPU functions are reached from gRPC handler
 // goroutines (grpc-go runs one goroutine per stream) and from healthCheck goroutines: every entry into the library
 // takes kvgMu.
 var kvgMu sync.Mutex
@@ -484,6 +484,147 @@ func revalidateGroupsGPU(devs []string, want []string) (first int, err error) {
 		return -1, nil
 	}
 	return int(bad), nil
+}
+
+// allocMember is one member of a requested IOMMU group, as Allocate visits it: its address and the group the maps
+// hold for it.
+type allocMember struct{ addr, group string }
+
+// allocDecision is what allocateCheckGPU decides for one container request.
+type allocDecision struct {
+	bad   int         // position of the first member the reference rejects, or -1
+	panic interface{} // what that member's vendor read panicked with, when the reference reaches the read; else nil
+	egm   []string    // the EGM device paths to mount, sorted (egmPathsForAllocatedGPUs :159-184)
+}
+
+// allocateCheckGPU takes every decision of the passthrough plugin's Allocate (generic_device_plugin.go:352-444) for
+// all container requests of one AllocateRequest in one launch of kvg_pci_allocate_check (Python twin: kvgpu/serve.py
+// AllocateCheck, tested against GroupCheck and the CPU EGM rule by tests/test_serve_allocate_check.py).  It is the
+// twin of revalidateGroupsGPU and egmPathsForAllocatedGPUs together: members[r] lists request r's group members in
+// the reference's order, ids[r] its DevicesIDs.  Every member's link and vendor are read with the reference's
+// readers, request by request; a panicking read is recovered per member and handed back only when the reference
+// would reach it.  The EGM strings are interned with the reference's own strings.ToLower(strings.TrimSpace(s)), so
+// the keys are exactly the ones egmPathsForAllocatedGPUs compares.  The caller replays each request in the
+// reference's order (lookup error, re-check failure or panic, iommufd read, requested device found, EGM specs) and
+// returns the first error of the first failing request.  It touches no scan state.
+func allocateCheckGPU(members [][]allocMember, ids [][]string, egmDevices []EGMDeviceInfo) ([]allocDecision, error) {
+	if len(members) == 0 {
+		return nil, nil
+	}
+	key := func(s string) string { return strings.ToLower(strings.TrimSpace(s)) }
+	egmHandle := map[string]uint32{}
+	egmOff, egmGPU := []C.uint32_t{}, []C.uint32_t{}
+	if len(egmDevices) > 0 {
+		egmOff = append(egmOff, 0)
+	}
+	for _, e := range egmDevices {
+		for _, g := range e.GPUBDFs {
+			h, ok := egmHandle[key(g)]
+			if !ok {
+				h = uint32(len(egmHandle))
+				egmHandle[key(g)] = h
+			}
+			egmGPU = append(egmGPU, C.uint32_t(h))
+		}
+		egmOff = append(egmOff, C.uint32_t(len(egmGPU)))
+	}
+	nEgmGPUs := uint32(len(egmHandle))
+	intern := map[string]uint32{}
+	id := func(s string) uint32 {
+		if v, ok := intern[s]; ok {
+			return v
+		}
+		v := uint32(len(intern))
+		intern[s] = v
+		return v
+	}
+	creqs := make([]C.kvg_alloc_req, len(members))
+	recs, wantGroup, cids := []C.kvg_pci_rec{}, []C.uint32_t{}, []C.uint32_t{}
+	linkOK, panics := []bool{}, map[int]interface{}{}
+	for r, ms := range members {
+		for _, m := range ms {
+			i := len(recs)
+			rec := C.kvg_pci_rec{addr: C.uint32_t(i), vendor: 0xffff}
+			wantGroup = append(wantGroup, C.uint32_t(id(m.group)))
+			group, err := readLink(basePath, m.addr, "iommu_group")
+			ok := false
+			if err != nil {
+				rec.flags |= C.KVG_PF_IOMMU_ERR
+			} else {
+				rec.iommu_group = C.uint32_t(id(group))
+				ok = group == m.group
+			}
+			vendorID, err := func() (v string, err error) {
+				defer func() {
+					if p := recover(); p != nil {
+						panics[i], err = p, fmt.Errorf("panic")
+					}
+				}()
+				return readIDFromFile(basePath, m.addr, "vendor")
+			}()
+			if err != nil {
+				rec.flags |= C.KVG_PF_VENDOR_ERR
+			} else if vendorID == nvidiaVendorID {
+				rec.vendor = 0x10de
+			}
+			recs = append(recs, rec)
+			linkOK = append(linkOK, ok)
+		}
+		for _, d := range ids[r] {
+			h, ok := egmHandle[key(d)]
+			if !ok {
+				h = nEgmGPUs
+			}
+			cids = append(cids, C.uint32_t(h))
+		}
+		creqs[r] = C.kvg_alloc_req{n_members: C.uint32_t(len(ms)), n_ids: C.uint32_t(len(ids[r]))}
+	}
+	firstBad := make([]C.uint32_t, len(members))
+	take := make([]C.uint8_t, len(members)*len(egmDevices)+1)
+	var recp *C.kvg_pci_rec
+	var wantp, idp, offp, gpup *C.uint32_t
+	if len(recs) > 0 {
+		recp, wantp = &recs[0], &wantGroup[0]
+	}
+	if len(cids) > 0 {
+		idp = &cids[0]
+	}
+	if len(egmOff) > 0 {
+		offp = &egmOff[0]
+	}
+	if len(egmGPU) > 0 {
+		gpup = &egmGPU[0]
+	}
+	kvgMu.Lock()
+	defer kvgMu.Unlock()
+	if err := kvgEnsure(); err != nil {
+		return nil, err
+	}
+	if rc := C.kvg_pci_allocate_check(kvgCtx, &creqs[0], C.uint32_t(len(creqs)), recp, wantp, C.size_t(len(recs)), idp,
+		C.size_t(len(cids)), offp, gpup, C.uint32_t(len(egmDevices)), C.uint32_t(nEgmGPUs), &firstBad[0],
+		&take[0]); rc != C.KVG_OK {
+		return nil, fmt.Errorf("kvg_pci_allocate_check: %s", C.GoString(C.kvg_last_error(kvgCtx)))
+	}
+	out := make([]allocDecision, len(members))
+	at := 0
+	for r, ms := range members {
+		d := allocDecision{bad: -1, egm: []string{}}
+		if b := int(firstBad[r]); b < len(ms) {
+			d.bad = b
+			if linkOK[at+b] {
+				d.panic = panics[at+b]
+			}
+		}
+		for e, dev := range egmDevices {
+			if take[r*len(egmDevices)+e] != 0 {
+				d.egm = append(d.egm, dev.DevPath)
+			}
+		}
+		sort.Strings(d.egm)
+		out[r] = d
+		at += len(ms)
+	}
+	return out, nil
 }
 
 // preferredAllocationGPU is GetPreferredAllocation's NUMA packing (generic_device_plugin.go:470-608) for every container

@@ -49,11 +49,11 @@ def main(argv=None) -> int:
             return 0
         from . import dpapi, serve
         sockdir = args.socket_dir or dpapi.DEVICE_PLUGIN_PATH
-        reval = serve.GroupCheck(ds.ctx.pci_group_check, args.base_path)
+        allocate_check = serve.AllocateCheck(ds.ctx.pci_allocate_check, args.base_path)
         vgpu_check = serve.MdevLabelCheck(ds.ctx.mdev_label_match, args.vgpu_base_path)
         prefer = serve.NumaPacker(ds.ctx.preferred_allocation)
-        plugins = serve.plugins_from_specs(specs, ds.maps, reval, vgpu_check=vgpu_check, prefer=prefer,
-                                           socket_dir=sockdir, base_path=args.base_path, root_path=args.root_path,
+        plugins = serve.plugins_from_specs(specs, ds.maps, None, vgpu_check=vgpu_check, prefer=prefer,
+                                           allocate_check=allocate_check, socket_dir=sockdir, base_path=args.base_path, root_path=args.root_path,
                                            vgpu_base_path=args.vgpu_base_path)
         watchers, started = [], []
         for p in plugins:                 # createDevicePlugins :131-137, :158-165: a failed start is logged, the rest go on

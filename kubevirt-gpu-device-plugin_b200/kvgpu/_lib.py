@@ -45,9 +45,11 @@ PREF_ID = np.dtype([("handle", "<u4"), ("node", "<u4")])
 PREF_REQ = np.dtype([("n_must", "<u4"), ("n_avail", "<u4"), ("size", "<i4"), ("pad", "<u4")])
 PREF_RES = np.dtype([("n_out", "<i4"), ("n_must_distinct", "<u4")])
 PREF_NODE_NONE = 0xFFFFFFFF
+ALLOC_REQ = np.dtype([("n_members", "<u4"), ("n_ids", "<u4")])
+ALLOC_MAX_EGM_GPUS = 65536
 assert PCI_REC.itemsize == 16 and PCI_SURV.itemsize == 16 and PCI_CHANGE.itemsize == 32
 assert MDEV_REC.itemsize == 32 and MDEV_SURV.itemsize == 32 and MDEV_CHANGE.itemsize == 48
-assert PREF_ID.itemsize == 8 and PREF_REQ.itemsize == 16 and PREF_RES.itemsize == 8
+assert PREF_ID.itemsize == 8 and PREF_REQ.itemsize == 16 and PREF_RES.itemsize == 8 and ALLOC_REQ.itemsize == 8
 
 
 class KvgError(RuntimeError):
@@ -166,6 +168,7 @@ def load() -> C.CDLL:
         "kvg_mdev_label_match": (C.c_int, [vp, P(TypeDict), vp, sz, vp]),
         "kvg_pci_group_check": (C.c_int, [vp, vp, vp, sz, P(sz)]),
         "kvg_preferred_allocation": (C.c_int, [vp, vp, u32, vp, sz, vp, vp]),
+        "kvg_pci_allocate_check": (C.c_int, [vp, vp, u32, vp, vp, sz, vp, sz, vp, vp, u32, u32, vp, vp]),
         "kvg_health_rescan": (C.c_int, [vp, vp, sz, P(P(HealthDeltaC))]),
         "kvg_health_reset": (C.c_int, [vp]),
         "kvg_health_rescan_mdev": (C.c_int, [vp, vp, sz, u32, vp, sz, P(P(HealthDeltaC))]),

@@ -280,6 +280,33 @@ class Context:
                                                C.byref(first)))
         return None if first.value == len(recs) else first.value
 
+    def pci_allocate_check(self, recs: np.ndarray, want, n_members, ids, n_ids, egm_off, egm_gpu,
+                           n_egm_gpus: int) -> tuple:
+        """The passthrough plugin's Allocate decisions for every container request of one call, one launch
+        (include/kvgpu.h kvg_pci_allocate_check).  recs / want: the members of every request, request after request,
+        as for pci_group_check; ids: the requests' DevicesIDs as EGM handles, request after request; n_members, n_ids:
+        one count per request; egm_off / egm_gpu: each EGM device's GPU handles (egm_off has one entry more than there
+        are devices, or none for no device).  Returns (first_bad, take): first_bad[r] = the first failing position of
+        request r, or n_members[r]; take[r, e] = request r holds every GPU of EGM device e."""
+        recs = np.ascontiguousarray(recs, dtype=L.PCI_REC)
+        want = np.ascontiguousarray(want, dtype=np.uint32)
+        ids = np.ascontiguousarray(ids, dtype=np.uint32)
+        egm_off = np.ascontiguousarray(egm_off, dtype=np.uint32)
+        egm_gpu = np.ascontiguousarray(egm_gpu, dtype=np.uint32)
+        if len(want) != len(recs) or len(n_members) != len(n_ids):
+            raise ValueError("pci_allocate_check: %d records but %d wanted groups, %d / %d per-request counts"
+                             % (len(recs), len(want), len(n_members), len(n_ids)))
+        reqs = np.zeros(len(n_members), dtype=L.ALLOC_REQ)
+        reqs["n_members"], reqs["n_ids"] = n_members, n_ids
+        n_egm = max(len(egm_off) - 1, 0)
+        first_bad = np.zeros(len(reqs), dtype=np.uint32)
+        take = np.zeros((len(reqs), n_egm), dtype=np.uint8)
+        self._ck(self._lib.kvg_pci_allocate_check(
+            self._h, reqs.ctypes.data, len(reqs), recs.ctypes.data, want.ctypes.data, len(recs), ids.ctypes.data,
+            len(ids), egm_off.ctypes.data if len(egm_off) else None, egm_gpu.ctypes.data, n_egm, n_egm_gpus,
+            first_bad.ctypes.data, take.ctypes.data))
+        return first_bad, take.astype(bool)
+
     def preferred_allocation(self, ids, n_must, n_avail, sizes) -> list:
         """GetPreferredAllocation's NUMA packing for every container request of one call, one launch
         (include/kvgpu.h kvg_preferred_allocation).  ids: PREF_ID entries, request after request, each request's

@@ -3,7 +3,7 @@
 SURVEY.md 8(f): (1) host glue + a mock kubelet to replay Register -> ListAndWatch -> Allocate,
 (2) Allocate-time re-validation as ONE batched re-scan, (3) a health feed driven by the K6 delta
 kernel, (4) GetPreferredAllocation NUMA packing (on the GPU through NumaPacker) and EGM path
-selection (host logic), both pinned by the reference's own tests.  Function by function this mirrors
+selection (EGM discovery on the host, the all-GPUs match on the GPU through AllocateCheck), both pinned by the reference's own tests.  Function by function this mirrors
 
     pkg/device_plugin/generic_device_plugin.go       (passthrough plugin)
     pkg/device_plugin/generic_vgpu_device_plugin.go  (vGPU plugin)
@@ -15,8 +15,9 @@ Allocate" is testable end to end in an image without a Go toolchain.
 
 Nothing here computes on the CPU what the scan computes on the GPU: the maps come from
 plugin.DiscoveryScan (libkvgpu.so); the passthrough re-validation's group and vendor rule goes through
-Context.pci_group_check (GroupCheck; BatchRevalidator, the same check through Context.scan_pci (K3), is the
-reference it is tested against), the vGPU plugin's label check through Context.mdev_label_match (MdevLabelCheck;
+Context.pci_allocate_check together with the EGM match, one call per AllocateRequest (AllocateCheck; GroupCheck
+through Context.pci_group_check with the CPU EGM rule, and BatchRevalidator, the same check through
+Context.scan_pci (K3), are the references it is tested against), the vGPU plugin's label check through Context.mdev_label_match (MdevLabelCheck;
 a vGPU plugin built without a check keeps the reference's CPU rule, the path the GPU check is tested
 against), the passthrough plugin's GetPreferredAllocation through Context.preferred_allocation (NumaPacker;
 preferred_allocation below stays the reference it is tested against); the health feeds through Context.health_rescan, Context.health_rescan_mdev and
@@ -151,11 +152,17 @@ def discover_egm_devices(root_path: str = "/") -> list:
     return out
 
 
+def egm_key(bdf: str) -> str:
+    """The string egmPathsForAllocatedGPUs compares (:167, :173): strings.ToLower(strings.TrimSpace(bdf)).  Python's
+    strip() and lower() agree with Go's on ASCII; exotic Unicode input may differ."""
+    return bdf.strip().lower()
+
+
 def egm_paths_for_allocated_gpus(allocated_bdfs, egm_devices) -> list:
     """egmPathsForAllocatedGPUs :159-184: an EGM node is injected only when ALL its GPUs are allocated."""
-    allocated = {b.strip().lower() for b in allocated_bdfs}
+    allocated = {egm_key(b) for b in allocated_bdfs}
     return sorted(e.dev_path for e in (egm_devices or [])
-                  if all(g.strip().lower() in allocated for g in e.gpu_bdfs))
+                  if all(egm_key(g) in allocated for g in e.gpu_bdfs))
 
 
 def supports_iommufd(root_path: str = "/") -> bool:
@@ -285,6 +292,74 @@ class GroupCheck:
         if bad is not None and bad in panics and link_ok[bad]:
             raise panics[bad]
         return bad
+
+
+class AllocateCheck:
+    """The passthrough plugin's Allocate decisions (generic_device_plugin.go:352-444) for every container request of
+    one AllocateRequest in ONE launch: the group re-check of GroupCheck and the EGM match of
+    egm_paths_for_allocated_gpus.  A drop-in `allocate_check` for GenericDevicePlugin; GroupCheck with the CPU EGM
+    rule stays as the reference it is tested against.
+
+    Every member's iommu_group link and vendor are read with the reference's readers, in the reference's order
+    (request by request, BDF by BDF, member by member); a reader panic is caught per member.  The group strings are
+    interned in one table per call, as GroupCheck does.  The EGM devices' GPU strings are interned by egm_key first,
+    and each DevicesID goes as the handle of its key, or as n_egm_gpus when no EGM device lists that key.  `call` is
+    Context.pci_allocate_check; what it returns is mapped back, and nothing is decided here."""
+
+    def __init__(self, call, base_path: str = "/sys/bus/pci/devices", read_link=_read_link, read_id=_read_id):
+        self.call, self.base_path = call, base_path
+        self.read_link, self.read_id = read_link, read_id
+
+    def __call__(self, requests, egm_devices) -> list:
+        """requests: [(pairs, devices_ids)] in request order, where pairs = [(addr, expected iommu group)] in the
+        order the reference would visit them; egm_devices: the discovered EGM devices (None or [] for none).
+        Returns per request (bad, panic, egm_paths): the position of the first member the reference would reject
+        (None: none), the ReferencePanic its vendor read raised if the reference reaches that read (None: no panic),
+        and the dev paths of the EGM devices to mount, sorted."""
+        egm_devices = list(egm_devices or [])
+        egm_handle, egm_off, egm_gpu = {}, [0] if egm_devices else [], []
+        for e in egm_devices:
+            egm_gpu.extend(egm_handle.setdefault(egm_key(g), len(egm_handle)) for g in e.gpu_bdfs)
+            egm_off.append(len(egm_gpu))
+        n_egm_gpus = len(egm_handle)
+        n_pairs = sum(len(pairs) for pairs, _ in requests)
+        recs, want = np.zeros(n_pairs, dtype=L.PCI_REC), np.zeros(n_pairs, dtype=np.uint32)
+        intern, link_ok, panics, ids, n_members, n_ids = {}, [False] * n_pairs, {}, [], [], []
+        i = 0
+        for pairs, devices_ids in requests:
+            for addr, expect in pairs:
+                want[i] = intern.setdefault(expect, len(intern))
+                flags, vendor, group = 0, 0xFFFF, 0
+                got, err = self.read_link(self.base_path, addr, "iommu_group")
+                if err:
+                    flags |= L.PF_IOMMU_ERR
+                else:
+                    group = intern.setdefault(got, len(intern))
+                    link_ok[i] = got == expect
+                try:
+                    v, err = self.read_id(self.base_path, addr, "vendor")
+                except ReferencePanic as e:
+                    panics[i] = e
+                    v, err = "", True
+                if err:
+                    flags |= L.PF_VENDOR_ERR
+                elif v == NVIDIA_VENDOR_ID:
+                    vendor = 0x10de
+                recs[i] = (i, vendor, 0, group, 0, flags, 0)
+                i += 1
+            ids.extend(egm_handle.get(egm_key(b), n_egm_gpus) for b in devices_ids)
+            n_members.append(len(pairs))
+            n_ids.append(len(devices_ids))
+        first_bad, take = self.call(recs, want, n_members, ids, n_ids, egm_off, egm_gpu, n_egm_gpus)
+        out, at = [], 0
+        for r, n in enumerate(n_members):
+            bad = None if int(first_bad[r]) == n else int(first_bad[r])
+            # a panicking read fails its record; the reference reaches it only as the first rejected member, and only
+            # when its link check passed (the vendor is read after it)
+            panic = panics.get(at + bad) if bad is not None and link_ok[at + bad] else None
+            out.append((bad, panic, sorted(e.dev_path for e, t in zip(egm_devices, take[r]) if t)))
+            at += n
+        return out
 
 
 # ------------------------------------------------------------------------------------------------
@@ -438,15 +513,18 @@ class _PluginBase:
 class GenericDevicePlugin(_PluginBase):
     """The passthrough plugin (generic_device_plugin.go).  `maps` supplies what returnIommuMap /
     returnBdfToIommuMap supply in the reference; `revalidate` is the Allocate-time re-check
-    (GroupCheck, or BatchRevalidator over a scan function); `prefer` answers GetPreferredAllocation
+    (GroupCheck, or BatchRevalidator over a scan function); `allocate_check` (AllocateCheck), when set, takes every
+    Allocate decision of an AllocateRequest in one GPU call instead: the re-check and the EGM match of every container
+    request; `prefer` answers GetPreferredAllocation
     (NumaPacker: every container request in one GPU call; None: preferred_allocation per request on the CPU)."""
 
     def __init__(self, device_name, device_path, devs, maps: Maps, *, revalidate=None,
-                 base_path="/sys/bus/pci/devices", root_path="/", discover_egm=None, prefer=None, **kw):
+                 base_path="/sys/bus/pci/devices", root_path="/", discover_egm=None, prefer=None, allocate_check=None,
+                 **kw):
         super().__init__(device_name, devs, **kw)
         self.device_path, self.maps = device_path, maps
         self.base_path, self.root_path = base_path, root_path
-        self.revalidate, self.prefer = revalidate, prefer
+        self.revalidate, self.prefer, self.allocate_check = revalidate, prefer, allocate_check
         self.discover_egm = discover_egm or (lambda: discover_egm_devices(self.root_path))
 
     def GetPreferredAllocation(self, request, context):
@@ -464,10 +542,26 @@ class GenericDevicePlugin(_PluginBase):
             resp.container_responses.append(dpapi.ContainerPreferredAllocationResponse(deviceIDs=ids))
         return resp
 
+    def _plan(self, req):
+        """Map lookups only: the (bdf, group, members) the reference would visit, in order, and the (position, bdf)
+        of a lookup error that stops the request, or None."""
+        iommu_map, bdf_to_iommu = self.maps.iommuMap, self.maps.bdfToIommuMap
+        plan = []
+        for k, bdf in enumerate(req.devices_ids):
+            group = bdf_to_iommu.get(bdf)
+            members = iommu_map.get(group, []) if group is not None else []
+            if group is None or not members:
+                return plan, (k, bdf)
+            plan.append((bdf, group, members))
+        return plan, None
+
     def Allocate(self, request, context):
-        """:352-447.  The sequence of checks, device specs and env values is the reference's; the
-        per-device re-validation of a request is handed to `self.revalidate` as one batch."""
-        if self.revalidate is None:
+        """:352-447.  The sequence of checks, device specs and env values is the reference's.  With
+        `allocate_check`, every container request is planned first and ONE call decides the re-check and the EGM match
+        of them all; each request is then replayed in the reference's order, so the first error of the first failing
+        request wins.  Otherwise the per-device re-validation of each request is handed to `self.revalidate` as one
+        batch, and the EGM match is the CPU rule."""
+        if self.revalidate is None and self.allocate_check is None:
             raise AllocateError("no re-validation function configured (the scan context is required)")
         responses = dpapi.AllocateResponse()
         env_list = {}                       # declared OUTSIDE the request loop in the reference (:361)
@@ -476,7 +570,14 @@ class GenericDevicePlugin(_PluginBase):
             egm_devices = self.discover_egm()
         except Exception:                   # :366-370 a discovery failure only disables EGM mounts
             egm_devices = None
-        for req in request.container_requests:
+        reqs = list(request.container_requests)
+        plans = decided = None
+        if self.allocate_check is not None:
+            plans = [self._plan(req) for req in reqs]
+            decided = iter(self.allocate_check(
+                [([(d.addr, group) for _, group, members in plan for d in members], list(req.devices_ids))
+                 for req, (plan, _) in zip(reqs, plans)], egm_devices))
+        for r, req in enumerate(reqs):
             specs, seen = [], set()
 
             def append_spec(host_path):
@@ -484,23 +585,21 @@ class GenericDevicePlugin(_PluginBase):
                     seen.add(host_path)
                     specs.append(dpapi.DeviceSpec(host_path=host_path, container_path=host_path, permissions="mrw"))
 
-            iommu_map, bdf_to_iommu = self.maps.iommuMap, self.maps.bdfToIommuMap
             # plan: which devices would be visited, in order, and where a lookup error would stop
-            plan, lookup_error_at = [], None
-            for k, bdf in enumerate(req.devices_ids):
-                group = bdf_to_iommu.get(bdf)
-                members = iommu_map.get(group, []) if group is not None else []
-                if group is None or not members:
-                    lookup_error_at = (k, bdf)
-                    break
-                plan.append((bdf, group, members))
-            pairs = [(d.addr, group) for _, group, members in plan for d in members]
-            bad = self.revalidate(pairs)    # ONE batch for the whole container request
+            plan, lookup_error_at = plans[r] if plans is not None else self._plan(req)
+            if decided is not None:
+                bad, panic, egm_paths = next(decided)
+            else:
+                pairs = [(d.addr, group) for _, group, members in plan for d in members]
+                bad, panic = self.revalidate(pairs), None    # ONE batch for the whole container request
+                egm_paths = None
             pos = 0
             for bdf, group, members in plan:   # replay in the reference's order: the FIRST error wins
                 addrs, found = [], False
                 for dev in members:
                     if bad is not None and pos == bad:
+                        if panic is not None:   # the reference's vendor read of this member panics
+                            raise panic
                         raise AllocateError("invalid allocation request: unknown device: %s" % dev.addr)
                     pos += 1
                     addrs.append(dev.addr)
@@ -521,7 +620,9 @@ class GenericDevicePlugin(_PluginBase):
                 env_list.setdefault("%s_%s" % (GPU_PREFIX, self.device_name.upper()), []).extend(addrs)
             if lookup_error_at is not None:
                 raise AllocateError("invalid allocation request: unknown device: %s" % lookup_error_at[1])
-            for path in egm_paths_for_allocated_gpus(list(req.devices_ids), egm_devices):
+            if egm_paths is None:
+                egm_paths = egm_paths_for_allocated_gpus(list(req.devices_ids), egm_devices)
+            for path in egm_paths:
                 append_spec(path)
             responses.container_responses.append(dpapi.ContainerAllocateResponse(
                 envs={k: ",".join(v) for k, v in env_list.items()}, devices=specs))   # buildEnv :100-106
@@ -639,10 +740,11 @@ def _read_vgpu_label(base, addr, prop):
     return re.sub(rb"[\t\n\f\r ]+", b"_", raw.strip(b"\n")).decode("latin-1"), False
 
 
-def plugins_from_specs(specs, maps: Maps, revalidate, vgpu_check=None, prefer=None, **kw) -> list:
+def plugins_from_specs(specs, maps: Maps, revalidate, vgpu_check=None, prefer=None, allocate_check=None, **kw) -> list:
     """createDevicePlugins' server half (device_plugin.go:99-157): one plugin object per spec.  `revalidate` is the
-    passthrough plugins' Allocate-time re-check, `vgpu_check` the vGPU plugins' (None: the CPU rule), `prefer` the
-    passthrough plugins' GetPreferredAllocation (None: the CPU rule)."""
+    passthrough plugins' Allocate-time re-check, `allocate_check` their Allocate decisions in one call per
+    AllocateRequest (AllocateCheck; None: `revalidate` and the CPU EGM rule), `vgpu_check` the vGPU plugins' re-check
+    (None: the CPU rule), `prefer` the passthrough plugins' GetPreferredAllocation (None: the CPU rule)."""
     out = []
     for spec in specs:
         devs = devices_from_spec(spec)
@@ -652,7 +754,8 @@ def plugins_from_specs(specs, maps: Maps, revalidate, vgpu_check=None, prefer=No
                                                                                           "vgpu_base_path")}))
         else:
             out.append(GenericDevicePlugin(spec.device_name, VFIO_DEVICE_PATH, devs, maps, revalidate=revalidate,
-                                           prefer=prefer, **{k: v for k, v in kw.items() if k != "vgpu_base_path"}))
+                                           prefer=prefer, allocate_check=allocate_check,
+                                           **{k: v for k, v in kw.items() if k != "vgpu_base_path"}))
     return out
 
 

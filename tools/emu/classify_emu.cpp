@@ -225,13 +225,34 @@ int emu_mdev_label_match(const uint8_t* raw, const uint32_t* raw_off, uint32_t n
   return 0;
 }
 
-// kvg_pci_group_check's kernel in its launch shape (one CTA of GROUP_CHECK_THREADS): recs: n x 16 B records; want: n
-// group handles.  first_bad_out: the smallest failing index, or n; seq_out: the sequence word (7 when done).
+// kvg_pci_allocate_check's kernel in its launch shape (min(n_reqs, ALLOC_CHECK_MAX_GRID) CTAs of GROUP_CHECK_THREADS):
+// reqs: n_reqs x {n_members, n_ids}; recs / want: the requests' members one after another; ids: their EGM handles;
+// egm_off: n_egm + 1 offsets into egm_gpu.  first_bad_out: n_reqs words; take_out: n_reqs x n_egm bytes; seq_out: the
+// sequence word (7 when done).  The CTA counter and the request offsets are the harness's, as the library's are its own.
+int emu_pci_allocate_check(const uint32_t* reqs, uint32_t n_reqs, const uint4* recs, const uint32_t* want,
+                           const uint32_t* ids, const uint32_t* egm_off, const uint32_t* egm_gpu, uint32_t n_egm,
+                           uint32_t n_egm_gpus, uint32_t* first_bad_out, uint8_t* take_out, uint32_t* seq_out) {
+  if (n_reqs == 0) return -1;
+  std::vector<uint4> req(n_reqs);
+  for (uint32_t r = 0, rec_at = 0, id_at = 0; r < n_reqs; r++) {
+    req[r] = make_uint4(rec_at, reqs[2 * r], id_at, reqs[2 * r + 1]);
+    rec_at += reqs[2 * r];
+    id_at += reqs[2 * r + 1];
+  }
+  uint32_t done = 0;
+  const uint32_t grid = std::min(n_reqs, ALLOC_CHECK_MAX_GRID);
+  emu_launch(k_pci_allocate_check, dim3(grid), GROUP_CHECK_THREADS, (const uint4*)req.data(), recs, want, ids, egm_off,
+             egm_gpu, n_reqs, n_egm, n_egm_gpus, &done, first_bad_out, take_out, seq_out, 7u);
+  return done == grid ? 0 : -2;
+}
+
+// kvg_pci_group_check's launch: k_pci_allocate_check with one request and no EGM device.  recs: n x 16 B records;
+// want: n group handles.  first_bad_out: the smallest failing index, or n; seq_out: the sequence word (7 when done).
 int emu_pci_group_check(const uint4* recs, const uint32_t* want, uint32_t n, uint32_t* first_bad_out,
                         uint32_t* seq_out) {
   if (n == 0) return -1;
-  emu_launch(k_pci_group_check, dim3(1), GROUP_CHECK_THREADS, recs, want, n, first_bad_out, seq_out, 7u);
-  return 0;
+  const uint32_t req[2] = {n, 0};
+  return emu_pci_allocate_check(req, 1, recs, want, nullptr, nullptr, nullptr, 0, 0, first_bad_out, nullptr, seq_out);
 }
 
 // kvg_preferred_allocation's kernel in its launch shape (min(n_reqs, PREF_MAX_GRID) CTAs of PREF_THREADS): reqs: n_reqs x

@@ -167,6 +167,7 @@ static inline uint32_t __byte_perm(uint32_t x, uint32_t y, uint32_t s) {
 }
 
 static inline uint32_t atomicAdd(uint32_t* p, uint32_t v) { return __atomic_fetch_add(p, v, __ATOMIC_SEQ_CST); }
+static inline uint32_t atomicOr(uint32_t* p, uint32_t v) { return __atomic_fetch_or(p, v, __ATOMIC_SEQ_CST); }
 static inline uint32_t atomicExch(uint32_t* p, uint32_t v) { return __atomic_exchange_n(p, v, __ATOMIC_SEQ_CST); }
 static inline uint32_t atomicMax(uint32_t* p, uint32_t v) {
   uint32_t old = __atomic_load_n(p, __ATOMIC_SEQ_CST);

@@ -1,5 +1,6 @@
 """Latency of the request-path rules on the GPU: the vGPU plugin's label check (kvg_mdev_label_match), the passthrough
-plugin's group check (kvg_pci_group_check) and its GetPreferredAllocation packing (kvg_preferred_allocation), beside
+plugin's group check (kvg_pci_group_check), its Allocate decisions (kvg_pci_allocate_check) and its
+GetPreferredAllocation packing (kvg_preferred_allocation), beside
 the passthrough plugin's older re-validation batch (kvg_scan_pci, the figure bench.py reports as
 allocate_revalidation) and the CPU rules of serve._read_vgpu_label and serve.preferred_allocation, in one process.
 
@@ -13,11 +14,16 @@ allocate_revalidation) and the CPU rules of serve._read_vgpu_label and serve.pre
       (interning, the call, the IDs mapped back) and serve.preferred_allocation, the CPU rule, on the same requests:
       1 request of 4, 8 and 16 available devices over two NUMA nodes, with 0 and 2 must-include IDs; 4 requests of 8
       in one call; 1 request of 10,000 and 1 of 100,000 available devices over eight nodes.  The two large legs take
-      min(--calls, 100) timed calls.
+      min(--calls, 100) timed calls;
+  (f) kvg_pci_allocate_check, the group check and the EGM match of every container request in one call, as
+      serve.AllocateCheck builds it: 1 request of 1, 2, 4, 8 and 16 members (the records of (d), one DevicesID per
+      group) with 0, 1 and 2 EGM devices of two GPUs each, whose strings are the request's first DevicesIDs; and 4
+      requests of 4 members in one call, beside what the plugin does without it: four kvg_pci_group_check calls and
+      serve.egm_paths_for_allocated_gpus, the CPU rule, per request.
 
 Each size: 50 warm-up calls, then the p50 and p99 of the host wall time of 1,000 calls; every result is checked
 against the CPU rule, the group check's against its numpy restatement, the packing's against
-serve.preferred_allocation.  The file contents are those of a live
+serve.preferred_allocation, the allocate check's against the group check and the CPU EGM rule.  The file contents are those of a live
 mdev_type/name ("GRID A100-4C\\n"), with one in four of another type.  The card's name, power limit and maximum SM
 clock are read with a read-only nvidia-smi query in the same run.
 
@@ -97,7 +103,7 @@ def main():
     lib = kvgpu.load()
     out = {"card": card, "calls": a.calls, "warmup": WARMUP, "what": "host wall time of one call", "label_match": {},
            "scan_pci_16": None, "cpu_rule": {}, "group_check": {}, "preferred_allocation": {}, "numa_packer": {},
-           "preferred_cpu_rule": {}}
+           "preferred_cpu_rule": {}, "allocate_check": {}, "allocate_check_4x4": None, "group_check_4x4_egm_cpu": None}
     legs = [("%d" % k, k) for k in (1, 2, 4, 8, 16)] + [("4x4", 16)]
     with kvgpu.Context(0) as ctx:
         with gzip.open(os.path.join(ROOT, "tests", "golden", "pci.ids.gz"), "rb") as f:
@@ -182,6 +188,59 @@ def main():
             out["preferred_cpu_rule"][label] = timed(
                 lambda: [serve.preferred_allocation(devs, av, m, sz) for av, m, sz in reqs], calls)
 
+        # (f) the group check and the EGM match of every container request in one call
+        egm_devs = [serve.EGMDeviceInfo("/dev/egm0", ["0000:00:00.0", "0000:00:01.0"]),
+                    serve.EGMDeviceInfo("/dev/egm1", ["0000:00:02.0", "0000:00:03.0"])]
+
+        def alloc_args(n_reqs, k, n_egm):
+            """The arrays AllocateCheck builds for n_reqs requests of k members (the records of (d)) and one DevicesID
+            per group; the IDs are the first GPU strings of the EGM devices, then strings no device lists."""
+            recs = np.concatenate([rr[:k]] * n_reqs)
+            recs["driver"][::3] = kvgpu._lib.DRV_OTHER
+            want = np.ascontiguousarray(recs["iommu_group"], dtype=np.uint32)
+            n_ids = (k + 1) // 2
+            devices_ids = ["0000:00:%02x.0" % i for i in range(n_ids)]
+            handle = {serve.egm_key(g): h for h, g in enumerate(g for e in egm_devs[:n_egm] for g in e.gpu_bdfs)}
+            ids = np.array([handle.get(serve.egm_key(b), len(handle)) for b in devices_ids] * n_reqs, dtype=np.uint32)
+            egm_off = np.array([0, 2, 4][:n_egm + 1] if n_egm else [], dtype=np.uint32)
+            egm_gpu = np.arange(2 * n_egm, dtype=np.uint32)
+            reqs = np.zeros(n_reqs, dtype=kvgpu._lib.ALLOC_REQ)
+            reqs["n_members"], reqs["n_ids"] = k, n_ids
+            return recs, want, reqs, ids, egm_off, egm_gpu, len(handle), devices_ids
+
+        def alloc_leg(n_reqs, k, n_egm):
+            recs, want, reqs, ids, egm_off, egm_gpu, n_egm_gpus, devices_ids = alloc_args(n_reqs, k, n_egm)
+            first = np.zeros(n_reqs, dtype=np.uint32)
+            take = np.zeros(max(n_reqs * n_egm, 1), dtype=np.uint8)
+            expect_take = [p in egm_paths_for(devices_ids, egm_devs[:n_egm]) for p in
+                           [e.dev_path for e in egm_devs[:n_egm]]] * n_reqs
+            args = (ctx.handle, reqs.ctypes.data, n_reqs, recs.ctypes.data, want.ctypes.data, len(recs),
+                    ids.ctypes.data, len(ids), egm_off.ctypes.data if n_egm else None, egm_gpu.ctypes.data, n_egm,
+                    n_egm_gpus, first.ctypes.data, take.ctypes.data)    # the pointers taken once, as a host would
+
+            def gpu():
+                assert lib.kvg_pci_allocate_check(*args) == 0
+            before = ctx.launch_count
+            st = timed(gpu, a.calls)
+            assert ctx.launch_count - before == WARMUP + a.calls      # one launch per call
+            assert first.tolist() == [group_rule(recs[:k], want[:k])] * n_reqs == [k] * n_reqs
+            assert take[:n_reqs * n_egm].astype(bool).tolist() == expect_take
+            return st, recs, want, devices_ids
+        egm_paths_for = serve.egm_paths_for_allocated_gpus
+        for k in GROUP_SIZES:
+            for n_egm in (0, 1, 2):
+                out["allocate_check"]["1x%d egm%d" % (k, n_egm)] = alloc_leg(1, k, n_egm)[0]
+        out["allocate_check_4x4"], recs, want, devices_ids = alloc_leg(4, 4, 2)
+        first = C.c_size_t()
+        ptrs = [(recs[4 * r:].ctypes.data, want[4 * r:].ctypes.data) for r in range(4)]
+
+        def four_group_checks():
+            for rp, wp in ptrs:
+                assert lib.kvg_pci_group_check(ctx.handle, rp, wp, 4, C.byref(first)) == 0
+                assert first.value == 4
+                assert egm_paths_for(devices_ids, egm_devs) == ["/dev/egm0"]
+        out["group_check_4x4_egm_cpu"] = timed(four_group_checks, a.calls)
+
     print("%-28s %10s %10s" % ("call", "p50 us", "p99 us"))
     for label, _ in legs:
         s = out["label_match"][label]
@@ -199,6 +258,11 @@ def main():
         for label, *_ in PREF_LEGS:
             s = out[key][label]
             print("%-40s %10.1f %10.1f" % ("%s %s" % (what, label), s["p50_us"], s["p99_us"]))
+    for label, s in out["allocate_check"].items():
+        print("%-40s %10.1f %10.1f" % ("kvg_pci_allocate_check " + label, s["p50_us"], s["p99_us"]))
+    for label, s in (("kvg_pci_allocate_check 4x4 egm2", out["allocate_check_4x4"]),
+                     ("4 x kvg_pci_group_check + CPU EGM", out["group_check_4x4_egm_cpu"])):
+        print("%-40s %10.1f %10.1f" % (label, s["p50_us"], s["p99_us"]))
     if a.out:
         os.makedirs(a.out, exist_ok=True)
         with open(os.path.join(a.out, "time_allocate.json"), "w") as f:
