@@ -292,15 +292,14 @@ class ShardedScan:
                  p2p_cap: int = 0):
         """broadcast_bytes(b: bytes | None, src=0) -> bytes : collective byte broadcast (NCCL unique id).
         allgather_bytes(b: bytes) -> list[bytes] (rank order) + p2p_cap (PCI records per shard; an mdev
-        record takes two): also set up the peer windows (CUDA IPC over NVLink); on any failure the NCCL
-        path is used."""
+        record takes two): set up the peer windows (CUDA IPC over NVLink) first; only if that fails on any
+        rank is the NCCL communicator created.  Every rank takes the same decision (it follows from the
+        all-gathered status bytes), so libnccl is never loaded when the peer windows work — and ranks that
+        share one GPU, which NCCL refuses, can still exchange."""
         self.ctx, self.rank, self.world = ctx, rank, world
         self._bcast, self._allgather = broadcast_bytes, allgather_bytes
         self.mdev_prev_labels, self.mdev_labels = [], []   # dictionaries of the last fetch_mdev_delta: before, now
         self.mode = "nccl"
-        uid = ctx.comm_unique_id() if rank == 0 else None
-        uid = broadcast_bytes(uid, 0)
-        ctx.comm_init(rank, world, uid)
         if allgather_bytes is not None and p2p_cap > 0:
             try:
                 mine = ctx.comm_p2p_export(rank, world, p2p_cap)
@@ -317,6 +316,10 @@ class ShardedScan:
                 if all(g == b"\1" for g in allgather_bytes(good)):
                     ctx.comm_p2p_enable(True)
                     self.mode = "p2p"
+        if self.mode == "nccl":
+            uid = ctx.comm_unique_id() if rank == 0 else None
+            uid = broadcast_bytes(uid, 0)
+            ctx.comm_init(rank, world, uid)
 
     def scan_device_shard(self, d_recs: int, n_local: int):
         self.ctx.dev_scan_pci_sharded(d_recs, n_local)

@@ -13,7 +13,7 @@ move) and checks every step:
     one rank makes ShardedScan.fetch_mdev_delta reset every rank;
   - the call costs exactly three launches beyond the plain fetch, under stable labels.
 
-Arguments: n_per_rank mode (p2p | nccl)."""
+Arguments: n_per_rank mode (p2p | nccl | one-device: every rank on GPU 0, gloo, peer windows; tests/_one_device.py)."""
 import os
 import sys
 
@@ -26,6 +26,7 @@ import numpy as np
 import torch
 import torch.distributed as dist
 
+import _one_device
 import delta_ref
 import kvgpu
 import mdev_delta_ref
@@ -36,9 +37,13 @@ from test_gpu_mdev_delta import KINDS, NT, snapshot, step
 
 def main():
     n_per_rank, mode = int(sys.argv[1]), sys.argv[2]
-    rank, world, local_rank = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"]), int(os.environ["LOCAL_RANK"])
-    torch.cuda.set_device(local_rank)
-    dist.init_process_group("nccl", device_id=torch.device("cuda", local_rank))
+    one_device = mode == "one-device"
+    if one_device:                     # every rank on GPU 0 over gloo: peer windows only
+        rank, world, local_rank = _one_device.init()
+    else:
+        rank, world, local_rank = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"]), int(os.environ["LOCAL_RANK"])
+        torch.cuda.set_device(local_rank)
+        dist.init_process_group("nccl", device_id=torch.device("cuda", local_rank))
     text = util.pciids_text()
     ids = O.nv_ids(text)
     ctx = kvgpu.Context(local_rank)
@@ -66,10 +71,14 @@ def main():
         dist.all_gather_object(out, obj)
         return out
 
+    if one_device:
+        bcast, allgather = _one_device.broadcast, _one_device.allgather
+
     n = n_per_rank * world
     shard_cap = n_per_rank + n_per_rank // 50 + 64           # room for creates and moving boundaries
     # p2p_cap counts PCI records and an mdev record takes two
-    sh = kvgpu.ShardedScan(ctx, rank, world, bcast, allgather if mode == "p2p" else None, 2 * shard_cap)
+    sh = kvgpu.ShardedScan(ctx, rank, world, bcast, allgather if mode != "nccl" else None, 2 * shard_cap)
+    assert sh.mode == "p2p" or not one_device, "rank %d: no peer windows on one device" % rank
     if mode == "p2p" and sh.mode != "p2p" and rank == 0:
         print("note: peer windows unavailable, fell back to NCCL")
     buf = torch.empty(shard_cap * 32, dtype=torch.uint8, device="cuda")
@@ -87,6 +96,10 @@ def main():
         assert hi - lo <= shard_cap
         buf[:part.nbytes].copy_(torch.from_numpy(part.view(np.uint8).ravel()))
         torch.cuda.synchronize()
+        # the ranks line up before every sharded scan: a rank's exchange waits at most ~10 s for its peers, and the
+        # checks between two scans take longer on the ranks that own more keys (at P = 2 rank 0 owns every vGpuMap
+        # key: the canonical ids of the synthetic dictionary are even)
+        dist.barrier()
         sh.scan_device_mdev_shard(buf.data_ptr(), hi - lo, types)
         return part
 
@@ -147,6 +160,7 @@ def main():
         assert d3.changes.tobytes() == want["changes"].tobytes() and d3.type_gone == want["type_gone"], \
             "kvg_scan_mdev_delta disturbed"
         state["mdev"] = r3
+        dist.barrier()                           # as in scan()
         sh.scan_device_shard(pbuf.data_ptr(), phi - plo)
         pres, pd = sh.fetch_delta()
         pp = state["pci"] if state["pci"] is not None else pres.local[:0]

@@ -2,7 +2,8 @@
 the union of the ranks' parts — every rank holds the keys it owns, with ALL their members — must equal the
 oracle on the unsharded snapshot, byte for byte, for several back-to-back steps (window reuse, acks).
 
-Arguments: n [mode [m_total [table]]]; table "long-names" scans against util.long_name_pciids() with the
+Arguments: n [mode [m_total [table]]]; mode p2p | nccl | one-device (every rank on GPU 0, gloo, peer windows:
+tests/_one_device.py); table "long-names" scans against util.long_name_pciids() with the
 type names of util.long_name_types() (vGPU resource names of up to 60,000 bytes) instead of the shipped
 pci.ids and the synthetic type names."""
 import hashlib
@@ -18,6 +19,7 @@ import numpy as np
 import torch
 import torch.distributed as dist
 
+import _one_device
 import kvgpu
 import util
 from oracle import oracle as O
@@ -28,9 +30,13 @@ def main():
     mode = sys.argv[2] if len(sys.argv) > 2 else "p2p"
     m_total = int(sys.argv[3]) if len(sys.argv) > 3 else max(n // 8, 3)
     long_names = len(sys.argv) > 4 and sys.argv[4] == "long-names"
-    rank, world, local_rank = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"]), int(os.environ["LOCAL_RANK"])
-    torch.cuda.set_device(local_rank)
-    dist.init_process_group("nccl", device_id=torch.device("cuda", local_rank))
+    one_device = mode == "one-device"
+    if one_device:                     # every rank on GPU 0 over gloo: peer windows only
+        rank, world, local_rank = _one_device.init()
+    else:
+        rank, world, local_rank = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"]), int(os.environ["LOCAL_RANK"])
+        torch.cuda.set_device(local_rank)
+        dist.init_process_group("nccl", device_id=torch.device("cuda", local_rank))
     text = util.long_name_pciids() if long_names else util.pciids_text()
     ids = O.nv_ids(text)
     ctx = kvgpu.Context(local_rank)
@@ -56,10 +62,13 @@ def main():
         dist.all_gather(outs, t)
         return [bytes(o.cpu().numpy().tobytes()) for o in outs]
 
+    if one_device:
+        bcast, allgather = _one_device.broadcast, _one_device.allgather
     lo, hi = kvgpu.shard_range(n, rank, world)
     mlo, mhi = kvgpu.shard_range(m_total, rank, world)
     cap = max((n + world - 1) // world + 1, 2 * ((m_total + world - 1) // world + 1))
-    sh = kvgpu.ShardedScan(ctx, rank, world, bcast, allgather if mode == "p2p" else None, cap)
+    sh = kvgpu.ShardedScan(ctx, rank, world, bcast, allgather if mode != "nccl" else None, cap)
+    assert sh.mode == "p2p" or not one_device, "rank %d: no peer windows on one device" % rank
     if mode == "p2p" and sh.mode != "p2p" and rank == 0:
         print("note: peer windows unavailable, fell back to NCCL")
     buf = torch.empty(max(hi - lo, 1) * 16, dtype=torch.uint8, device="cuda")

@@ -12,7 +12,7 @@ of the records per step; the record count changes, so shard boundaries move) and
     one rank makes ShardedScan.fetch_delta reset every rank;
   - the call costs exactly two launches beyond the plain fetch.
 
-Arguments: n_per_rank mode (p2p | nccl)."""
+Arguments: n_per_rank mode (p2p | nccl | one-device: every rank on GPU 0, gloo, peer windows; tests/_one_device.py)."""
 import os
 import sys
 
@@ -25,6 +25,7 @@ import numpy as np
 import torch
 import torch.distributed as dist
 
+import _one_device
 import delta_ref
 import kvgpu
 import util
@@ -34,9 +35,13 @@ from test_gpu_delta import KINDS, snapshot, step
 
 def main():
     n_per_rank, mode = int(sys.argv[1]), sys.argv[2]
-    rank, world, local_rank = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"]), int(os.environ["LOCAL_RANK"])
-    torch.cuda.set_device(local_rank)
-    dist.init_process_group("nccl", device_id=torch.device("cuda", local_rank))
+    one_device = mode == "one-device"
+    if one_device:                     # every rank on GPU 0 over gloo: peer windows only
+        rank, world, local_rank = _one_device.init()
+    else:
+        rank, world, local_rank = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"]), int(os.environ["LOCAL_RANK"])
+        torch.cuda.set_device(local_rank)
+        dist.init_process_group("nccl", device_id=torch.device("cuda", local_rank))
     text = util.pciids_text()
     ids = O.nv_ids(text)
     ctx = kvgpu.Context(local_rank)
@@ -64,9 +69,13 @@ def main():
         dist.all_gather_object(out, obj)
         return out
 
+    if one_device:
+        bcast, allgather = _one_device.broadcast, _one_device.allgather
+
     n = n_per_rank * world
     cap = n_per_rank + n_per_rank // 50 + 64                 # room for hot-adds and moving boundaries
-    sh = kvgpu.ShardedScan(ctx, rank, world, bcast, allgather if mode == "p2p" else None, cap)
+    sh = kvgpu.ShardedScan(ctx, rank, world, bcast, allgather if mode != "nccl" else None, cap)
+    assert sh.mode == "p2p" or not one_device, "rank %d: no peer windows on one device" % rank
     if mode == "p2p" and sh.mode != "p2p" and rank == 0:
         print("note: peer windows unavailable, fell back to NCCL")
     buf = torch.empty(cap * 16, dtype=torch.uint8, device="cuda")
@@ -78,6 +87,9 @@ def main():
         assert hi - lo <= cap
         buf[:part.nbytes].copy_(torch.from_numpy(part.view(np.uint8)))
         torch.cuda.synchronize()
+        # the ranks line up before every sharded scan: a rank's exchange waits at most ~10 s for its peers, and the
+        # checks between two scans take longer on the ranks that own more keys
+        dist.barrier()
         sh.scan_device_shard(buf.data_ptr(), hi - lo)
         return part
 

@@ -2,7 +2,8 @@
 (world = min(GPU count, 8); on a single-GPU box world 1, where the owned lists equal the local list but the exchange
 and both delta kernels still run), over both transports, at 10 k records per rank (classify and send fused in one
 kernel over peer windows) and at 2 Mi + 1000 (standalone send, split classify steps).  tests/_shard_delta_worker.py
-holds the checks.  Every test here needs an H100 (`-m gpu`)."""
+holds the checks; tests/test_gpu_exchange_one_device.py runs it at P > 1 with the ranks sharing one GPU.
+Every test here needs an H100 (`-m gpu`)."""
 import os
 import subprocess
 import sys
