@@ -21,6 +21,9 @@
  *   kvg_health_rescan_*_keyed             <- the same two checks with the state kept per UUID / address, so it
  *                                            survives re-scans that change the device list (the reference never
  *                                            re-scans)
+ *   kvg_scan_pci_raw                      <- createIommuDeviceMap from the raw reads of its walk callback:
+ *                                            readIDFromFileFunc :294-302, readNUMANodeFunc :304-320,
+ *                                            readLinkFunc :323-331, isSupportedVfioDriver :249-252
  *   kvg_scan_pci_delta                    <- (no reference equivalent: the reference never re-scans)
  *   kvg_scan_mdev_delta                   <- (no reference equivalent: createVgpuIDMap runs once)
  *   kvg_comm_*, kvg_scan_pci_sharded      <- (no reference equivalent; BASELINE.json config 4)
@@ -57,7 +60,8 @@ enum {
   KVG_ENOMEM = -3, /* host or device allocation failed */
   KVG_ENCCL = -4,  /* NCCL not loadable or a collective failed */
   KVG_ESTATE = -5, /* call order (e.g. scan before kvg_pciids_load) */
-  KVG_ERANGE = -6  /* output buffer too small / value does not fit the wire format */
+  KVG_ERANGE = -6, /* output buffer too small / value does not fit the wire format */
+  KVG_EPANIC = -7  /* the Go reference would panic on this input (kvg_scan_pci_raw) */
 };
 
 /* ---- wire format ---------------------------------------------------------------------------- */
@@ -359,6 +363,65 @@ int kvg_scan_pci(kvg_ctx *ctx, const kvg_pci_rec *recs, size_t n, kvg_pci_result
  *  chunk by chunk on separate copy streams; results are identical.  KVG_PIPELINE=0 disables.) */
 int kvg_scan_mdev(kvg_ctx *ctx, const kvg_mdev_rec *recs, size_t n, const kvg_type_dict *types,
                   kvg_mdev_result **res);
+/* The reads of createIommuDeviceMap's walk callback (device_plugin.go:191-246), raw, one entry per visited
+ * non-directory Walk entry in Walk order, decoded on the GPU into the records above, then scanned as kvg_scan_pci
+ * scans them.  Field f of entry i is bytes[off[i*KVG_RAW_FIELDS + f] .. off[i*KVG_RAW_FIELDS + f + 1]): the entry
+ * name, the vendor, device and numa_node file contents as os.ReadFile returned them, and the driver and iommu_group
+ * link TARGETS as os.Readlink returned them.  state[i] bit f: read f was made; bit 8 + f: it failed (the bits of
+ * KVG_RAW_NAME are unused).  A read the reference does not reach may be skipped or made: the answer is the same. */
+enum { KVG_RAW_NAME, KVG_RAW_VENDOR, KVG_RAW_DRIVER, KVG_RAW_GROUP, KVG_RAW_NUMA, KVG_RAW_DEVICE, KVG_RAW_FIELDS };
+typedef struct kvg_pci_raw {
+  size_t n;
+  const uint32_t *off;   /* [n * KVG_RAW_FIELDS + 1], off[0] == 0, non-decreasing */
+  const uint8_t *bytes;  /* [off[n * KVG_RAW_FIELDS]] */
+  const uint16_t *state; /* [n] */
+} kvg_pci_raw;
+
+/* The snapshot kvg_scan_pci_raw decoded (library-owned; kvg_result_free).  recs are what the host snapshotter packs:
+ *   packed_addr     1: addr is the packed BDF (every name is a canonical "dddd:bb:dd.f" and they ascend strictly);
+ *                   0: addr is the Walk index
+ *   groups_numeric  1: iommu_group is the link basename as a number (every non-empty basename reached is a canonical
+ *                   decimal below 2^32); 0: the handle of the basename, handles in order of first appearance from 0
+ *                   (an entry without a group also holds 0); group h = group_bytes[group_off[h] .. group_off[h + 1])
+ *   devices_numeric 1: device is the id as a number (every device string read is four lower-case hex digits);
+ *                   0: the handle of the string, as for groups (at most 65,536); device names are then asked per key
+ *                   through kvg_name_lookup, the result's name join is keyed by the handle and does not apply. */
+typedef struct kvg_pci_snap {
+  uint64_t n_records;
+  const kvg_pci_rec *recs;
+  uint8_t packed_addr, groups_numeric, devices_numeric;
+  uint32_t n_group_names;
+  const uint32_t *group_off; /* [n_group_names + 1] */
+  const uint8_t *group_bytes;
+  uint32_t n_device_names;
+  const uint32_t *device_off; /* [n_device_names + 1] */
+  const uint8_t *device_bytes;
+} kvg_pci_snap;
+
+/* Decode `raw` on the GPU with the reference's rules, in its short-circuit order (device_plugin.go:202-238):
+ *   vendor       data[2:], Trim "\n" (:294-302); four lower-case hex digits give the number, anything else 0xffff;
+ *                the rest is read only for "10de" (:209)
+ *   driver       the link basename (:323-331), then the dictionary of isSupportedVfioDriver (:249-252)
+ *   iommu_group  the link basename (:221-225)
+ *   numa_node    strings.TrimSpace over UTF-8 (unicode.IsSpace; an invalid byte is not a space), then
+ *                strconv.ParseInt(s, 10, 64); an error sets KVG_PF_NUMA_ERR (:226-230, :304-320); the value stays raw
+ *   device       data[2:], Trim "\n" (:234-238)
+ * choose the snapshot modes (kvg_pci_snap), intern the columns in index mode, pack the records into the context's
+ * record staging and scan them as kvg_scan_pci does: *res equals kvg_scan_pci(ctx, (*snap)->recs, n).  The call writes
+ * the scan state kvg_scan_pci writes and nothing else (delta, health and allocation state are untouched).
+ * Launches: one decode; per column in index mode one probe and one compaction; one pack unless every column is
+ * numeric; then the scan's.  The host waits for the decode (one synchronisation) and, in index mode, for the intern.
+ * Errors (neither writes *res or *snap):
+ *   KVG_EINVAL  nothing launched: ctx, raw, res or snap NULL; off or state NULL with n > 0; bytes NULL with bytes to
+ *               read; off[0] != 0 or decreasing offsets; n above 0xfffffff0 (the scan's bound).  Found by the decode:
+ *               a read the reference reaches was not made (kvg_last_error names the lowest entry and the file).
+ *   KVG_EPANIC  the reference would panic: data[2:] of a vendor or device file shorter than 2 bytes that it reaches;
+ *               kvg_last_error names the lowest such entry and the file.  Beats KVG_ERANGE.
+ *   KVG_ERANGE  a reached numa_node that parses but does not fit int16, or more than 65,536 distinct device strings
+ *               in index mode (the lowest entry is named).
+ *   KVG_ESTATE  before kvg_pciids_load, as kvg_scan_pci; a pending parse is handled as there.
+ * n = 0: an empty result and snapshot, nothing launched and no scan state changed. */
+int kvg_scan_pci_raw(kvg_ctx *ctx, const kvg_pci_raw *raw, kvg_pci_result **res, kvg_pci_snap **snap);
 /* Allocate-time re-check of the vGPU plugin (generic_vgpu_device_plugin.go:216-221): match[i] = 1 iff the label of
  * file i -- Trim(raw, "\n") then every RE2 \s+ run ([\t\n\f\r ]) -> "_" (device_plugin.go:341-342) -- equals the
  * name_len bytes at `name`, else 0.  `files` uses the layout of kvg_type_dict, one entry per file that WAS read; a

@@ -33,6 +33,7 @@
 #include "kvg_shard.cuh"
 #include "kvg_delta.cuh"
 #include "kvg_alloc.cuh"
+#include "kvg_snap.cuh"
 
 using namespace kvg;
 
@@ -40,6 +41,7 @@ using namespace kvg;
 #include "api/kvg_api_core.inc"
 #include "api/kvg_api_pciids.inc"
 #include "api/kvg_api_scan.inc"
+#include "api/kvg_api_snap.inc"
 #include "api/kvg_api_health.inc"
 #include "api/kvg_api_delta.inc"
 #include "api/kvg_api_mdev.inc"

@@ -244,6 +244,134 @@ func createIommuDeviceMapGPU() {
 	}
 }
 
+// createIommuDeviceMapRawGPU: createIommuDeviceMap (:187-247) with every reader's rule on the GPU.  The walk makes the
+// five reads of every entry and decodes nothing; kvg_scan_pci_raw applies readIDFromFileFunc, readLinkFunc,
+// readNUMANodeFunc and isSupportedVfioDriver in the reference's order, chooses the snapshot modes and scans.
+func createIommuDeviceMapRawGPU() {
+	kvgMu.Lock()
+	defer kvgMu.Unlock()
+	iommuMap = make(map[string][]NvidiaGpuDevice)
+	deviceMap = make(map[string][]NvidiaGpuDevice)
+	bdfToIommuMap = make(map[string]string)
+	var names []string
+	var bytes []byte
+	off := []uint32{0}
+	var state []uint16
+	filepath.Walk(basePath, func(path string, info os.FileInfo, err error) error {
+		if err != nil {
+			log.Printf("Error accessing file path %q: %v\n", path, err)
+			return err
+		}
+		if info.IsDir() {
+			return nil
+		}
+		name := info.Name()
+		var st uint16
+		bytes = append(bytes, name...)
+		off = append(off, uint32(len(bytes)))
+		for f, prop := range []string{"vendor", "driver", "iommu_group", "numa_node", "device"} {
+			p := filepath.Join(basePath, name, prop)
+			var data []byte
+			var err error
+			if prop == "driver" || prop == "iommu_group" {
+				var t string
+				t, err = os.Readlink(p)
+				data = []byte(t)
+			} else {
+				data, err = os.ReadFile(p)
+			}
+			st |= 1 << (f + 1)
+			if err != nil {
+				st |= 1 << (8 + f + 1)
+				data = nil
+			}
+			bytes = append(bytes, data...)
+			off = append(off, uint32(len(bytes)))
+		}
+		names = append(names, name)
+		state = append(state, st)
+		return nil
+	})
+	if err := kvgEnsure(); err != nil {
+		log.Printf("Error: %v", err) // maps stay empty, like a failed walk (:193-196)
+		return
+	}
+	// the library copies the inputs before it returns (cgo pointer rule): C copies of them
+	var raw C.kvg_pci_raw
+	raw.n = C.size_t(len(state))
+	if len(state) > 0 {
+		raw.off = (*C.uint32_t)(C.CBytes(unsafe.Slice((*byte)(unsafe.Pointer(&off[0])), 4*len(off))))
+		raw.state = (*C.uint16_t)(C.CBytes(unsafe.Slice((*byte)(unsafe.Pointer(&state[0])), 2*len(state))))
+		raw.bytes = (*C.uint8_t)(C.CBytes(append(bytes, 0)))
+		defer C.free(unsafe.Pointer(raw.off))
+		defer C.free(unsafe.Pointer(raw.state))
+		defer C.free(unsafe.Pointer(raw.bytes))
+	}
+	var res *C.kvg_pci_result
+	var snap *C.kvg_pci_snap
+	if rc := C.kvg_scan_pci_raw(kvgCtx, &raw, &res, &snap); rc != C.KVG_OK {
+		// KVG_EPANIC: the reference would panic here; the maps stay empty
+		log.Printf("Error: kvg_scan_pci_raw: %s", C.GoString(C.kvg_last_error(kvgCtx)))
+		return
+	}
+	defer C.kvg_result_free(unsafe.Pointer(res))
+	defer C.kvg_result_free(unsafe.Pointer(snap))
+	table := func(n C.uint32_t, o *C.uint32_t, b *C.uint8_t) []string {
+		if n == 0 {
+			return nil
+		}
+		offs := unsafe.Slice(o, int(n)+1)
+		all := C.GoBytes(unsafe.Pointer(b), C.int(offs[n]))
+		out := make([]string, int(n))
+		for h := range out {
+			out[h] = string(all[offs[h]:offs[h+1]])
+		}
+		return out
+	}
+	groupNames := table(snap.n_group_names, snap.group_off, snap.group_bytes)
+	deviceNames := table(snap.n_device_names, snap.device_off, snap.device_bytes)
+	S := int(res.n_survivors)
+	surv := unsafe.Slice(res.survivors, S)
+	addr := func(i uint32) string {
+		a := uint32(surv[i].addr)
+		if snap.packed_addr == 0 {
+			return names[a]
+		}
+		return fmt.Sprintf("%04x:%02x:%02x.%x", a>>16, (a>>8)&0xff, (a>>3)&0x1f, a&7)
+	}
+	group := func(g C.uint32_t) string {
+		if snap.groups_numeric != 0 {
+			return strconv.FormatUint(uint64(g), 10)
+		}
+		return groupNames[g]
+	}
+	dev := func(i uint32) NvidiaGpuDevice { return NvidiaGpuDevice{addr: addr(i), numaNode: int64(surv[i].numa)} }
+	devKeys := unsafe.Slice(res.dev_keys, int(res.n_dev_keys))
+	devOff := unsafe.Slice(res.dev_off, int(res.n_dev_keys)+1)
+	devPerm := unsafe.Slice(res.dev_perm, S)
+	for k := range devKeys {
+		key := fmt.Sprintf("%04x", uint16(devKeys[k]))
+		if snap.devices_numeric == 0 {
+			key = deviceNames[devKeys[k]] // getDeviceName(key) is asked later with these exact bytes
+		}
+		for _, i := range devPerm[devOff[k]:devOff[k+1]] {
+			deviceMap[key] = append(deviceMap[key], dev(uint32(i)))
+		}
+	}
+	grpKeys := unsafe.Slice(res.grp_keys, int(res.n_groups))
+	grpOff := unsafe.Slice(res.grp_off, int(res.n_groups)+1)
+	grpPerm := unsafe.Slice(res.grp_perm, S)
+	for k := range grpKeys {
+		g := group(grpKeys[k])
+		for _, i := range grpPerm[grpOff[k]:grpOff[k+1]] {
+			iommuMap[g] = append(iommuMap[g], dev(uint32(i)))
+		}
+	}
+	for i := 0; i < S; i++ {
+		bdfToIommuMap[addr(uint32(i))] = group(surv[i].iommu_group)
+	}
+}
+
 // createVgpuIDMapGPU: :259-290 with the label rule (:341-342) and both group-bys on the GPU.
 func createVgpuIDMapGPU() {
 	kvgMu.Lock()

@@ -16,9 +16,11 @@ LIB_PATH = os.path.join(_PKG, "libkvgpu.so")
 HEADER_PATH = os.path.join(os.path.dirname(_PKG), "include", "kvgpu.h")
 
 KVG_OK, KVG_EINVAL, KVG_ECUDA, KVG_ENOMEM, KVG_ENCCL, KVG_ESTATE, KVG_ERANGE = 0, -1, -2, -3, -4, -5, -6
+KVG_EPANIC = -7
+RAW_NAME, RAW_VENDOR, RAW_DRIVER, RAW_GROUP, RAW_NUMA, RAW_DEVICE, RAW_FIELDS = range(7)
 KVG_NO_NAME = 0xFFFFFFFF
 ERR_NAMES = {0: "KVG_OK", -1: "KVG_EINVAL", -2: "KVG_ECUDA", -3: "KVG_ENOMEM", -4: "KVG_ENCCL",
-             -5: "KVG_ESTATE", -6: "KVG_ERANGE"}
+             -5: "KVG_ESTATE", -6: "KVG_ERANGE", -7: "KVG_EPANIC"}
 
 DRV_NONE, DRV_VFIO_PCI, DRV_NVGRACE, DRV_OTHER = 0, 1, 2, 3
 PF_VENDOR_ERR, PF_DRIVER_ERR, PF_IOMMU_ERR, PF_DEVICE_ERR, PF_NUMA_ERR = 1, 2, 4, 8, 16
@@ -71,6 +73,17 @@ class PciResultC(C.Structure):
                 ("n_groups", C.c_uint32), ("grp_keys", C.c_void_p), ("grp_off", C.c_void_p),
                 ("grp_perm", C.c_void_p),
                 ("name_pool", C.c_void_p), ("name_pool_len", C.c_size_t)]
+
+
+class PciRawC(C.Structure):
+    _fields_ = [("n", C.c_size_t), ("off", C.c_void_p), ("bytes", C.c_void_p), ("state", C.c_void_p)]
+
+
+class PciSnapC(C.Structure):
+    _fields_ = [("n_records", C.c_uint64), ("recs", C.c_void_p),
+                ("packed_addr", C.c_uint8), ("groups_numeric", C.c_uint8), ("devices_numeric", C.c_uint8),
+                ("n_group_names", C.c_uint32), ("group_off", C.c_void_p), ("group_bytes", C.c_void_p),
+                ("n_device_names", C.c_uint32), ("device_off", C.c_void_p), ("device_bytes", C.c_void_p)]
 
 
 class MdevResultC(C.Structure):
@@ -164,6 +177,7 @@ def load() -> C.CDLL:
         "kvg_name_table": (C.c_int, [vp, u32, u32, vp, vp, sz]),
         "kvg_pciids_info": (C.c_int, [vp, P(u32), P(u32), P(u32), P(u32)]),
         "kvg_scan_pci": (C.c_int, [vp, vp, sz, P(P(PciResultC))]),
+        "kvg_scan_pci_raw": (C.c_int, [vp, P(PciRawC), P(P(PciResultC)), P(P(PciSnapC))]),
         "kvg_scan_mdev": (C.c_int, [vp, vp, sz, P(TypeDict), P(P(MdevResultC))]),
         "kvg_mdev_label_match": (C.c_int, [vp, P(TypeDict), vp, sz, vp]),
         "kvg_pci_group_check": (C.c_int, [vp, vp, vp, sz, P(sz)]),

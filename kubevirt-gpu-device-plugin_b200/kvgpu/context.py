@@ -213,6 +213,33 @@ class Context:
         self._ck(self._lib.kvg_scan_pci(self._h, recs.ctypes.data, len(recs), C.byref(res)))
         return self._take_pci(res)
 
+    def scan_pci_raw(self, raw):
+        """createIommuDeviceMap from the raw reads of its walk (plugin.read_pci_tree_raw): the GPU decodes them into the
+        snapshot snapshot_pci_tree packs, then scans it -> (PciResult, PciSnapshot).  Raises plugin.ReferencePanic
+        where the Go reference would panic."""
+        from .plugin import PciSnapshot, ReferencePanic
+        off = np.ascontiguousarray(raw.off, dtype=np.uint32)
+        state = np.ascontiguousarray(raw.state, dtype=np.uint16)
+        blob = np.frombuffer(bytes(raw.bytes) + b"\0", dtype=np.uint8)
+        arg = L.PciRawC(len(state), off.ctypes.data, blob.ctypes.data, state.ctypes.data)
+        res, snap = C.POINTER(L.PciResultC)(), C.POINTER(L.PciSnapC)()
+        rc = self._lib.kvg_scan_pci_raw(self._h, C.byref(arg), C.byref(res), C.byref(snap))
+        if rc == L.KVG_EPANIC:
+            raise ReferencePanic((self._lib.kvg_last_error(self._h) or b"").decode("latin-1"))
+        self._ck(rc)
+        sn = snap.contents
+
+        def table(n, off_p, bytes_p):
+            o = L._arr(off_p, int(n) + 1, np.uint32)
+            b = C.string_at(bytes_p, int(o[-1])) if o[-1] else b""
+            return [b[o[k]:o[k + 1]].decode("latin-1") for k in range(int(n))]
+
+        out = PciSnapshot(L._arr(sn.recs, int(sn.n_records), L.PCI_REC), list(raw.names), bool(sn.packed_addr),
+                          None if sn.groups_numeric else table(sn.n_group_names, sn.group_off, sn.group_bytes),
+                          None if sn.devices_numeric else table(sn.n_device_names, sn.device_off, sn.device_bytes))
+        self._lib.kvg_result_free(snap)
+        return self._take_pci(res), out
+
     @staticmethod
     def _type_dict(raw_types):
         off = np.zeros(len(raw_types) + 1, dtype=np.uint32)

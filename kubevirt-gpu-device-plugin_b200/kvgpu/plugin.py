@@ -245,6 +245,51 @@ def snapshot_pci_tree(base_path: str) -> PciSnapshot:
     return PciSnapshot(recs, names, packed_ok, group_names, device_names)
 
 
+@dataclass
+class PciRaw:
+    """What the readers of createIommuDeviceMap's walk callback got, undecoded (include/kvgpu.h kvg_pci_raw): field f of
+    entry i is bytes[off[i * RAW_FIELDS + f]:off[i * RAW_FIELDS + f + 1]]; state[i] bit f: read f was made, bit 8 + f:
+    it failed.  names: the Walk-order entry names."""
+    names: list
+    off: np.ndarray     # u32 [n * RAW_FIELDS + 1]
+    bytes: bytes
+    state: np.ndarray   # u16 [n]
+
+
+def read_pci_tree_raw(base_path: str) -> PciRaw:
+    """The walk of snapshot_pci_tree with all five reads made for every entry and nothing decoded: file contents as
+    read, link targets as os.readlink returns them.  Reading what the reference would not reach is allowed: the GPU
+    decodes only what it reaches, so no panic is raised here."""
+    names, parts, state = [], [], []
+    bbase = os.fsencode(base_path)
+    for name, is_dir, err in _walk(base_path):
+        if err:
+            break
+        if is_dir:
+            continue
+        bname = os.fsencode(name)
+        st, row = 0, [bname]
+        for f, prop in ((L.RAW_VENDOR, b"vendor"), (L.RAW_DRIVER, b"driver"), (L.RAW_GROUP, b"iommu_group"),
+                        (L.RAW_NUMA, b"numa_node"), (L.RAW_DEVICE, b"device")):
+            path = os.path.join(bbase, bname, prop)
+            try:
+                data = os.readlink(path) if f in (L.RAW_DRIVER, L.RAW_GROUP) else open(path, "rb").read()
+            except OSError:
+                data, st = b"", st | (1 << (8 + f))
+            st |= 1 << f
+            row.append(data)
+        names.append(name)
+        parts.append(row)
+        state.append(st)
+    lens = np.array([len(x) for row in parts for x in row], dtype=np.int64)
+    off = np.zeros(len(lens) + 1, dtype=np.int64)
+    np.cumsum(lens, out=off[1:])
+    if off[-1] > 0xFFFFFFFF:
+        raise ValueError("the raw reads of %s exceed 4 GiB" % base_path)
+    return PciRaw(names, off.astype(np.uint32), b"".join(x for row in parts for x in row),
+                  np.array(state, dtype=np.uint16))
+
+
 def snapshot_pci_ids(base_path: str, bdfs, intern: dict) -> PciSnapshot:
     """Snapshot the PCI devices `bdfs` in THAT order (the health re-scan's fixed record order; a Walk would re-index
     when one vanishes), with the readers and flag rules of snapshot_pci_tree.  An address whose entry is gone reads as
@@ -701,8 +746,13 @@ class DiscoveryScan:
         self._ensure_table()
         return self.ctx.name_lookup(device_id)
 
-    def create_iommu_device_map(self) -> Maps:
+    def create_iommu_device_map(self, raw: bool = False) -> Maps:
+        """raw=True: the walk reads everything and the GPU decodes the reads (Context.scan_pci_raw); the Maps are the
+        same."""
         self._ensure_table()
+        if raw:
+            res, snap = self.ctx.scan_pci_raw(read_pci_tree_raw(self.basePath))
+            return pci_maps_from_result(res, snap, self.maps, name_of=self.ctx.name_lookup)
         try:
             snap = snapshot_pci_tree(self.basePath)
         except ReferencePanic:
