@@ -24,7 +24,10 @@
  *   kvg_scan_pci_raw                      <- createIommuDeviceMap from the raw reads of its walk callback:
  *                                            readIDFromFileFunc :294-302, readNUMANodeFunc :304-320,
  *                                            readLinkFunc :323-331, isSupportedVfioDriver :249-252
- *   kvg_scan_pci_delta                    <- (no reference equivalent: the reference never re-scans)
+ *   kvg_scan_mdev_raw                     <- createVgpuIDMap from the raw reads of its walk callback:
+ *                                            readVgpuIDFromFileFunc :334-344, readGpuIDForVgpuFunc :347-357,
+ *                                            readNUMANodeFunc :304-320
+ *   kvg_scan_pci_delta                   <- (no reference equivalent: the reference never re-scans)
  *   kvg_scan_mdev_delta                   <- (no reference equivalent: createVgpuIDMap runs once)
  *   kvg_comm_*, kvg_scan_pci_sharded      <- (no reference equivalent; BASELINE.json config 4)
  *   kvg_dev_scan_pci_shard_fetch_delta    <- (no reference equivalent: the re-scan delta of the sharded scan)
@@ -61,7 +64,7 @@ enum {
   KVG_ENCCL = -4,  /* NCCL not loadable or a collective failed */
   KVG_ESTATE = -5, /* call order (e.g. scan before kvg_pciids_load) */
   KVG_ERANGE = -6, /* output buffer too small / value does not fit the wire format */
-  KVG_EPANIC = -7  /* the Go reference would panic on this input (kvg_scan_pci_raw) */
+  KVG_EPANIC = -7  /* the Go reference would panic on this input (kvg_scan_pci_raw, kvg_scan_mdev_raw) */
 };
 
 /* ---- wire format ---------------------------------------------------------------------------- */
@@ -422,6 +425,69 @@ typedef struct kvg_pci_snap {
  *   KVG_ESTATE  before kvg_pciids_load, as kvg_scan_pci; a pending parse is handled as there.
  * n = 0: an empty result and snapshot, nothing launched and no scan state changed. */
 int kvg_scan_pci_raw(kvg_ctx *ctx, const kvg_pci_raw *raw, kvg_pci_result **res, kvg_pci_snap **snap);
+/* The reads of createVgpuIDMap's walk callback (device_plugin.go:259-290), raw, one entry per visited non-directory
+ * Walk entry of the mdev bus in Walk order, decoded on the GPU into kvg_mdev_rec records and a type dictionary, then
+ * scanned as kvg_scan_mdev scans them.  The off / state conventions are those of kvg_pci_raw with KVG_MRAW_FIELDS
+ * fields per entry: the entry name; the mdev_type/name contents as os.ReadFile returned them; the os.Readlink TARGET
+ * of the entry itself; the numa_node contents of the parent.
+ *   KVG_MRAW_NUMA is <pci base>/<P>/numa_node, where P is what readGpuIDForVgpuFunc (:347-357) returns for the
+ *   KVG_MRAW_LINK target.  This path is the one thing the host derives, because it has to name the file; the record's
+ *   parent key still comes from the GPU's own decode of KVG_MRAW_LINK. */
+enum { KVG_MRAW_NAME, KVG_MRAW_TYPE, KVG_MRAW_LINK, KVG_MRAW_NUMA, KVG_MRAW_FIELDS };
+typedef struct kvg_mdev_raw {
+  size_t n;
+  const uint32_t *off;   /* [n * KVG_MRAW_FIELDS + 1], off[0] == 0, non-decreasing */
+  const uint8_t *bytes;  /* [off[n * KVG_MRAW_FIELDS]] */
+  const uint16_t *state; /* [n] bit f: read f was made; bit 8 + f: it failed (the bits of KVG_MRAW_NAME are unused) */
+} kvg_mdev_raw;
+
+/* The snapshot kvg_scan_mdev_raw decoded (library-owned; kvg_result_free).  recs are what the host snapshotter packs:
+ *   uuid_ok         1: uuid holds the name's 16 bytes (every name is a canonical lower-case 8-4-4-4-12 UUID and they
+ *                   ascend strictly); 0: bytes 0..3 of uuid are the Walk index, big-endian, the rest 0
+ *   parents_packed  1: parent is the packed BDF of the decoded parent (every decoded parent, an empty one included, is
+ *                   a canonical "dddd:bb:dd.f"); 0: the handle of the parent string, handles in order of first
+ *                   appearance from 0; parent h = parent_bytes[parent_off[h] .. parent_off[h + 1])
+ *   A record without a decoded parent holds 0 either way (its record is dropped by the scan).
+ *   type_idx indexes the raw type dictionary: the distinct mdev_type/name contents in order of first appearance, type
+ *   h = type_bytes[type_off[h] .. type_off[h + 1]) (a record whose type read failed holds 0). */
+typedef struct kvg_mdev_snap {
+  uint64_t n_records;
+  const kvg_mdev_rec *recs;
+  uint8_t uuid_ok, parents_packed;
+  uint32_t n_types;
+  const uint32_t *type_off; /* [n_types + 1] */
+  const uint8_t *type_bytes;
+  uint32_t n_parent_names;    /* 0 when parents_packed */
+  const uint32_t *parent_off; /* [n_parent_names + 1] */
+  const uint8_t *parent_bytes;
+} kvg_mdev_snap;
+
+/* Decode `raw` on the GPU with the reference's rules, in its short-circuit order (device_plugin.go:269-284):
+ *   mdev_type/name  a failed read sets KVG_MF_TYPE_ERR and nothing else is reached; otherwise the raw bytes (empty
+ *                   included) are the type string, interned into the raw type dictionary (the label rule :341-342
+ *                   stays in the scan)
+ *   link            reached when the type read succeeded; a failed read sets KVG_MF_PARENT_ERR.  The parent is
+ *                   strings.Split(target, "/")[len-2] with Trim "\n" (:347-357): the bytes between the second-to-last
+ *                   '/' (or the start) and the last '/'; it may be empty.  No '/' at all: the reference panics.
+ *   numa_node       reached when a parent was decoded: strings.TrimSpace over UTF-8, then strconv.ParseInt(s, 10, 64)
+ *                   (:304-320); a failed read or a parse error sets KVG_MF_NUMA_ERR and keeps the record with 0
+ * choose the snapshot modes (kvg_mdev_snap), intern the type strings (always) and the parents (index mode), pack the
+ * records into the context's record staging and scan them as kvg_scan_mdev does: *res equals
+ * kvg_scan_mdev(ctx, (*snap)->recs, n, &dict), where dict is the snapshot's type dictionary.  The call writes the scan
+ * state kvg_scan_mdev writes and nothing else (the mdev delta, mdev health and allocation state are untouched).
+ * Launches: one decode; one probe and one compaction for the types, and for the parents in index mode; one pack; then
+ * the scan's.  The host waits for the decode (one synchronisation) and for the intern (one more).
+ * Errors (none writes *res or *snap):
+ *   KVG_EINVAL  nothing launched: ctx, raw, res or snap NULL; off or state NULL with n > 0; bytes NULL with bytes to
+ *               read; off[0] != 0 or decreasing offsets; n above 0xfffffff0.  Found by the decode: a read the
+ *               reference reaches was not made (kvg_last_error names the lowest entry and the file).
+ *   KVG_EPANIC  the reference would panic: a reached link target without '/' (splitStr[len-2], :353); kvg_last_error
+ *               names the lowest such entry.  Beats KVG_ERANGE.
+ *   KVG_ERANGE  a reached numa_node that parses but does not fit int16, or a 65,536th distinct type string (the
+ *               65,535-type limit of kvg_scan_mdev); the lowest entry is named.
+ *   KVG_ESTATE  before kvg_pciids_load, as kvg_scan_mdev.
+ * n = 0: an empty result and snapshot, nothing launched and no scan state changed. */
+int kvg_scan_mdev_raw(kvg_ctx *ctx, const kvg_mdev_raw *raw, kvg_mdev_result **res, kvg_mdev_snap **snap);
 /* Allocate-time re-check of the vGPU plugin (generic_vgpu_device_plugin.go:216-221): match[i] = 1 iff the label of
  * file i -- Trim(raw, "\n") then every RE2 \s+ run ([\t\n\f\r ]) -> "_" (device_plugin.go:341-342) -- equals the
  * name_len bytes at `name`, else 0.  `files` uses the layout of kvg_type_dict, one entry per file that WAS read; a

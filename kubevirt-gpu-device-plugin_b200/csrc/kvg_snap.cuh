@@ -9,6 +9,13 @@
 //   k_compact<RawInternOp>  first appearances in Walk order -> handles 0, 1, ... (stable look-back compaction) and
 //                  the handle -> span table the host copies the string tables from
 //   k_raw_pack     addresses (index mode), groups and device ids (interned) into the records
+//
+// and the readers of createVgpuIDMap's walk callback (kvg_scan_mdev_raw), into the 32-byte records kvg_scan_mdev takes:
+//
+//   k_mraw_decode  one thread per Walk entry of the mdev bus: the short-circuit order of device_plugin.go:269-284;
+//                  writes the record as the numeric snapshot has it, the type and parent spans, and the verdicts
+//   k_raw_probe, k_compact<RawInternOp>  as above: column 0 = the type contents (always), 1 = the parent (index mode)
+//   k_mraw_pack    type handles, parent handles (index mode) and the Walk index (names not canonical) into the records
 #pragma once
 #include "../../include/kvgpu.h"
 #include "kvg_common.cuh"
@@ -34,7 +41,7 @@ struct RawCtrl {
 };
 
 struct RawIn {
-  const uint32_t* off;    // [n * KVG_RAW_FIELDS + 1]
+  const uint32_t* off;    // [n * KVG_RAW_FIELDS + 1] (the mdev walk: KVG_MRAW_FIELDS)
   const uint16_t* state;  // [n]
   const uint8_t* bytes;
   uint32_t n;
@@ -311,14 +318,16 @@ __global__ void __launch_bounds__(RAW_THREADS) k_raw_probe(const uint8_t* __rest
 }
 
 // The first appearances of column `col` in Walk order, compacted by k_compact: handle h goes to the h-th first
-// appearance.  hnd[i] = the handle of first appearance i, tab[h] = its span; a handle above 0xffff in the device
-// column is the range error of the 65,537th distinct string.
+// appearance.  hnd[i] = the handle of first appearance i, tab[h] = its span; a handle above max_hnd is the range error
+// of its entry, noted on field range_field (the PCI device column: 0xffff, the 65,537th distinct string; the mdev
+// types: 65534, the 65,536th; ~0 where every handle fits).
 struct RawInternOp {
   using Item = uint32_t;
   const uint64_t* table;
   const uint32_t* slot_of;
   const uint2* span;
   uint32_t n, col;
+  uint32_t max_hnd, range_field;
   uint32_t* hnd;
   uint2* tab;
   RawCtrl* ctrl;
@@ -332,7 +341,7 @@ struct RawInternOp {
   __device__ __forceinline__ void emit(uint32_t pos, const Item&, uint32_t i, uint32_t) {
     hnd[i] = pos;
     tab[pos] = __ldg(&span[2 * (size_t)i + col]);
-    if (col == RAW_COL_DEVICE && pos > 0xffffu) raw_note(&ctrl->range, i, KVG_RAW_DEVICE);
+    if (pos > max_hnd) raw_note(&ctrl->range, i, range_field);
   }
   __device__ __forceinline__ void tile_epilogue() {}
   __device__ __forceinline__ void finish(uint32_t total) { ctrl->n_names[col] = total; }
@@ -362,6 +371,146 @@ __global__ void __launch_bounds__(RAW_THREADS) k_raw_pack(RawPackArgs a, uint4* 
   if (a.table[RAW_COL_GROUP]) r.z = h[RAW_COL_GROUP];
   if (a.table[RAW_COL_DEVICE]) r.y = (r.y & 0xffffu) | (h[RAW_COL_DEVICE] & 0xffffu) << 16;
   recs[i] = r;
+}
+
+// ---- the mdev bus (kvg_scan_mdev_raw) --------------------------------------------------------------------------
+// RawCtrl::broken of the mdev walk: the names are not canonical ascending UUIDs / a parent is not a canonical BDF
+enum : uint32_t { MRAW_BAD_UUID = 1u, MRAW_BAD_PARENT = 2u };
+enum : uint32_t { MRAW_COL_TYPE = 0, MRAW_COL_PARENT = 1 };
+
+__device__ __forceinline__ uint32_t raw_bswap(uint32_t x) { return __byte_perm(x, 0, 0x0123); }
+
+// a canonical lower-case 'xxxxxxxx-xxxx-xxxx-xxxx-xxxxxxxxxxxx' -> its 16 bytes as two big-endian halves; false else
+__device__ __forceinline__ bool raw_uuid(const uint8_t* s, uint32_t len, unsigned long long* hi, unsigned long long* lo) {
+  if (len != 36) return false;
+  unsigned long long h = 0, l = 0;
+  for (uint32_t j = 0, k = 0; j < 36; j++) {
+    const uint8_t c = s[j];
+    if (j == 8 || j == 13 || j == 18 || j == 23) {
+      if (c != '-') return false;
+      continue;
+    }
+    if (!raw_hex(c)) return false;
+    if (k++ < 16) h = h << 4 | raw_hexval(c);
+    else l = l << 4 | raw_hexval(c);
+  }
+  *hi = h;
+  *lo = l;
+  return true;
+}
+
+// One mdev Walk entry: rec[0] = the UUID words (numeric mode), rec[1] = parent (packed BDF or 0), flags << 16,
+// parent_numa; span: the type contents when read and the parent when decoded ({1, 0} = none); bad: MRAW_BAD_*.
+struct MRawEntry {
+  uint4 rec[2];
+  uint2 span[2];
+  uint32_t bad;
+};
+
+__device__ __forceinline__ MRawEntry mraw_decode_entry(const RawIn& in, uint32_t i, RawCtrl* ctrl) {
+  const uint8_t* b = in.bytes;
+  const uint32_t* o = in.off + (size_t)i * KVG_MRAW_FIELDS;
+  const uint32_t st = __ldg(&in.state[i]);
+  MRawEntry r;
+  r.span[0] = r.span[1] = make_uint2(1, 0);
+  r.bad = 0;
+  unsigned long long hi = 0, lo = 0;
+  if (!raw_uuid(b + o[KVG_MRAW_NAME], o[KVG_MRAW_NAME + 1] - o[KVG_MRAW_NAME], &hi, &lo)) {
+    r.bad |= MRAW_BAD_UUID;
+    hi = lo = 0;
+  } else if (i > 0) {  // strictly ascending, as 16 big-endian bytes
+    const uint32_t* p = o - KVG_MRAW_FIELDS;
+    unsigned long long ph, pl;
+    if (raw_uuid(b + p[KVG_MRAW_NAME], p[KVG_MRAW_NAME + 1] - p[KVG_MRAW_NAME], &ph, &pl) &&
+        (ph > hi || (ph == hi && pl >= lo)))
+      r.bad |= MRAW_BAD_UUID;
+  }
+  uint32_t parent = 0, flags = 0;
+  long long numa = 0;
+  auto reach = [&](uint32_t f, uint32_t err_flag) -> bool {
+    if (!((st >> f) & 1u)) {
+      raw_note(&ctrl->miss, i, f);
+      return false;
+    }
+    if ((st >> (8 + f)) & 1u) {
+      flags |= err_flag;
+      return false;
+    }
+    return true;
+  };
+  if (reach(KVG_MRAW_TYPE, KVG_MF_TYPE_ERR)) {  // :269-273
+    r.span[MRAW_COL_TYPE] = make_uint2(o[KVG_MRAW_TYPE], o[KVG_MRAW_TYPE + 1]);
+    if (reach(KVG_MRAW_LINK, KVG_MF_PARENT_ERR)) {  // :275-279, readGpuIDForVgpuFunc :347-357
+      const uint32_t a = o[KVG_MRAW_LINK];
+      uint32_t e = o[KVG_MRAW_LINK + 1];
+      while (e > a && b[e - 1] != '/') e--;
+      if (e == a) {
+        raw_note(&ctrl->panic, i, KVG_MRAW_LINK);  // splitStr[len(splitStr)-2] of a single component
+      } else {
+        e--;  // the last '/'
+        uint32_t s = e;
+        while (s > a && b[s - 1] != '/') s--;
+        while (s < e && b[s] == '\n') s++;  // strings.Trim(.., "\n")
+        while (e > s && b[e - 1] == '\n') e--;
+        r.span[MRAW_COL_PARENT] = make_uint2(s, e);
+        parent = raw_bdf(b + s, e - s);
+        if (parent == RAW_NONE) {
+          r.bad |= MRAW_BAD_PARENT;
+          parent = 0;
+        }
+        if (reach(KVG_MRAW_NUMA, KVG_MF_NUMA_ERR)) {  // :280-284 (an error keeps the entry with node 0)
+          if (!raw_numa(b, o[KVG_MRAW_NUMA], o[KVG_MRAW_NUMA + 1], &numa)) {
+            flags |= KVG_MF_NUMA_ERR;
+            numa = 0;
+          } else if (numa < -32768 || numa > 32767) {
+            raw_note(&ctrl->range, i, KVG_MRAW_NUMA);
+          }
+        }
+      }
+    }
+  }
+  r.rec[0] = make_uint4(raw_bswap((uint32_t)(hi >> 32)), raw_bswap((uint32_t)hi), raw_bswap((uint32_t)(lo >> 32)),
+                        raw_bswap((uint32_t)lo));
+  r.rec[1] = make_uint4(parent, flags << 16, (uint32_t)numa & 0xffffu, 0);
+  return r;
+}
+
+__global__ void __launch_bounds__(RAW_THREADS) k_mraw_decode(RawIn in, uint4* __restrict__ recs, uint2* __restrict__ span,
+                                                             RawCtrl* ctrl) {
+  pdl_enter();
+  const uint32_t i = blockIdx.x * RAW_THREADS + threadIdx.x;
+  uint32_t bad = 0;
+  if (i < in.n) {
+    const MRawEntry e = mraw_decode_entry(in, i, ctrl);
+    recs[2 * (size_t)i] = e.rec[0];
+    recs[2 * (size_t)i + 1] = e.rec[1];
+    span[2 * (size_t)i] = e.span[0];
+    span[2 * (size_t)i + 1] = e.span[1];
+    bad = e.bad;
+  }
+  const uint32_t u = __ballot_sync(KVG_FULL, bad & MRAW_BAD_UUID) ? MRAW_BAD_UUID : 0u;
+  const uint32_t p = __ballot_sync(KVG_FULL, bad & MRAW_BAD_PARENT) ? MRAW_BAD_PARENT : 0u;
+  if (lane_id() == 0 && (u | p)) atomicOr(&ctrl->broken, u | p);
+}
+
+// The modes applied to the 32-byte records: type_idx from the type handles (always interned; 0 without a type),
+// parent from the parent handles when a.table[MRAW_COL_PARENT] is set (0 without a parent), and the Walk index,
+// big-endian, in bytes 0..3 of the UUID when a.index_addr is set.
+__global__ void __launch_bounds__(RAW_THREADS) k_mraw_pack(RawPackArgs a, uint4* __restrict__ recs) {
+  pdl_enter();
+  const uint32_t i = blockIdx.x * RAW_THREADS + threadIdx.x;
+  if (i >= a.n) return;
+  if (a.index_addr) recs[2 * (size_t)i] = make_uint4(raw_bswap(i), 0, 0, 0);
+  uint4 r = recs[2 * (size_t)i + 1];
+  uint32_t h[2] = {0, 0};
+  for (int c = 0; c < 2; c++) {
+    if (!a.table[c]) continue;
+    const uint32_t s = __ldg(&a.slot_of[c][i]);
+    if (s != RAW_NONE) h[c] = __ldg(&a.hnd[c][(uint32_t)ld_relaxed_u64(a.table[c] + s)]);
+  }
+  r.y = (r.y & 0xffff0000u) | (h[MRAW_COL_TYPE] & 0xffffu);
+  if (a.table[MRAW_COL_PARENT]) r.x = h[MRAW_COL_PARENT];
+  recs[2 * (size_t)i + 1] = r;
 }
 
 }  // namespace kvg

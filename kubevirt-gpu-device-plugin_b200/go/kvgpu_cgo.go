@@ -468,6 +468,126 @@ func createVgpuIDMapGPU() {
 	_ = sort.Strings // (kept: callers that want deterministic logs sort the keys)
 }
 
+// createVgpuIDMapRawGPU: createVgpuIDMap (:255-291) with every reader's rule on the GPU.  The walk reads the type file,
+// the entry's link target and the parent's numa_node and decodes nothing; kvg_scan_mdev_raw applies
+// readGpuIDForVgpuFunc, readNUMANodeFunc, the type dictionary and the snapshot modes, then scans.  The one thing
+// derived here is the numa_node path, which needs the parent component of the target (strings.Split(t, "/")[len-2],
+// Trim "\n"); the GPU decodes the parent key itself.  A vGPU with an empty parent is listed under gpuVgpuMap[""], as
+// in the reference.  Source only, like the rest of this file: it has never been compiled.
+func createVgpuIDMapRawGPU() {
+	kvgMu.Lock()
+	defer kvgMu.Unlock()
+	vGpuMap = make(map[string][]NvidiaGpuDevice)
+	gpuVgpuMap = make(map[string][]string)
+	var names []string
+	var bytes []byte
+	off := []uint32{0}
+	var state []uint16
+	filepath.Walk(vGpuBasePath, func(path string, info os.FileInfo, err error) error {
+		if err != nil {
+			return err
+		}
+		if info.IsDir() {
+			return nil
+		}
+		name := info.Name()
+		var st uint16
+		field := func(f int, data []byte, err error) {
+			st |= 1 << f
+			if err != nil {
+				st |= 1 << (8 + f)
+				data = nil
+			}
+			bytes = append(bytes, data...)
+			off = append(off, uint32(len(bytes)))
+		}
+		bytes = append(bytes, name...)
+		off = append(off, uint32(len(bytes)))
+		data, err := os.ReadFile(filepath.Join(vGpuBasePath, name, "mdev_type/name"))
+		field(C.KVG_MRAW_TYPE, data, err)
+		target, lerr := os.Readlink(filepath.Join(vGpuBasePath, name))
+		field(C.KVG_MRAW_LINK, []byte(target), lerr)
+		parts := strings.Split(target, "/")
+		if lerr == nil && len(parts) >= 2 {
+			data, err = os.ReadFile(filepath.Join(basePath, strings.Trim(parts[len(parts)-2], "\n"), "numa_node"))
+			field(C.KVG_MRAW_NUMA, data, err)
+		} else {
+			off = append(off, uint32(len(bytes))) // not reached by the reference: not made
+		}
+		names = append(names, name)
+		state = append(state, st)
+		return nil
+	})
+	if err := kvgEnsure(); err != nil {
+		log.Printf("Error: %v", err)
+		return
+	}
+	var raw C.kvg_mdev_raw
+	raw.n = C.size_t(len(state))
+	if len(state) > 0 {
+		raw.off = (*C.uint32_t)(C.CBytes(unsafe.Slice((*byte)(unsafe.Pointer(&off[0])), 4*len(off))))
+		raw.state = (*C.uint16_t)(C.CBytes(unsafe.Slice((*byte)(unsafe.Pointer(&state[0])), 2*len(state))))
+		raw.bytes = (*C.uint8_t)(C.CBytes(append(bytes, 0)))
+		defer C.free(unsafe.Pointer(raw.off))
+		defer C.free(unsafe.Pointer(raw.state))
+		defer C.free(unsafe.Pointer(raw.bytes))
+	}
+	var res *C.kvg_mdev_result
+	var snap *C.kvg_mdev_snap
+	if rc := C.kvg_scan_mdev_raw(kvgCtx, &raw, &res, &snap); rc != C.KVG_OK {
+		// KVG_EPANIC: the reference would panic here; the maps stay empty
+		log.Printf("Error: kvg_scan_mdev_raw: %s", C.GoString(C.kvg_last_error(kvgCtx)))
+		return
+	}
+	defer C.kvg_result_free(unsafe.Pointer(res))
+	defer C.kvg_result_free(unsafe.Pointer(snap))
+	var parentNames []string
+	if snap.parents_packed == 0 && snap.n_parent_names > 0 {
+		offs := unsafe.Slice(snap.parent_off, int(snap.n_parent_names)+1)
+		all := C.GoBytes(unsafe.Pointer(snap.parent_bytes), C.int(offs[snap.n_parent_names]))
+		for h := 0; h < int(snap.n_parent_names); h++ {
+			parentNames = append(parentNames, string(all[offs[h]:offs[h+1]]))
+		}
+	}
+	S := int(res.n_survivors)
+	surv := unsafe.Slice(res.survivors, S)
+	uuid := func(i uint32) string {
+		if snap.uuid_ok == 0 {
+			return names[surv[i].src]
+		}
+		u := surv[i].uuid
+		return fmt.Sprintf("%x-%x-%x-%x-%x", u[0:4], u[4:6], u[6:8], u[8:10], u[10:16])
+	}
+	parent := func(p C.uint32_t) string {
+		if snap.parents_packed == 0 {
+			return parentNames[p]
+		}
+		a := uint32(p)
+		return fmt.Sprintf("%04x:%02x:%02x.%x", a>>16, (a>>8)&0xff, (a>>3)&0x1f, a&7)
+	}
+	labelOff := unsafe.Slice(res.label_off, int(res.n_types)+1)
+	labels := unsafe.Slice((*byte)(unsafe.Pointer(res.label_bytes)), int(labelOff[res.n_types]))
+	tKeys := unsafe.Slice(res.type_keys, int(res.n_type_keys))
+	tOff := unsafe.Slice(res.type_off, int(res.n_type_keys)+1)
+	tPerm := unsafe.Slice(res.type_perm, S)
+	for k := range tKeys {
+		t := tKeys[k]
+		label := string(labels[labelOff[t]:labelOff[t+1]])
+		for _, i := range tPerm[tOff[k]:tOff[k+1]] {
+			vGpuMap[label] = append(vGpuMap[label], NvidiaGpuDevice{addr: uuid(uint32(i)), numaNode: int64(surv[i].numa)})
+		}
+	}
+	pKeys := unsafe.Slice(res.par_keys, int(res.n_parents))
+	pOff := unsafe.Slice(res.par_off, int(res.n_parents)+1)
+	pPerm := unsafe.Slice(res.par_perm, S)
+	for k := range pKeys {
+		g := parent(pKeys[k])
+		for _, i := range pPerm[pOff[k]:pOff[k+1]] {
+			gpuVgpuMap[g] = append(gpuVgpuMap[g], uuid(uint32(i)))
+		}
+	}
+}
+
 // cTypeDict lays raw out as a kvg_type_dict.  The dictionary struct holds two pointers: they must not be Go pointers
 // (cgo rule: a Go pointer passed to C may not point at memory that itself holds Go pointers), so both arrays live in
 // C memory; free releases them after the call.

@@ -18,6 +18,7 @@ HEADER_PATH = os.path.join(os.path.dirname(_PKG), "include", "kvgpu.h")
 KVG_OK, KVG_EINVAL, KVG_ECUDA, KVG_ENOMEM, KVG_ENCCL, KVG_ESTATE, KVG_ERANGE = 0, -1, -2, -3, -4, -5, -6
 KVG_EPANIC = -7
 RAW_NAME, RAW_VENDOR, RAW_DRIVER, RAW_GROUP, RAW_NUMA, RAW_DEVICE, RAW_FIELDS = range(7)
+MRAW_NAME, MRAW_TYPE, MRAW_LINK, MRAW_NUMA, MRAW_FIELDS = range(5)
 KVG_NO_NAME = 0xFFFFFFFF
 ERR_NAMES = {0: "KVG_OK", -1: "KVG_EINVAL", -2: "KVG_ECUDA", -3: "KVG_ENOMEM", -4: "KVG_ENCCL",
              -5: "KVG_ESTATE", -6: "KVG_ERANGE", -7: "KVG_EPANIC"}
@@ -84,6 +85,16 @@ class PciSnapC(C.Structure):
                 ("packed_addr", C.c_uint8), ("groups_numeric", C.c_uint8), ("devices_numeric", C.c_uint8),
                 ("n_group_names", C.c_uint32), ("group_off", C.c_void_p), ("group_bytes", C.c_void_p),
                 ("n_device_names", C.c_uint32), ("device_off", C.c_void_p), ("device_bytes", C.c_void_p)]
+
+
+class MdevRawC(C.Structure):
+    _fields_ = [("n", C.c_size_t), ("off", C.c_void_p), ("bytes", C.c_void_p), ("state", C.c_void_p)]
+
+
+class MdevSnapC(C.Structure):
+    _fields_ = [("n_records", C.c_uint64), ("recs", C.c_void_p), ("uuid_ok", C.c_uint8), ("parents_packed", C.c_uint8),
+                ("n_types", C.c_uint32), ("type_off", C.c_void_p), ("type_bytes", C.c_void_p),
+                ("n_parent_names", C.c_uint32), ("parent_off", C.c_void_p), ("parent_bytes", C.c_void_p)]
 
 
 class MdevResultC(C.Structure):
@@ -179,6 +190,7 @@ def load() -> C.CDLL:
         "kvg_scan_pci": (C.c_int, [vp, vp, sz, P(P(PciResultC))]),
         "kvg_scan_pci_raw": (C.c_int, [vp, P(PciRawC), P(P(PciResultC)), P(P(PciSnapC))]),
         "kvg_scan_mdev": (C.c_int, [vp, vp, sz, P(TypeDict), P(P(MdevResultC))]),
+        "kvg_scan_mdev_raw": (C.c_int, [vp, P(MdevRawC), P(P(MdevResultC)), P(P(MdevSnapC))]),
         "kvg_mdev_label_match": (C.c_int, [vp, P(TypeDict), vp, sz, vp]),
         "kvg_pci_group_check": (C.c_int, [vp, vp, vp, sz, P(sz)]),
         "kvg_preferred_allocation": (C.c_int, [vp, vp, u32, vp, sz, vp, vp]),

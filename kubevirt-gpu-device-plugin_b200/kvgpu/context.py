@@ -282,6 +282,34 @@ class Context:
         del keep
         return self._take_mdev(res)
 
+    def scan_mdev_raw(self, raw):
+        """createVgpuIDMap from the raw reads of its walk (plugin.read_mdev_tree_raw): the GPU decodes them into a
+        snapshot and its raw type dictionary, then scans it -> (MdevResult, MdevSnapshot).  Raises plugin.ReferencePanic
+        where the Go reference would panic."""
+        from .plugin import MdevSnapshot, ReferencePanic
+        off = np.ascontiguousarray(raw.off, dtype=np.uint32)
+        state = np.ascontiguousarray(raw.state, dtype=np.uint16)
+        blob = np.frombuffer(bytes(raw.bytes) + b"\0", dtype=np.uint8)
+        arg = L.MdevRawC(len(state), off.ctypes.data, blob.ctypes.data, state.ctypes.data)
+        res, snap = C.POINTER(L.MdevResultC)(), C.POINTER(L.MdevSnapC)()
+        rc = self._lib.kvg_scan_mdev_raw(self._h, C.byref(arg), C.byref(res), C.byref(snap))
+        if rc == L.KVG_EPANIC:
+            raise ReferencePanic((self._lib.kvg_last_error(self._h) or b"").decode("latin-1"))
+        self._ck(rc)
+        sn = snap.contents
+
+        def table(n, off_p, bytes_p):
+            o = L._arr(off_p, int(n) + 1, np.uint32)
+            b = C.string_at(bytes_p, int(o[-1])) if o[-1] else b""
+            return [b[o[k]:o[k + 1]] for k in range(int(n))]
+
+        parents = None if sn.parents_packed else [p.decode("latin-1") for p in
+                                                  table(sn.n_parent_names, sn.parent_off, sn.parent_bytes)]
+        out = MdevSnapshot(L._arr(sn.recs, int(sn.n_records), L.MDEV_REC), list(raw.names),
+                           table(sn.n_types, sn.type_off, sn.type_bytes), parents, bool(sn.uuid_ok))
+        self._lib.kvg_result_free(snap)
+        return self._take_mdev(res), out
+
     def mdev_label_match(self, raw_files: list, name) -> np.ndarray:
         r"""The vGPU plugin's Allocate-time re-check (include/kvgpu.h kvg_mdev_label_match), one launch: element i is
         True iff the label of raw_files[i] (Trim "\n", then every \s+ run -> "_") equals `name`.  A str name is

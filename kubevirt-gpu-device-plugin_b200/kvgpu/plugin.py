@@ -419,6 +419,64 @@ def snapshot_mdev_tree(vgpu_base: str, pci_base: str) -> MdevSnapshot:
     return MdevSnapshot(recs, names, raw_types, parent_names, uuid_ok)
 
 
+@dataclass
+class MdevRaw:
+    """What the readers of createVgpuIDMap's walk callback got, undecoded (include/kvgpu.h kvg_mdev_raw): field f of
+    entry i is bytes[off[i * MRAW_FIELDS + f]:off[i * MRAW_FIELDS + f + 1]] (name, mdev_type/name contents, the entry's
+    link target, the parent's numa_node contents); state[i] bit f: read f was made, bit 8 + f: it failed.
+    names: the Walk-order entry names."""
+    names: list
+    off: np.ndarray     # u32 [n * MRAW_FIELDS + 1]
+    bytes: bytes
+    state: np.ndarray   # u16 [n]
+
+
+def mdev_numa_parent(target: bytes):
+    """The parent component readGpuIDForVgpuFunc (:347-357) takes from a link target -- strings.Split(target, "/")
+    [len-2] with Trim "\n" -- which names the numa_node file to read; None where the reference panics (no '/')."""
+    parts = target.split(b"/")
+    return None if len(parts) < 2 else parts[-2].strip(b"\n")
+
+
+def read_mdev_tree_raw(vgpu_base: str, pci_base: str) -> MdevRaw:
+    """The walk of snapshot_mdev_tree with every read it can make and nothing decoded: the type file as read, the link
+    target as os.readlink returns it, and <pci_base>/<parent>/numa_node for the parent of that target (not made when
+    the link is unreadable or has no '/').  The GPU decodes only what the reference reaches."""
+    names, parts, state = [], [], []
+    vbase, pbase = os.fsencode(vgpu_base), os.fsencode(pci_base)
+    for name, is_dir, err in _walk(vgpu_base):
+        if err:
+            break
+        if is_dir:
+            continue
+        bname = os.fsencode(name)
+        st, row = 0, [bname, b"", b"", b""]
+
+        def take(f, read):
+            nonlocal st
+            st |= 1 << f
+            try:
+                row[f] = read()
+            except OSError:
+                st |= 1 << (8 + f)
+
+        take(L.MRAW_TYPE, lambda: open(os.path.join(vbase, bname, b"mdev_type", b"name"), "rb").read())
+        take(L.MRAW_LINK, lambda: os.readlink(os.path.join(vbase, bname)))
+        parent = mdev_numa_parent(row[L.MRAW_LINK]) if not (st >> (8 + L.MRAW_LINK)) & 1 else None
+        if parent is not None:
+            take(L.MRAW_NUMA, lambda: open(os.path.join(pbase, parent, b"numa_node"), "rb").read())
+        names.append(name)
+        parts.append(row)
+        state.append(st)
+    lens = np.array([len(x) for row in parts for x in row], dtype=np.int64)
+    off = np.zeros(len(lens) + 1, dtype=np.int64)
+    np.cumsum(lens, out=off[1:])
+    if off[-1] > 0xFFFFFFFF:
+        raise ValueError("the raw reads of %s exceed 4 GiB" % vgpu_base)
+    return MdevRaw(names, off.astype(np.uint32), b"".join(x for row in parts for x in row),
+                   np.array(state, dtype=np.uint16))
+
+
 def snapshot_mdev_ids(vgpu_base: str, pci_base: str, uuids, intern: dict) -> MdevSnapshot:
     """Snapshot the mdevs `uuids` in THAT order (the health re-scan's fixed record order; a Walk would re-index when
     one vanishes, which is the very event health has to see), with the readers and flag rules of snapshot_mdev_tree.
@@ -771,8 +829,14 @@ class DiscoveryScan:
             return _rebuild_pci_maps(self.maps, res, snap, self.ctx.name_lookup)
         return apply_pci_delta(self.maps, res, delta, snap, prev, name_of=self.ctx.name_lookup)
 
-    def create_vgpu_id_map(self) -> Maps:
+    def create_vgpu_id_map(self, raw: bool = False) -> Maps:
+        """raw=True: the walk reads everything and the GPU decodes the reads (Context.scan_mdev_raw).  The Maps are the
+        same, except that a vGPU whose parent component is empty is listed under gpuVgpuMap[""] as in the reference
+        (the default path lists it under "0000:00:00.0")."""
         self._ensure_table()
+        if raw:
+            res, snap = self.ctx.scan_mdev_raw(read_mdev_tree_raw(self.vGpuBasePath, self.basePath))
+            return mdev_maps_from_result(res, snap, self.maps)
         snap = snapshot_mdev_tree(self.vGpuBasePath, self.basePath)
         res = self.ctx.scan_mdev(snap.recs, snap.raw_types)
         return mdev_maps_from_result(res, snap, self.maps)
