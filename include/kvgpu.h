@@ -545,6 +545,71 @@ int kvg_pci_allocate_check(kvg_ctx *ctx, const kvg_alloc_req *reqs, uint32_t n_r
                            const uint32_t *want_group, size_t n_recs, const uint32_t *ids, size_t n_ids,
                            const uint32_t *egm_off, const uint32_t *egm_gpu, uint32_t n_egm, uint32_t n_egm_gpus,
                            uint32_t *first_bad, uint8_t *egm_take);
+/* The passthrough plugin's Allocate decisions (generic_device_plugin.go:352-444) for every container request of one
+ * AllocateRequest, decided on the GPU from the raw reads the reference makes for them: the group re-check of every
+ * member (:387-399), EGM discovery's decoding of the class entries (discoverEGMDevicesFunc :120-157) and the EGM match
+ * (egmPathsForAllocatedGPUs :159-184).  The host lists directories, stats and reads; it decodes nothing.
+ * Members: every member of every requested group, request after request, reqs[r].n_members per request, in the order
+ * the reference visits them.  Field f of member i is member_bytes[member_off[3i + f] .. member_off[3i + f + 1]):
+ *   KVG_AMEM_LINK    the iommu_group link TARGET as os.Readlink returned it
+ *   KVG_AMEM_VENDOR  the vendor file contents as os.ReadFile returned them
+ *   KVG_AMEM_GROUP   the group string the maps hold for the member (bdfToIommu[bdf]); always present
+ * member_state[i] bit f: read f was made; bit 8 + f: it failed (only LINK and VENDOR have bits).
+ * IDs: the requests' DevicesIDs, reqs[r].n_ids per request; ID k = id_bytes[id_off[k] .. id_off[k + 1]).
+ * EGM class entries: every entry of the EGM class directory in ReadDir order; field f of entry e is
+ * egm_bytes[egm_off[2e + f] .. egm_off[2e + f + 1]): KVG_AEGM_NAME the entry name, KVG_AEGM_GPUS the gpu_devices
+ * contents.  egm_state[e] bit f / 8 + f: read f made / failed, for KVG_AEGM_GPUS and for KVG_AEGM_STAT, the Stat of
+ * /dev/<name> (it has no bytes).  Every offset table starts at 0 and does not decrease.
+ * Rules, in the reference's short-circuit order:
+ *   member     the link's basename (filepath.Split) must equal the group string byte for byte ("042" is not "42"),
+ *              else the member fails and its vendor is not reached; a failed read fails it.  Then the vendor: a failed
+ *              read fails the member; fewer than 2 bytes is the reference's panic (data[2:]); else Trim(data[2:], "\n")
+ *              must be exactly "10de".
+ *   request    first_bad[r] = the smallest failing position within the request, or reqs[r].n_members; panic[r] = 1
+ *              iff the member at first_bad[r] failed by that panic (a per-request output, not a call error: an earlier
+ *              request may fail first).  The reads of a request up to and including its first failing member are
+ *              reached; the later ones may be made or skipped.
+ *   EGM entry  egm_kept[e] = 1 iff its name has the prefix "egm", its gpu_devices read succeeded, strings.Fields of
+ *              the contents (unicode.IsSpace over UTF-8; an invalid byte is RuneError, not a space) is not empty, and
+ *              the Stat succeeded.  gpu_devices is reached for "egm" names, the Stat when there are fields.
+ *   keys       strings.ToLower(strings.TrimSpace(s)) with Go's semantics: runes through unicode.ToLower (simple case
+ *              mapping, Unicode 15.0.0), each invalid byte one U+FFFD, so "\xff" and "\xfe" are the same key.
+ *              egm_take[r * n_egm + e] = 1 iff entry e is kept and the key of every field of e is the key of one of
+ *              request r's IDs.  Duplicates do not matter.  The reference mounts /dev/<name> of the taken entries,
+ *              sorted.
+ * Launches: one member decode when there are members, one key kernel when n_egm > 0, and k_pci_allocate_check when
+ * n_reqs > 0, so at most three; none for a call with no requests and no EGM entries, or one refused before launch
+ * (the KVG_EINVAL argument errors below).  A refusal found on the device launches what the call would have launched.
+ * One host synchronisation per call that launches.  The call uses buffers of its own: no scan, fetch, delta, health or
+ * name-table state changes, and it does not wait for a pci.ids parse.
+ * Errors (the outputs stay unwritten):
+ *   KVG_EINVAL  nothing launched: ctx NULL; reqs, first_bad or panic NULL with n_reqs > 0; raw NULL; an offset table,
+ *               state or bytes NULL with entries or bytes to read; egm_kept NULL with n_egm > 0; egm_take NULL with
+ *               n_reqs * n_egm > 0; member or ID counts that do not add up; n_members or n_ids > UINT32_MAX; an offset
+ *               table that does not start at 0 or decreases.  Found on the device: a reached read that was not made;
+ *               kvg_last_error names the lowest (the EGM entries first, as the reference discovers them before it reads
+ *               any member, then request by request).
+ *   KVG_ERANGE  more than KVG_ALLOC_RAW_MAX_EGM_KEYS distinct keys among the kept entries' fields; kvg_last_error
+ *               names the lowest entry that carries one beyond the cap.  A missing read beats it. */
+enum { KVG_AMEM_LINK, KVG_AMEM_VENDOR, KVG_AMEM_GROUP, KVG_AMEM_FIELDS };
+enum { KVG_AEGM_NAME, KVG_AEGM_GPUS, KVG_AEGM_FIELDS, KVG_AEGM_STAT = KVG_AEGM_FIELDS };
+/* distinct EGM keys per call: the bitmap of kvg_pci_allocate_check, less one handle that marks an entry not kept */
+#define KVG_ALLOC_RAW_MAX_EGM_KEYS (KVG_ALLOC_MAX_EGM_GPUS - 1)
+typedef struct kvg_alloc_raw {
+  size_t n_members;
+  const uint32_t *member_off;   /* [n_members * KVG_AMEM_FIELDS + 1] */
+  const uint8_t *member_bytes;
+  const uint16_t *member_state; /* [n_members] */
+  size_t n_ids;
+  const uint32_t *id_off;       /* [n_ids + 1] */
+  const uint8_t *id_bytes;
+  uint32_t n_egm;
+  const uint32_t *egm_off;      /* [n_egm * KVG_AEGM_FIELDS + 1] */
+  const uint8_t *egm_bytes;
+  const uint16_t *egm_state;    /* [n_egm] */
+} kvg_alloc_raw;
+int kvg_pci_allocate_raw(kvg_ctx *ctx, const kvg_alloc_req *reqs, uint32_t n_reqs, const kvg_alloc_raw *raw,
+                         uint32_t *first_bad, uint8_t *panic, uint8_t *egm_kept, uint8_t *egm_take);
 /* GetPreferredAllocation of the passthrough plugin (generic_device_plugin.go:470-608): the NUMA packing of every
  * container request of one PreferredAllocationRequest, in one launch.
  * Entries: request r's entries follow those of requests 0..r-1 in `ids`, its n_must must-include IDs first, then its

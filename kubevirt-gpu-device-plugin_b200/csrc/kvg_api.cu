@@ -34,6 +34,7 @@
 #include "kvg_delta.cuh"
 #include "kvg_alloc.cuh"
 #include "kvg_snap.cuh"
+#include "kvg_alloc_raw.cuh"
 
 using namespace kvg;
 

@@ -28,7 +28,9 @@ package device_plugin
 import "C"
 
 import (
+	"errors"
 	"fmt"
+	"io/fs"
 	"log"
 	"os"
 	"path/filepath"
@@ -997,4 +999,174 @@ func revalidateVgpuBatchGPU(ids []string, deviceName string) ([]bool, error) {
 		keep[at[k]] = m != 0
 	}
 	return keep, nil
+}
+
+// EGMEntryRaw is one entry of the EGM class directory as discoverEGMDevicesFunc's reads returned it, undecoded.
+type EGMEntryRaw struct {
+	Name       string
+	GPUDevices []byte
+	GPUErr     error // the gpu_devices read
+	StatErr    error // os.Stat of /dev/<name>
+}
+
+// discoverEGMRaw lists and reads what discoverEGMDevicesFunc (generic_device_plugin.go:120-157) reads, for every
+// entry, and decodes nothing: kvg_pci_allocate_raw applies the "egm" prefix, strings.Fields and the Stat rule.
+func discoverEGMRaw() ([]EGMEntryRaw, error) {
+	egmClassDir := filepath.Join(rootPath, strings.TrimPrefix(egmClassPath, "/"))
+	entries, err := os.ReadDir(egmClassDir)
+	if err != nil {
+		if errors.Is(err, fs.ErrNotExist) {
+			return nil, nil
+		}
+		return nil, err
+	}
+	out := make([]EGMEntryRaw, 0, len(entries))
+	for _, entry := range entries {
+		e := EGMEntryRaw{Name: entry.Name()}
+		e.GPUDevices, e.GPUErr = os.ReadFile(filepath.Join(egmClassDir, e.Name, "gpu_devices"))
+		_, e.StatErr = os.Stat(filepath.Join(rootPath, strings.TrimPrefix(filepath.Join(deviceDir, e.Name), "/")))
+		out = append(out, e)
+	}
+	return out, nil
+}
+
+// allocateRawGPU is allocateCheckGPU with no decoding in Go (Python twin: kvgpu/serve.py AllocateRawCheck, tested
+// against AllocateCheck by tests/test_serve_allocate_raw.py): every member's iommu_group link target and vendor
+// contents are read raw with os.Readlink and os.ReadFile, and together with the group string the maps hold, the
+// DevicesIDs and discoverEGMRaw's entries go to one kvg_pci_allocate_raw call, which applies readLinkFunc,
+// readIDFromFileFunc, discoverEGMDevicesFunc and egmPathsForAllocatedGPUs' key rule on the GPU.  Where the library
+// reports that the reference's vendor read panics (panic[r]), vendorPanic re-slices the same bytes, so d.panic is the
+// runtime.Error the reference's data[2:] raises, the value allocateCheckGPU recovers.  Like the rest of the file it
+// is source only and has not been compiled.
+func allocateRawGPU(members [][]allocMember, ids [][]string, egm []EGMEntryRaw) ([]allocDecision, error) {
+	if len(members) == 0 && len(egm) == 0 {
+		return nil, nil
+	}
+	var mOff, iOff, eOff []uint32
+	var mBytes, iBytes, eBytes []byte
+	var mState, eState []uint16
+	var vendors [][]byte // per member, the vendor contents as read
+	push := func(off *[]uint32, b *[]byte, data []byte) {
+		if len(*off) == 0 {
+			*off = append(*off, 0)
+		}
+		*b = append(*b, data...)
+		*off = append(*off, uint32(len(*b)))
+	}
+	reqs := make([]C.kvg_alloc_req, len(members))
+	for r := range members {
+		for _, m := range members[r] {
+			st := uint16(1<<C.KVG_AMEM_LINK | 1<<C.KVG_AMEM_VENDOR)
+			target, err := os.Readlink(filepath.Join(basePath, m.addr, "iommu_group"))
+			if err != nil {
+				st |= 1 << (8 + C.KVG_AMEM_LINK)
+			}
+			vendor, err := os.ReadFile(filepath.Join(basePath, m.addr, "vendor"))
+			if err != nil {
+				st |= 1 << (8 + C.KVG_AMEM_VENDOR)
+			}
+			push(&mOff, &mBytes, []byte(target))
+			push(&mOff, &mBytes, vendor)
+			push(&mOff, &mBytes, []byte(m.group))
+			mState = append(mState, st)
+			vendors = append(vendors, vendor)
+		}
+		for _, id := range ids[r] {
+			push(&iOff, &iBytes, []byte(id))
+		}
+		reqs[r] = C.kvg_alloc_req{n_members: C.uint32_t(len(members[r])), n_ids: C.uint32_t(len(ids[r]))}
+	}
+	for _, e := range egm {
+		st := uint16(1<<C.KVG_AEGM_GPUS | 1<<C.KVG_AEGM_STAT)
+		if e.GPUErr != nil {
+			st |= 1 << (8 + C.KVG_AEGM_GPUS)
+		}
+		if e.StatErr != nil {
+			st |= 1 << (8 + C.KVG_AEGM_STAT)
+		}
+		push(&eOff, &eBytes, []byte(e.Name))
+		push(&eOff, &eBytes, e.GPUDevices)
+		eState = append(eState, st)
+	}
+	// the library copies the inputs before it returns (cgo pointer rule): C copies of every table and byte array, so
+	// &raw, a Go value, holds no Go pointer
+	var cmem []unsafe.Pointer
+	defer func() {
+		for _, p := range cmem {
+			C.free(p)
+		}
+	}()
+	cCopy := func(b []byte) unsafe.Pointer {
+		if len(b) == 0 {
+			return nil
+		}
+		p := C.CBytes(b)
+		cmem = append(cmem, p)
+		return p
+	}
+	u32 := func(v []uint32) *C.uint32_t {
+		if len(v) == 0 {
+			return nil
+		}
+		return (*C.uint32_t)(cCopy(unsafe.Slice((*byte)(unsafe.Pointer(&v[0])), 4*len(v))))
+	}
+	u16 := func(v []uint16) *C.uint16_t {
+		if len(v) == 0 {
+			return nil
+		}
+		return (*C.uint16_t)(cCopy(unsafe.Slice((*byte)(unsafe.Pointer(&v[0])), 2*len(v))))
+	}
+	var raw C.kvg_alloc_raw
+	raw.n_members = C.size_t(len(mState))
+	raw.member_off, raw.member_state = u32(mOff), u16(mState)
+	raw.member_bytes = (*C.uint8_t)(cCopy(mBytes))
+	if len(iOff) > 0 {
+		raw.n_ids = C.size_t(len(iOff) - 1)
+	}
+	raw.id_off, raw.id_bytes = u32(iOff), (*C.uint8_t)(cCopy(iBytes))
+	raw.n_egm = C.uint32_t(len(egm))
+	raw.egm_off, raw.egm_state = u32(eOff), u16(eState)
+	raw.egm_bytes = (*C.uint8_t)(cCopy(eBytes))
+	firstBad := make([]C.uint32_t, len(members)+1)
+	panics := make([]C.uint8_t, len(members)+1)
+	kept := make([]C.uint8_t, len(egm)+1)
+	take := make([]C.uint8_t, len(members)*len(egm)+1)
+	kvgMu.Lock()
+	defer kvgMu.Unlock()
+	if err := kvgEnsure(); err != nil {
+		return nil, err
+	}
+	var reqPtr *C.kvg_alloc_req
+	if len(reqs) > 0 {
+		reqPtr = &reqs[0]
+	}
+	if rc := C.kvg_pci_allocate_raw(kvgCtx, reqPtr, C.uint32_t(len(reqs)), &raw, &firstBad[0], &panics[0], &kept[0],
+		&take[0]); rc != C.KVG_OK {
+		return nil, fmt.Errorf("kvg_pci_allocate_raw: %d %s", int(rc), C.GoString(C.kvg_last_error(kvgCtx)))
+	}
+	out := make([]allocDecision, len(members))
+	for r, m0 := 0, 0; r < len(members); m0, r = m0+len(members[r]), r+1 {
+		d := allocDecision{bad: -1, egm: []string{}}
+		if int(firstBad[r]) < len(members[r]) {
+			d.bad = int(firstBad[r])
+			if panics[r] != 0 {
+				d.panic = vendorPanic(vendors[m0+d.bad])
+			}
+		}
+		for e := range egm { // ReadDir order is name order, so the paths come out sorted
+			if kept[e] != 0 && take[r*len(egm)+e] != 0 {
+				d.egm = append(d.egm, filepath.Join(deviceDir, egm[e].Name))
+			}
+		}
+		out[r] = d
+	}
+	return out, nil
+}
+
+// vendorPanic is what readIDFromFileFunc's strings.Trim(string(data[2:]), "\n") panics with on `data`: the recovered
+// runtime.Error, or nil when it does not panic.
+func vendorPanic(data []byte) (p interface{}) {
+	defer func() { p = recover() }()
+	_ = strings.Trim(string(data[2:]), "\n")
+	return nil
 }

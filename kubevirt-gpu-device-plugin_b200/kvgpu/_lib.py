@@ -19,6 +19,9 @@ KVG_OK, KVG_EINVAL, KVG_ECUDA, KVG_ENOMEM, KVG_ENCCL, KVG_ESTATE, KVG_ERANGE = 0
 KVG_EPANIC = -7
 RAW_NAME, RAW_VENDOR, RAW_DRIVER, RAW_GROUP, RAW_NUMA, RAW_DEVICE, RAW_FIELDS = range(7)
 MRAW_NAME, MRAW_TYPE, MRAW_LINK, MRAW_NUMA, MRAW_FIELDS = range(5)
+AMEM_LINK, AMEM_VENDOR, AMEM_GROUP, AMEM_FIELDS = range(4)
+AEGM_NAME, AEGM_GPUS, AEGM_FIELDS = range(3)
+AEGM_STAT = AEGM_FIELDS
 KVG_NO_NAME = 0xFFFFFFFF
 ERR_NAMES = {0: "KVG_OK", -1: "KVG_EINVAL", -2: "KVG_ECUDA", -3: "KVG_ENOMEM", -4: "KVG_ENCCL",
              -5: "KVG_ESTATE", -6: "KVG_ERANGE", -7: "KVG_EPANIC"}
@@ -50,6 +53,7 @@ PREF_RES = np.dtype([("n_out", "<i4"), ("n_must_distinct", "<u4")])
 PREF_NODE_NONE = 0xFFFFFFFF
 ALLOC_REQ = np.dtype([("n_members", "<u4"), ("n_ids", "<u4")])
 ALLOC_MAX_EGM_GPUS = 65536
+ALLOC_RAW_MAX_EGM_KEYS = ALLOC_MAX_EGM_GPUS - 1
 assert PCI_REC.itemsize == 16 and PCI_SURV.itemsize == 16 and PCI_CHANGE.itemsize == 32
 assert MDEV_REC.itemsize == 32 and MDEV_SURV.itemsize == 32 and MDEV_CHANGE.itemsize == 48
 assert PREF_ID.itemsize == 8 and PREF_REQ.itemsize == 16 and PREF_RES.itemsize == 8 and ALLOC_REQ.itemsize == 8
@@ -78,6 +82,12 @@ class PciResultC(C.Structure):
 
 class PciRawC(C.Structure):
     _fields_ = [("n", C.c_size_t), ("off", C.c_void_p), ("bytes", C.c_void_p), ("state", C.c_void_p)]
+
+
+class AllocRawC(C.Structure):
+    _fields_ = [("n_members", C.c_size_t), ("member_off", C.c_void_p), ("member_bytes", C.c_void_p),
+                ("member_state", C.c_void_p), ("n_ids", C.c_size_t), ("id_off", C.c_void_p), ("id_bytes", C.c_void_p),
+                ("n_egm", C.c_uint32), ("egm_off", C.c_void_p), ("egm_bytes", C.c_void_p), ("egm_state", C.c_void_p)]
 
 
 class PciSnapC(C.Structure):
@@ -195,6 +205,7 @@ def load() -> C.CDLL:
         "kvg_pci_group_check": (C.c_int, [vp, vp, vp, sz, P(sz)]),
         "kvg_preferred_allocation": (C.c_int, [vp, vp, u32, vp, sz, vp, vp]),
         "kvg_pci_allocate_check": (C.c_int, [vp, vp, u32, vp, vp, sz, vp, sz, vp, vp, u32, u32, vp, vp]),
+        "kvg_pci_allocate_raw": (C.c_int, [vp, vp, u32, P(AllocRawC), vp, vp, vp, vp]),
         "kvg_health_rescan": (C.c_int, [vp, vp, sz, P(P(HealthDeltaC))]),
         "kvg_health_reset": (C.c_int, [vp]),
         "kvg_health_rescan_mdev": (C.c_int, [vp, vp, sz, u32, vp, sz, P(P(HealthDeltaC))]),

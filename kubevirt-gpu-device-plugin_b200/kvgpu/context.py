@@ -362,6 +362,35 @@ class Context:
             first_bad.ctypes.data, take.ctypes.data))
         return first_bad, take.astype(bool)
 
+    def pci_allocate_raw(self, raw) -> tuple:
+        """The passthrough plugin's Allocate decisions for every container request of one call, from the raw reads
+        (include/kvgpu.h kvg_pci_allocate_raw; plugin.pack_alloc_raw builds `raw`).  Returns (first_bad, panic, kept,
+        take): first_bad[r] = the first failing position of request r, or its member count; panic[r] = that member's
+        vendor read is the reference's panic; kept[e] = EGM class entry e is an EGM device; take[r, e] = request r
+        mounts entry e.  Raises KvgError for a reached read that was not made (KVG_EINVAL) and for more than
+        ALLOC_RAW_MAX_EGM_KEYS distinct EGM keys (KVG_ERANGE)."""
+        arr = lambda a, t: np.ascontiguousarray(a, dtype=t)   # noqa: E731
+        blob = lambda b: np.frombuffer(bytes(b) + b"\0", dtype=np.uint8)   # noqa: E731
+        n_members, n_ids = arr(raw.n_members, np.uint32), arr(raw.n_ids, np.uint32)
+        moff, mst, ioff = arr(raw.member_off, np.uint32), arr(raw.member_state, np.uint16), arr(raw.id_off, np.uint32)
+        eoff, est = arr(raw.egm_off, np.uint32), arr(raw.egm_state, np.uint16)
+        mb, ib, eb = blob(raw.member_bytes), blob(raw.id_bytes), blob(raw.egm_bytes)
+        if len(n_members) != len(n_ids):
+            raise ValueError("pci_allocate_raw: %d / %d per-request counts" % (len(n_members), len(n_ids)))
+        reqs = np.zeros(len(n_members), dtype=L.ALLOC_REQ)
+        reqs["n_members"], reqs["n_ids"] = n_members, n_ids
+        n_egm = len(est)
+        arg = L.AllocRawC(len(mst), moff.ctypes.data, mb.ctypes.data, mst.ctypes.data, max(len(ioff) - 1, 0),
+                          ioff.ctypes.data, ib.ctypes.data, n_egm, eoff.ctypes.data, eb.ctypes.data, est.ctypes.data)
+        first_bad = np.zeros(len(reqs), dtype=np.uint32)
+        panic = np.zeros(len(reqs), dtype=np.uint8)
+        kept = np.zeros(n_egm, dtype=np.uint8)
+        take = np.zeros((len(reqs), n_egm), dtype=np.uint8)
+        self._ck(self._lib.kvg_pci_allocate_raw(self._h, reqs.ctypes.data, len(reqs), C.byref(arg),
+                                                first_bad.ctypes.data, panic.ctypes.data, kept.ctypes.data,
+                                                take.ctypes.data))
+        return first_bad, panic.astype(bool), kept.astype(bool), take.astype(bool)
+
     def preferred_allocation(self, ids, n_must, n_avail, sizes) -> list:
         """GetPreferredAllocation's NUMA packing for every container request of one call, one launch
         (include/kvgpu.h kvg_preferred_allocation).  ids: PREF_ID entries, request after request, each request's

@@ -290,6 +290,71 @@ def read_pci_tree_raw(base_path: str) -> PciRaw:
                   np.array(state, dtype=np.uint16))
 
 
+NOT_READ = "not read"   # a read that was not made (pack_alloc_raw); the library refuses one the reference reaches
+
+
+@dataclass
+class AllocRaw:
+    """The raw reads of one AllocateRequest (include/kvgpu.h kvg_alloc_raw), undecoded.  n_members / n_ids: one count
+    per container request; member_off / member_bytes / member_state: per member the iommu_group link target, the
+    vendor contents and the group string the maps hold; id_off / id_bytes: the DevicesIDs; egm_off / egm_bytes /
+    egm_state: per EGM class entry its name and gpu_devices contents, and the made / failed bits of both reads and of
+    the Stat of its device node."""
+    n_members: np.ndarray   # u32 [n_reqs]
+    n_ids: np.ndarray       # u32 [n_reqs]
+    member_off: np.ndarray  # u32 [n * AMEM_FIELDS + 1]
+    member_bytes: bytes
+    member_state: np.ndarray  # u16 [n]
+    id_off: np.ndarray      # u32 [n_ids + 1]
+    id_bytes: bytes
+    egm_off: np.ndarray     # u32 [n_egm * AEGM_FIELDS + 1]
+    egm_bytes: bytes
+    egm_state: np.ndarray   # u16 [n_egm]
+
+
+def _offsets(parts) -> np.ndarray:
+    off = np.zeros(len(parts) + 1, dtype=np.int64)
+    np.cumsum([len(p) for p in parts], out=off[1:])
+    if off[-1] > 0xFFFFFFFF:
+        raise ValueError("the raw reads exceed 4 GiB")
+    return off.astype(np.uint32)
+
+
+def pack_alloc_raw(requests, egm_entries) -> AllocRaw:
+    """requests: [(members, ids)] in request order, members = [(link target, vendor contents, group string)] in the
+    order the reference visits them, ids = the DevicesIDs; egm_entries: [(name, gpu_devices contents, stat ok)] in
+    ReadDir order.  A read is bytes (what it returned), None (it failed) or NOT_READ; a stat is True (it succeeded),
+    False (it failed) or NOT_READ.  Strings are encoded with os.fsencode, the bytes Go holds for them."""
+    enc = lambda v: os.fsencode(v) if isinstance(v, str) else v   # noqa: E731
+    mparts, mstate, iparts, n_members, n_ids = [], [], [], [], []
+    for members, ids in requests:
+        for link, vendor, group in members:
+            st = 0
+            for f, v in ((L.AMEM_LINK, link), (L.AMEM_VENDOR, vendor)):
+                if v is not NOT_READ:
+                    st |= 1 << f
+                    if v is None:
+                        st |= 1 << (8 + f)
+            mparts += [enc(link) if isinstance(link, (bytes, str)) else b"",
+                       enc(vendor) if isinstance(vendor, (bytes, str)) else b"", enc(group)]
+            mstate.append(st)
+        iparts += [enc(b) for b in ids]
+        n_members.append(len(members))
+        n_ids.append(len(ids))
+    eparts, estate = [], []
+    for name, gpus, stat in egm_entries:
+        st = 0
+        if gpus is not NOT_READ:
+            st |= 1 << L.AEGM_GPUS | (1 << (8 + L.AEGM_GPUS) if gpus is None else 0)
+        if stat is not NOT_READ:
+            st |= 1 << L.AEGM_STAT | (0 if stat else 1 << (8 + L.AEGM_STAT))
+        eparts += [enc(name), enc(gpus) if isinstance(gpus, (bytes, str)) else b""]
+        estate.append(st)
+    return AllocRaw(np.array(n_members, dtype=np.uint32), np.array(n_ids, dtype=np.uint32), _offsets(mparts),
+                    b"".join(mparts), np.array(mstate, dtype=np.uint16), _offsets(iparts), b"".join(iparts),
+                    _offsets(eparts), b"".join(eparts), np.array(estate, dtype=np.uint16))
+
+
 def snapshot_pci_ids(base_path: str, bdfs, intern: dict) -> PciSnapshot:
     """Snapshot the PCI devices `bdfs` in THAT order (the health re-scan's fixed record order; a Walk would re-index
     when one vanishes), with the readers and flag rules of snapshot_pci_tree.  An address whose entry is gone reads as

@@ -39,7 +39,7 @@ from . import _lib as L
 from . import dpapi
 from .plugin import (DEVICE_NAMESPACE, GPU_PREFIX, VGPU_PREFIX, Maps, PluginSpec, ReferencePanic, _read_id,
                      _read_link, _read_vgpu_raw, _rebuild_mdev_maps, _rebuild_pci_maps, apply_mdev_delta,
-                     apply_pci_delta, format_uuid, parse_bdf, plugin_specs_from_maps)
+                     apply_pci_delta, format_uuid, pack_alloc_raw, parse_bdf, plugin_specs_from_maps)
 
 VFIO_DEVICE_PATH = "/dev/vfio"      # generic_device_plugin.go:54
 IOMMU_DEVICE_PATH = "/dev/iommu"    # :55
@@ -163,6 +163,42 @@ def egm_paths_for_allocated_gpus(allocated_bdfs, egm_devices) -> list:
     allocated = {egm_key(b) for b in allocated_bdfs}
     return sorted(e.dev_path for e in (egm_devices or [])
                   if all(egm_key(g) in allocated for g in e.gpu_bdfs))
+
+
+@dataclass
+class EGMEntryRaw:
+    """One entry of the EGM class directory as discoverEGMDevicesFunc's reads returned it (:120-157), undecoded:
+    gpu_devices is the file's bytes, None when the read failed, or plugin.NOT_READ; stat is whether os.Stat of
+    /dev/<name> succeeded, or plugin.NOT_READ."""
+    name: bytes
+    gpu_devices: object
+    stat: object
+
+
+def discover_egm_raw(root_path: str = "/") -> list:
+    """The reads of discoverEGMDevicesFunc :120-157, decoding nothing: every entry of the EGM class directory in
+    ReadDir order (sorted by name bytes), its gpu_devices contents and the Stat of its device node, each made for every
+    entry (the GPU decides which the reference reaches).  A missing class directory is no entry (:124-126); any other
+    listing error raises, so that Allocate continues without EGM mounts (:366-370)."""
+    class_dir = os.fsencode(os.path.join(root_path, EGM_CLASS_PATH.lstrip("/")))
+    try:
+        names = sorted(os.listdir(class_dir))
+    except FileNotFoundError:
+        return []
+    out = []
+    for name in names:
+        try:
+            with open(os.path.join(class_dir, name, b"gpu_devices"), "rb") as f:
+                gpus = f.read()
+        except OSError:
+            gpus = None
+        try:
+            os.stat(os.path.join(os.fsencode(root_path), DEVICE_DIR.lstrip("/").encode(), name))
+            stat = True
+        except OSError:
+            stat = False
+        out.append(EGMEntryRaw(name, gpus, stat))
+    return out
 
 
 def supports_iommufd(root_path: str = "/") -> bool:
@@ -359,6 +395,48 @@ class AllocateCheck:
             panic = panics.get(at + bad) if bad is not None and link_ok[at + bad] else None
             out.append((bad, panic, sorted(e.dev_path for e, t in zip(egm_devices, take[r]) if t)))
             at += n
+        return out
+
+
+class AllocateRawCheck:
+    """The passthrough plugin's Allocate decisions (generic_device_plugin.go:352-444) for every container request of
+    one AllocateRequest, decided on the GPU from the raw reads: a drop-in `allocate_check` for GenericDevicePlugin with
+    AllocateCheck's contract, whose `discover_egm` is discover_egm_raw.  AllocateCheck stays as the reference it is
+    tested against.
+
+    Every member's iommu_group link target and vendor contents are read raw, in the reference's order; with the group
+    string the maps hold for the member, the DevicesIDs and the EGM class entries they go to ONE `call`
+    (Context.pci_allocate_raw), which decodes, compares and matches them all.  Nothing is decoded or interned here:
+    what the call returns is mapped back to (bad, panic, egm_paths) per request."""
+
+    def __init__(self, call, base_path: str = "/sys/bus/pci/devices"):
+        self.call, self.base_path = call, base_path
+
+    def _read(self, addr, prop, link):
+        path = os.path.join(os.fsencode(self.base_path), os.fsencode(addr), prop)
+        try:
+            if link:
+                return os.readlink(path)
+            with open(path, "rb") as f:
+                return f.read()
+        except OSError:
+            return None
+
+    def __call__(self, requests, egm_entries) -> list:
+        """requests: [(pairs, devices_ids)] as for AllocateCheck; egm_entries: discover_egm_raw's entries (None or []
+        for none).  Returns per request (bad, panic, egm_paths) as AllocateCheck does."""
+        egm = list(egm_entries or [])
+        raw = pack_alloc_raw(
+            [([(self._read(addr, b"iommu_group", True), self._read(addr, b"vendor", False), group)
+               for addr, group in pairs], list(devices_ids)) for pairs, devices_ids in requests],
+            [(e.name, e.gpu_devices, e.stat) for e in egm])
+        first_bad, panic, kept, take = self.call(raw)
+        out = []
+        for r, (pairs, _) in enumerate(requests):
+            bad = None if int(first_bad[r]) == len(pairs) else int(first_bad[r])
+            p = (ReferencePanic("slice bounds out of range reading %s/vendor" % pairs[bad][0]) if panic[r] else None)
+            names = sorted(e.name for e, k, t in zip(egm, kept, take[r]) if k and t)
+            out.append((bad, p, [os.path.join(DEVICE_DIR, os.fsdecode(n)) for n in names]))
         return out
 
 
