@@ -29,6 +29,8 @@
  *                                            readNUMANodeFunc :304-320
  *   kvg_scan_pci_delta                   <- (no reference equivalent: the reference never re-scans)
  *   kvg_scan_mdev_delta                   <- (no reference equivalent: createVgpuIDMap runs once)
+ *   kvg_scan_pci_raw_delta                <- (no reference equivalent: the reference never re-scans)
+ *   kvg_scan_mdev_raw_delta               <- (no reference equivalent: the reference never re-scans)
  *   kvg_comm_*, kvg_scan_pci_sharded      <- (no reference equivalent; BASELINE.json config 4)
  *   kvg_dev_scan_pci_shard_fetch_delta    <- (no reference equivalent: the re-scan delta of the sharded scan)
  *   kvg_dev_scan_mdev_shard_fetch_delta   <- (no reference equivalent: the re-scan delta of the sharded vGPU scan)
@@ -781,6 +783,49 @@ int kvg_scan_pci_delta(kvg_ctx *ctx, const kvg_pci_rec *recs, size_t n, kvg_pci_
 /* forget the previous result: the next kvg_scan_pci_delta reports everything as added */
 int kvg_scan_pci_delta_reset(kvg_ctx *ctx);
 
+/* kvg_scan_pci_raw on `raw`, and the keyed diff of its result against the previous one, keyed by ENTRY NAME (the
+ * KVG_RAW_NAME bytes), so that it is exact in every snapshot mode.
+ *
+ * *res and *snap are byte for byte what kvg_scan_pci_raw(ctx, raw, ...) returns, with the same errors and refusals;
+ * *res, *snap and *delta are all freed with kvg_result_free.
+ *
+ * "Previous" is the result and snapshot of the last SUCCESSFUL kvg_scan_pci_raw_delta on this context since
+ * kvg_ctx_create or kvg_scan_pci_raw_delta_reset; before any such call it is empty (and numeric).  The library keeps
+ * its own copy, strings included, in a slot no other call touches: kvg_scan_pci_delta, the sharded deltas, the raw
+ * scans, the health calls, the Allocate calls, kvg_pciids_load and every other reset leave it unchanged, and this
+ * call changes no other delta's.  A refused call hands out nothing and leaves the previous result as it was.
+ *
+ * Identity: a survivor is its entry name.  Survivor names must ascend strictly byte-wise (Walk order does); this is
+ * checked on the device, and a violation returns KVG_EINVAL with text in kvg_last_error, state unchanged.
+ * kvg_scan_pci_raw accepts such input, but a delta is undefined without an order.
+ *
+ * changes: one per name that survives on exactly one side, or on both with another iommu_group string
+ * (KVG_CH_GROUP), another device string (KVG_CH_DEVICE) or another clamped NUMA node (KVG_CH_NUMA), ascending by
+ * name.  Strings are compared as strings: "042" is not "42", and "1db6" then "1DB6" is a change.
+ *   addr                 this snapshot's address handle when the name survives now, else the previous snapshot's
+ *   prev_* / now_*       each side in its own snapshot's encoding: the number in numeric mode, else a handle into
+ *                        that snapshot's string table; 0 on the absent side
+ *   now_index/prev_index as in kvg_scan_pci_delta
+ * dev_dirty / grp_dirty: deviceMap (iommuMap) key k, indexing res->dev_keys (res->grp_keys), is dirty iff the
+ * (entry name, clamped NUMA) sequence of its members, in Walk order, differs between the two results, keys being
+ * matched by string; new keys are dirty.  dev_gone / grp_gone: the previous result's keys whose string has no
+ * survivor now, in the previous snapshot's encoding, ascending.  The caller names a removed entry or a gone key
+ * through the previous kvg_pci_snap, so it keeps that snapshot until the next call returns.
+ *
+ * Both snapshots fully numeric (packed_addr, groups_numeric and devices_numeric on both sides): *delta is byte for
+ * byte what kvg_scan_pci_delta(snap->recs) returns for the same pair, from the same two kernels on the decoded
+ * records.
+ *
+ * Cost beyond kvg_scan_pci_raw on the same input: numeric pair, the two launches of kvg_scan_pci_delta
+ * (delta_merge, delta_lists) and one synchronisation; any other mode pair adds two re-key launches (raw_rekey: name
+ * ranks, key indices and the new keys' string table; raw_xlate: each previous key to the new key with its string).
+ * A snapshot with a column in index mode also has its staged walk copied, device to device, into the slot (the next
+ * call's re-key reads its strings); a fully numeric one copies nothing beyond the survivors and keys. */
+int kvg_scan_pci_raw_delta(kvg_ctx *ctx, const kvg_pci_raw *raw, kvg_pci_result **res, kvg_pci_snap **snap,
+                           kvg_pci_delta **delta);
+/* forget the previous result: the next kvg_scan_pci_raw_delta reports everything as added */
+int kvg_scan_pci_raw_delta_reset(kvg_ctx *ctx);
+
 /* Scan mdev `recs` with dictionary `types` and diff the result against the previous one, keyed by survivor UUID.
  *
  * *res is byte for byte what kvg_scan_mdev(ctx, recs, n, types, ...) returns for the same input, dictionary arrays
@@ -816,6 +861,30 @@ int kvg_scan_mdev_delta(kvg_ctx *ctx, const kvg_mdev_rec *recs, size_t n, const 
                         kvg_mdev_result **res, kvg_mdev_delta **delta);
 /* forget the previous result: the next kvg_scan_mdev_delta reports everything as added */
 int kvg_scan_mdev_delta_reset(kvg_ctx *ctx);
+
+/* kvg_scan_mdev_raw on `raw`, and the keyed diff of its result against the previous one, keyed by ENTRY NAME (the
+ * KVG_MRAW_NAME bytes, the UUID string), so that it is exact in every snapshot mode.  The contract is that of
+ * kvg_scan_pci_raw_delta with these differences:
+ *   - *res and *snap are byte for byte what kvg_scan_mdev_raw returns; its slot is its own (kvg_scan_mdev_delta, the
+ *     sharded deltas, the raw scans, the health calls, the Allocate calls and kvg_scan_pci_raw_delta leave it alone).
+ *   - changes: one per name that survives on one side only, or on both with another sanitised type label
+ *     (KVG_CH_TYPE, as kvg_scan_mdev_delta compares it), another decoded parent string (KVG_CH_PARENT) or another
+ *     clamped NUMA node, ascending by name.  uuid is the record's uuid bytes from the side the handle comes from (this
+ *     snapshot when the name survives now); prev_parent / now_parent are each side's own encoding (packed BDF or a
+ *     handle into that snapshot's parent table); prev_type / now_type are canonical ids of each side's dictionary.
+ *   - type_dirty / type_gone keep their meaning (by label).  par_dirty: gpuVgpuMap key k, indexing res->par_keys, is
+ *     dirty iff the entry-name sequence of its members changed, parents matched by string; par_gone lists previous
+ *     parent keys whose string has no survivor now, in the previous snapshot's encoding, ascending.
+ *   - Both snapshots fully numeric (uuid_ok and parents_packed on both sides): *delta is byte for byte what
+ *     kvg_scan_mdev_delta(snap->recs, dict) returns for the same pair.
+ *   - Survivor names must ascend strictly byte-wise (checked on the device: KVG_EINVAL, state unchanged).
+ * Cost beyond kvg_scan_mdev_raw: numeric pair, the three launches of kvg_scan_mdev_delta (mdev_delta_types,
+ * mdev_delta_merge, mdev_delta_lists) and one synchronisation; any other mode pair adds the two re-key launches
+ * (raw_rekey, raw_xlate). */
+int kvg_scan_mdev_raw_delta(kvg_ctx *ctx, const kvg_mdev_raw *raw, kvg_mdev_result **res, kvg_mdev_snap **snap,
+                            kvg_mdev_delta **delta);
+/* forget the previous result: the next kvg_scan_mdev_raw_delta reports everything as added */
+int kvg_scan_mdev_raw_delta_reset(kvg_ctx *ctx);
 
 /* ---- device-resident entry points (inputs already in HBM; used by bench.py "value") -------- */
 

@@ -12,6 +12,9 @@
 //   k_delta_lists      the four key lists (dirty / gone of both maps) from those tags: one look-back compaction per
 //                      list (blockIdx.y) through the same tile body
 //   k_mdev_delta_types the previous result's type keys in the new key space: same sanitised label, or none
+//   k_raw_rekey<MDEV>, k_raw_xlate<MDEV>  kvg_scan_pci_raw_delta / kvg_scan_mdev_raw_delta outside the all-numeric
+//                      pair: both snapshots' survivors onto the entry-name space they share (PciRawDeltaRec /
+//                      MdevRawDeltaRec), and each previous key to the new key with the same string
 #pragma once
 #include "../../include/kvgpu.h"
 #include "kvg_common.cuh"
@@ -69,6 +72,18 @@ struct DeltaKeys {
       else if ((k = delta_find(keys_prev, n_prev, prev_key)) != DELTA_NONE)
         flag_prev[k] = tag;
     }
+  }
+  // mark<true> when both keys are already indices into keys_now / keys_prev (the re-keyed raw delta): no searches
+  __device__ __forceinline__ void mark_index(bool has_now, uint32_t now_k, bool has_prev, uint32_t prev_k,
+                                             uint32_t tag) const {
+    if (has_now) flag_now[now_k] = tag;
+    if (!has_prev) return;
+    const uint32_t same = __ldg(&xlate[prev_k]);
+    if (has_now && same == now_k) return;
+    if (same != DELTA_NONE)
+      flag_now[same] = tag;
+    else
+      flag_prev[prev_k] = tag;
   }
 };
 
@@ -161,6 +176,71 @@ struct MdevDeltaRec {
     if (what & (KVG_CH_ADDED | KVG_CH_REMOVED | KVG_CH_TYPE | KVG_CH_NUMA))
       type.mark<true>(hn, q.hi.y & 0xffffu, hp, p.hi.y & 0xffffu, tag);
     if (what & (KVG_CH_ADDED | KVG_CH_REMOVED | KVG_CH_PARENT)) par.mark(hn, q.hi.x, hp, p.hi.x, tag);
+  }
+};
+
+// The re-keyed PCI survivor of kvg_scan_pci_raw_delta (k_raw_rekey): {name rank, index of its group in the side's
+// grp_keys, index of its device id in the side's dev_keys | numa << 16, the side's own address handle}; key = the
+// name rank, which two snapshots share.  A previous key index goes to the new key index with the same string through
+// DeltaKeys::xlate: k0.xlate is the whole table (previous device indices from 0, previous group indices from
+// RAW_XLATE_GROUP), so that diff, which sees k0 only, reads both; k1.xlate points at the group part.
+constexpr uint32_t RAW_XLATE_GROUP = 65536;
+struct PciRawDeltaRec : PciDeltaRec {
+  __device__ __forceinline__ static uint32_t diff(const Rec& p, const Rec& q, const DeltaKeys& dev) {
+    const uint32_t* xl = dev.xlate;
+    return (__ldg(&xl[RAW_XLATE_GROUP + p.y]) != q.y ? (uint32_t)KVG_CH_GROUP : 0u) |
+           (__ldg(&xl[p.z & 0xffffu]) != (q.z & 0xffffu) ? (uint32_t)KVG_CH_DEVICE : 0u) |
+           ((p.z >> 16) != (q.z >> 16) ? (uint32_t)KVG_CH_NUMA : 0u);
+  }
+  // kvg_pci_change with each side's own handles: the new address when the name survives now, else the previous one
+  __device__ __forceinline__ static void emit(uint4* out, uint32_t pos, uint32_t what, bool hp, bool hn, uint32_t a,
+                                              uint32_t b, const Rec& p, const Rec& q, const DeltaKeys& dev,
+                                              const DeltaKeys& grp, uint32_t tag) {
+    const uint32_t pg = hp ? __ldg(&grp.keys_prev[p.y]) : 0u, ng = hn ? __ldg(&grp.keys_now[q.y]) : 0u;
+    const uint32_t pd = hp ? __ldg(&dev.keys_prev[p.z & 0xffffu]) : 0u, nd = hn ? __ldg(&dev.keys_now[q.z & 0xffffu]) : 0u;
+    st_stream(out + 2 * (size_t)pos, make_uint4(hn ? q.w : p.w, what, pg, ng));
+    st_stream(out + 2 * (size_t)pos + 1, make_uint4(pd | (nd << 16), (p.z >> 16) | (q.z & 0xffff0000u), b, a));
+    mark(what, hp, hn, p, q, dev, grp, tag);
+  }
+  __device__ __forceinline__ static void mark(uint32_t what, bool hp, bool hn, const Rec& p, const Rec& q,
+                                              const DeltaKeys& dev, const DeltaKeys& grp, uint32_t tag) {
+    if (what & (KVG_CH_ADDED | KVG_CH_REMOVED | KVG_CH_DEVICE | KVG_CH_NUMA))
+      dev.mark_index(hn, q.z & 0xffffu, hp, p.z & 0xffffu, tag);
+    if (what & (KVG_CH_ADDED | KVG_CH_REMOVED | KVG_CH_GROUP | KVG_CH_NUMA)) grp.mark_index(hn, q.y, hp, p.y, tag);
+  }
+};
+
+// The re-keyed mdev survivor of kvg_scan_mdev_raw_delta: lo = the UUID bytes, hi = {index of its parent in the side's
+// par_keys, canonical type id | numa << 16, name rank, 0}; key = the name rank.  k0.xlate is the table of the merge:
+// previous canonical type ids -> new ones by label (k_mdev_delta_types) from 0, previous parent indices -> new ones
+// by string from RAW_XLATE_GROUP; k1.xlate points at the parent part.
+struct MdevRawDeltaRec : MdevDeltaRec {
+  using Key = uint32_t;
+  __device__ __forceinline__ static Key key(const Rec& r) { return r.hi.z; }
+  __device__ __forceinline__ static Key key_at(const Rec* list, uint32_t i) { return __ldg(&list[i].hi.z); }
+  __device__ __forceinline__ static bool le(Key a, Key b) { return a <= b; }
+  __device__ __forceinline__ static bool eq(Key a, Key b) { return a == b; }
+  __device__ __forceinline__ static uint32_t diff(const Rec& p, const Rec& q, const DeltaKeys& type) {
+    const uint32_t* xl = type.xlate;
+    return (__ldg(&xl[p.hi.y & 0xffffu]) != (q.hi.y & 0xffffu) ? (uint32_t)KVG_CH_TYPE : 0u) |
+           (__ldg(&xl[RAW_XLATE_GROUP + p.hi.x]) != q.hi.x ? (uint32_t)KVG_CH_PARENT : 0u) |
+           ((p.hi.y >> 16) != (q.hi.y >> 16) ? (uint32_t)KVG_CH_NUMA : 0u);
+  }
+  // kvg_mdev_change with each side's own parent handles: the new UUID bytes when the name survives now
+  __device__ __forceinline__ static void emit(uint4* out, uint32_t pos, uint32_t what, bool hp, bool hn, uint32_t a,
+                                              uint32_t b, const Rec& p, const Rec& q, const DeltaKeys& type,
+                                              const DeltaKeys& par, uint32_t tag) {
+    const uint32_t pp = hp ? __ldg(&par.keys_prev[p.hi.x]) : 0u, np = hn ? __ldg(&par.keys_now[q.hi.x]) : 0u;
+    st_stream(out + 3 * (size_t)pos, hn ? q.lo : p.lo);
+    st_stream(out + 3 * (size_t)pos + 1, make_uint4(what, pp, np, (p.hi.y & 0xffffu) | (q.hi.y << 16)));
+    st_stream(out + 3 * (size_t)pos + 2, make_uint4((p.hi.y >> 16) | (q.hi.y & 0xffff0000u), b, a, 0u));
+    mark(what, hp, hn, p, q, type, par, tag);
+  }
+  __device__ __forceinline__ static void mark(uint32_t what, bool hp, bool hn, const Rec& p, const Rec& q,
+                                              const DeltaKeys& type, const DeltaKeys& par, uint32_t tag) {
+    if (what & (KVG_CH_ADDED | KVG_CH_REMOVED | KVG_CH_TYPE | KVG_CH_NUMA))
+      type.mark<true>(hn, q.hi.y & 0xffffu, hp, p.hi.y & 0xffffu, tag);
+    if (what & (KVG_CH_ADDED | KVG_CH_REMOVED | KVG_CH_PARENT)) par.mark_index(hn, q.hi.x, hp, p.hi.x, tag);
   }
 };
 
@@ -554,6 +634,222 @@ __global__ void __launch_bounds__(XMAP_THREADS) k_mdev_delta_types(MdevTypeLabel
     }
     xlate[c] = to;
   }
+}
+
+// ---- the re-key of kvg_scan_pci_raw_delta / kvg_scan_mdev_raw_delta: two snapshots in any mode pair onto the name
+// space they share ---------------------------------------------------------------------------------------------------
+//   k_raw_rekey  one thread per survivor of either side: the name's merge-path rank (its index plus the other side's
+//                names below it, by binary search), the indices of its keys among its side's keys, the strict ascent
+//                of the new names; and one thread per new key of a string-keyed map: into that map's table
+//   k_raw_xlate  one thread per previous key of a string-keyed map: the new key index with the same string, or
+//                DELTA_NONE
+// PCI: both maps are string-keyed (device ids, groups).  mdev: the survivor keeps its canonical type id (vGpuMap keys
+// are translated by label, k_mdev_delta_types) and only the parents (gpuVgpuMap) go through the tables.
+// A string is either bytes the walk read or, in a numeric column, the canonical formatting of the number, produced
+// one character at a time so that nothing is materialised.
+enum : uint32_t { RSTR_BYTES, RSTR_DEC, RSTR_HEX4, RSTR_BDF, RSTR_UUID };
+struct RawStr {
+  const uint8_t* p;
+  uint32_t len, v, kind;
+};
+__device__ __forceinline__ uint8_t rstr_hex(uint32_t d) { return (uint8_t)(d < 10 ? '0' + d : 'a' + d - 10); }
+__device__ __forceinline__ uint8_t rstr_at(const RawStr& s, uint32_t i) {
+  if (s.kind == RSTR_BYTES) return __ldg(&s.p[i]);
+  if (s.kind == RSTR_HEX4) return rstr_hex((s.v >> (4 * (3 - i))) & 15u);
+  if (s.kind == RSTR_DEC) {
+    uint32_t v = s.v;
+    for (uint32_t k = i + 1; k < s.len; k++) v /= 10;
+    return (uint8_t)('0' + v % 10);
+  }
+  if (s.kind == RSTR_UUID) {  // 8-4-4-4-12 lower-case hex of the 16 bytes at p
+    if (i == 8 || i == 13 || i == 18 || i == 23) return '-';
+    const uint32_t h = i - (i > 8) - (i > 13) - (i > 18) - (i > 23);
+    const uint32_t b = __ldg(&s.p[h >> 1]);
+    return rstr_hex((h & 1) ? b & 15u : b >> 4);
+  }
+  // "dddd:bb:dd.f" of domain << 16 | bus << 8 | dev << 3 | fn (kvg_snap.cuh raw_bdf)
+  if (i == 4 || i == 7) return ':';
+  if (i == 10) return '.';
+  const uint32_t f = i < 4 ? s.v >> 16 : i < 7 ? (s.v >> 8) & 0xffu : i < 10 ? (s.v >> 3) & 31u : s.v & 7u;
+  const uint32_t w = i < 4 ? 3 - i : i < 7 ? 6 - i : i < 10 ? 9 - i : 0;
+  return rstr_hex((f >> (4 * w)) & 15u);
+}
+__device__ __forceinline__ RawStr rstr_dec(uint32_t v) {
+  uint32_t len = 1;
+  for (uint32_t x = v; x >= 10; x /= 10) len++;
+  return {nullptr, len, v, RSTR_DEC};
+}
+// byte-wise order: <0, 0, >0
+__device__ __forceinline__ int rstr_cmp(const RawStr& a, const RawStr& b) {
+  const uint32_t m = min(a.len, b.len);
+  for (uint32_t i = 0; i < m; i++) {
+    const uint32_t x = rstr_at(a, i), y = rstr_at(b, i);
+    if (x != y) return x < y ? -1 : 1;
+  }
+  return a.len < b.len ? -1 : a.len > b.len ? 1 : 0;
+}
+__device__ __forceinline__ uint64_t rstr_fnv(const RawStr& s) {
+  uint64_t h = 1469598103934665603ull;
+  for (uint32_t i = 0; i < s.len; i++) h = (h ^ rstr_at(s, i)) * 1099511628211ull;
+  return h;
+}
+
+// One snapshot's survivors and the strings behind them.  Map m: PCI 0 = deviceMap, 1 = iommuMap; mdev 0 = vGpuMap
+// (no keys here), 1 = gpuVgpuMap.
+enum : uint32_t { RAW_NUM_ADDR = 1u, RAW_NUM_DEVICE = 2u, RAW_NUM_GROUP = 4u };  // mdev: UUID names, -, parents
+struct RawDeltaSide {
+  const uint4* surv;        // kvg_pci_surv (PCI) or kvg_mdev_surv (mdev, two uint4), Walk order
+  uint32_t n;
+  const uint32_t* off;      // the walk's offsets and bytes: the names and key strings in index mode (NULL when numeric)
+  const uint8_t* bytes;
+  const uint2* tab[2];      // handle -> span in bytes of the map's key strings in index mode
+  const uint32_t* keys[2];  // the distinct keys of the side's result
+  uint32_t n_keys[2];
+  uint32_t numeric;         // RAW_NUM_*: the columns in numeric mode
+
+  __device__ __forceinline__ RawStr span_str(uint2 s) const { return {bytes + s.x, s.y - s.x, 0u, RSTR_BYTES}; }
+  __device__ __forceinline__ RawStr walk_name(uint32_t w, uint32_t fields) const {
+    const uint32_t* o = off + (size_t)w * fields;
+    return span_str(make_uint2(__ldg(&o[0]), __ldg(&o[1])));
+  }
+  template <bool MDEV>
+  __device__ __forceinline__ RawStr name(uint32_t i) const {
+    if constexpr (MDEV) {  // the UUID bytes of a canonical snapshot, else the name at the Walk index `src`
+      if (numeric & RAW_NUM_ADDR) return {reinterpret_cast<const uint8_t*>(surv + 2 * (size_t)i), 36u, 0u, RSTR_UUID};
+      return walk_name(__ldg(&surv[2 * (size_t)i + 1].z), KVG_MRAW_FIELDS);
+    } else {
+      const uint32_t addr = __ldg(&surv[i].x);
+      if (numeric & RAW_NUM_ADDR) return {nullptr, 12u, addr, RSTR_BDF};
+      return walk_name(addr, KVG_RAW_FIELDS);
+    }
+  }
+  template <bool MDEV>
+  __device__ __forceinline__ RawStr key(uint32_t m, uint32_t h) const {
+    if (m == 0) return (numeric & RAW_NUM_DEVICE) ? RawStr{nullptr, 4u, h, RSTR_HEX4} : span_str(__ldg(&tab[0][h]));
+    if (numeric & RAW_NUM_GROUP) return MDEV ? RawStr{nullptr, 12u, h, RSTR_BDF} : rstr_dec(h);
+    return span_str(__ldg(&tab[1][h]));
+  }
+};
+
+constexpr uint32_t REKEY_THREADS = 256;
+struct RawRekeyArgs {
+  RawDeltaSide side[2];  // previous, new
+  uint4* out[2];         // PciRawDeltaRec / MdevRawDeltaRec survivors of each side
+  uint64_t* table[2];    // per map: the new keys, slot = tag << 32 | key index (another call's tag: free)
+  uint32_t mask[2];
+  uint32_t tag;
+  uint32_t* xlate;       // the merge's table: map 0 from 0 (PCI), map 1 from RAW_XLATE_GROUP
+  ScanCtrl* ctrl;        // reserved2[DELTA_W_ERROR]: the new names do not ascend strictly
+};
+
+template <bool MDEV>
+__global__ void __launch_bounds__(REKEY_THREADS) k_raw_rekey(RawRekeyArgs a) {
+  pdl_enter();
+  const uint32_t t = blockIdx.x * REKEY_THREADS + threadIdx.x;
+  const uint32_t n0 = a.side[0].n;
+  if (t < n0 + a.side[1].n) {
+    const uint32_t s = t < n0 ? 0 : 1, i = s ? t - n0 : t;
+    const RawDeltaSide& me = a.side[s];
+    const RawDeltaSide& other = a.side[s ^ 1];
+    const RawStr nm = me.name<MDEV>(i);
+    uint32_t lo = 0, hi = other.n;  // the other side's names below this one
+    while (lo < hi) {
+      const uint32_t mid = (lo + hi) >> 1;
+      if (rstr_cmp(other.name<MDEV>(mid), nm) < 0)
+        lo = mid + 1;
+      else
+        hi = mid;
+    }
+    if (s == 1 && i > 0 && rstr_cmp(me.name<MDEV>(i - 1), nm) >= 0) a.ctrl->reserved2[DELTA_W_ERROR] = 1u;
+    if constexpr (MDEV) {  // {uuid bytes}, {parent index, type_key | numa << 16, rank, 0}
+      const uint4 u = __ldg(&me.surv[2 * (size_t)i]), r = __ldg(&me.surv[2 * (size_t)i + 1]);
+      a.out[s][2 * (size_t)i] = u;
+      a.out[s][2 * (size_t)i + 1] = make_uint4(delta_find(me.keys[1], me.n_keys[1], r.x), r.y, i + lo, 0u);
+    } else {
+      const uint4 r = __ldg(&me.surv[i]);
+      const uint32_t gi = delta_find(me.keys[1], me.n_keys[1], r.y);
+      const uint32_t di = delta_find(me.keys[0], me.n_keys[0], r.z & 0xffffu);
+      a.out[s][i] = make_uint4(i + lo, gi, di | (r.z & 0xffff0000u), r.x);
+    }
+  }
+  const RawDeltaSide& now = a.side[1];
+  const uint64_t mine = (uint64_t)a.tag << 32;
+  for (uint32_t m = MDEV ? 1 : 0; m < 2; m++) {
+    if (t >= now.n_keys[m]) continue;
+    unsigned long long* cas = reinterpret_cast<unsigned long long*>(a.table[m]);
+    bool placed = false;
+    for (uint32_t s = (uint32_t)rstr_fnv(now.key<MDEV>(m, __ldg(&now.keys[m][t]))) & a.mask[m]; !placed;
+         s = (s + 1) & a.mask[m]) {
+      uint64_t w = ld_relaxed_u64(a.table[m] + s);
+      while (!placed && (uint32_t)(w >> 32) != a.tag) {
+        const uint64_t seen = atomicCAS(cas + s, (unsigned long long)w, (unsigned long long)(mine | t));
+        placed = seen == w;
+        w = seen;
+      }
+    }
+  }
+}
+
+template <bool MDEV>
+__global__ void __launch_bounds__(REKEY_THREADS) k_raw_xlate(RawRekeyArgs a) {
+  pdl_enter();
+  const uint32_t t = blockIdx.x * REKEY_THREADS + threadIdx.x;
+  const RawDeltaSide &prev = a.side[0], &now = a.side[1];
+  uint32_t m = 1, k = t;  // mdev: parents only
+  if constexpr (!MDEV) {
+    m = t < prev.n_keys[0] ? 0 : 1;
+    k = m ? t - prev.n_keys[0] : t;
+  }
+  if (k >= prev.n_keys[m]) return;
+  const RawStr want = prev.key<MDEV>(m, __ldg(&prev.keys[m][k]));
+  uint32_t to = DELTA_NONE;
+  for (uint32_t s = (uint32_t)rstr_fnv(want) & a.mask[m];; s = (s + 1) & a.mask[m]) {
+    const uint64_t w = ld_relaxed_u64(a.table[m] + s);
+    if ((uint32_t)(w >> 32) != a.tag) break;  // free: no new key has this string
+    const uint32_t j = (uint32_t)w;
+    if (rstr_cmp(now.key<MDEV>(m, __ldg(&now.keys[m][j])), want) == 0) {
+      to = j;
+      break;
+    }
+  }
+  a.xlate[(m ? RAW_XLATE_GROUP : 0u) + k] = to;
+}
+
+// The launch arguments, built on the host by kvg_api_delta.inc and by the CPU emulator alike.
+// Both snapshots fully numeric: the plain merge on the decoded survivors, no re-key
+inline bool raw_rekey_needed(uint32_t prev_numeric, uint32_t now_numeric, uint32_t all) {
+  return prev_numeric != all || now_numeric != all;
+}
+// the two sides' survivors re-keyed into `rekeyed` (the previous side first; mdev: two uint4 per survivor), the key
+// tables of the string-keyed maps at `table` (raw_rekey_table_words of it), the translation into `xlate` (at least
+// RAW_XLATE_GROUP + the previous side's map-1 keys); returns the grids of k_raw_rekey and k_raw_xlate
+template <bool MDEV>
+inline RawRekeyArgs raw_rekey_args(const RawDeltaSide& prev, const RawDeltaSide& now, uint4* rekeyed, uint64_t* table,
+                                   uint32_t* xlate, uint32_t tag, ScanCtrl* ctrl, uint32_t* grid_rekey,
+                                   uint32_t* grid_xlate) {
+  RawRekeyArgs a = {};
+  a.side[0] = prev;
+  a.side[1] = now;
+  a.mask[0] = MDEV ? 0u : delta_xmap_mask(now.n_keys[0]);
+  a.mask[1] = delta_xmap_mask(now.n_keys[1]);
+  a.out[0] = rekeyed;
+  a.out[1] = rekeyed + (MDEV ? 2 : 1) * (size_t)prev.n;
+  a.table[0] = table;
+  a.table[1] = table + (MDEV ? 0 : a.mask[0] + 1);
+  a.tag = tag;
+  a.xlate = xlate;
+  a.ctrl = ctrl;
+  uint32_t n = prev.n + now.n, nk = now.n_keys[1] + 0;
+  if (!MDEV && now.n_keys[0] > nk) nk = now.n_keys[0];
+  if (nk > n) n = nk;
+  *grid_rekey = n ? (n + REKEY_THREADS - 1) / REKEY_THREADS : 1;
+  n = (MDEV ? 0 : prev.n_keys[0]) + prev.n_keys[1];
+  *grid_xlate = n ? (n + REKEY_THREADS - 1) / REKEY_THREADS : 1;
+  return a;
+}
+// the table words raw_rekey_args uses for a new side with n_keys keys per map
+inline size_t raw_rekey_table_words(bool mdev, const uint32_t (&n_keys)[2]) {
+  return (mdev ? 0 : (size_t)delta_xmap_mask(n_keys[0]) + 1) + delta_xmap_mask(n_keys[1]) + 1;
 }
 
 }  // namespace kvg

@@ -216,6 +216,11 @@ def load() -> C.CDLL:
         "kvg_health_rescan_groups_keyed": (C.c_int, [vp, vp, sz, vp, sz, P(P(HealthDeltaC))]),
         "kvg_scan_pci_delta": (C.c_int, [vp, vp, sz, P(P(PciResultC)), P(P(PciDeltaC))]),
         "kvg_scan_pci_delta_reset": (C.c_int, [vp]),
+        "kvg_scan_pci_raw_delta": (C.c_int, [vp, P(PciRawC), P(P(PciResultC)), P(P(PciSnapC)), P(P(PciDeltaC))]),
+        "kvg_scan_pci_raw_delta_reset": (C.c_int, [vp]),
+        "kvg_scan_mdev_raw_delta": (C.c_int, [vp, P(MdevRawC), P(P(MdevResultC)), P(P(MdevSnapC)),
+                                              P(P(MdevDeltaC))]),
+        "kvg_scan_mdev_raw_delta_reset": (C.c_int, [vp]),
         "kvg_scan_mdev_delta": (C.c_int, [vp, vp, sz, P(TypeDict), P(P(MdevResultC)), P(P(MdevDeltaC))]),
         "kvg_scan_mdev_delta_reset": (C.c_int, [vp]),
         "kvg_text_pad": (sz, [sz]),

@@ -80,6 +80,7 @@ class PciDelta:
     dev_gone: np.ndarray        # u16 device ids absent now, ascending
     grp_dirty: np.ndarray       # u32 indices into the result's grp_keys, ascending
     grp_gone: np.ndarray        # u32 groups absent now, ascending
+    by_name: bool = False       # scan_pci_raw_delta: keyed by entry name, each side in its own snapshot's encoding
 
 
 @dataclass
@@ -91,6 +92,7 @@ class MdevDelta:
     type_gone: list             # labels (bytes) of the vGpuMap keys absent now, ascending previous canonical id
     par_dirty: np.ndarray       # u32 indices into the result's par_keys, ascending
     par_gone: np.ndarray        # u32 parent handles absent now, ascending
+    by_name: bool = False       # scan_mdev_raw_delta: keyed by entry name, each side in its own snapshot's encoding
 
 
 class _LockedLib:
@@ -217,13 +219,33 @@ class Context:
         """createIommuDeviceMap from the raw reads of its walk (plugin.read_pci_tree_raw): the GPU decodes them into the
         snapshot snapshot_pci_tree packs, then scans it -> (PciResult, PciSnapshot).  Raises plugin.ReferencePanic
         where the Go reference would panic."""
+        return self._scan_pci_raw(raw, None)
+
+    def scan_pci_raw_delta(self, raw):
+        """scan_pci_raw plus the diff against the previous scan_pci_raw_delta on this context, keyed by entry name and
+        exact in every snapshot mode -> (PciResult, PciSnapshot, PciDelta).  Each side of a change is in its own
+        snapshot's encoding, so the caller keeps the previous PciSnapshot to name what was removed or has gone."""
+        dl = C.POINTER(L.PciDeltaC)()
+        res, snap = self._scan_pci_raw(raw, dl)
+        delta = self._take_pci_delta(dl)
+        delta.by_name = True
+        return res, snap, delta
+
+    def scan_pci_raw_delta_reset(self):
+        self._ck(self._lib.kvg_scan_pci_raw_delta_reset(self._h))
+
+    def _scan_pci_raw(self, raw, dl):
+        """kvg_scan_pci_raw, or kvg_scan_pci_raw_delta into `dl` -> (PciResult, PciSnapshot)"""
         from .plugin import PciSnapshot, ReferencePanic
         off = np.ascontiguousarray(raw.off, dtype=np.uint32)
         state = np.ascontiguousarray(raw.state, dtype=np.uint16)
         blob = np.frombuffer(bytes(raw.bytes) + b"\0", dtype=np.uint8)
         arg = L.PciRawC(len(state), off.ctypes.data, blob.ctypes.data, state.ctypes.data)
         res, snap = C.POINTER(L.PciResultC)(), C.POINTER(L.PciSnapC)()
-        rc = self._lib.kvg_scan_pci_raw(self._h, C.byref(arg), C.byref(res), C.byref(snap))
+        if dl is None:
+            rc = self._lib.kvg_scan_pci_raw(self._h, C.byref(arg), C.byref(res), C.byref(snap))
+        else:
+            rc = self._lib.kvg_scan_pci_raw_delta(self._h, C.byref(arg), C.byref(res), C.byref(snap), C.byref(dl))
         if rc == L.KVG_EPANIC:
             raise ReferencePanic((self._lib.kvg_last_error(self._h) or b"").decode("latin-1"))
         self._ck(rc)
@@ -286,13 +308,33 @@ class Context:
         """createVgpuIDMap from the raw reads of its walk (plugin.read_mdev_tree_raw): the GPU decodes them into a
         snapshot and its raw type dictionary, then scans it -> (MdevResult, MdevSnapshot).  Raises plugin.ReferencePanic
         where the Go reference would panic."""
+        return self._scan_mdev_raw(raw, None)
+
+    def scan_mdev_raw_delta(self, raw):
+        """scan_mdev_raw plus the diff against the previous scan_mdev_raw_delta on this context, keyed by entry name (the
+        UUID string) and exact in every snapshot mode -> (MdevResult, MdevSnapshot, MdevDelta).  Parents are in each
+        side's own snapshot's encoding, so the caller keeps the previous MdevSnapshot to name gone parents."""
+        dl = C.POINTER(L.MdevDeltaC)()
+        res, snap = self._scan_mdev_raw(raw, dl)
+        delta = self._take_mdev_delta(dl)
+        delta.by_name = True
+        return res, snap, delta
+
+    def scan_mdev_raw_delta_reset(self):
+        self._ck(self._lib.kvg_scan_mdev_raw_delta_reset(self._h))
+
+    def _scan_mdev_raw(self, raw, dl):
+        """kvg_scan_mdev_raw, or kvg_scan_mdev_raw_delta into `dl` -> (MdevResult, MdevSnapshot)"""
         from .plugin import MdevSnapshot, ReferencePanic
         off = np.ascontiguousarray(raw.off, dtype=np.uint32)
         state = np.ascontiguousarray(raw.state, dtype=np.uint16)
         blob = np.frombuffer(bytes(raw.bytes) + b"\0", dtype=np.uint8)
         arg = L.MdevRawC(len(state), off.ctypes.data, blob.ctypes.data, state.ctypes.data)
         res, snap = C.POINTER(L.MdevResultC)(), C.POINTER(L.MdevSnapC)()
-        rc = self._lib.kvg_scan_mdev_raw(self._h, C.byref(arg), C.byref(res), C.byref(snap))
+        if dl is None:
+            rc = self._lib.kvg_scan_mdev_raw(self._h, C.byref(arg), C.byref(res), C.byref(snap))
+        else:
+            rc = self._lib.kvg_scan_mdev_raw_delta(self._h, C.byref(arg), C.byref(res), C.byref(snap), C.byref(dl))
         if rc == L.KVG_EPANIC:
             raise ReferencePanic((self._lib.kvg_last_error(self._h) or b"").decode("latin-1"))
         self._ck(rc)

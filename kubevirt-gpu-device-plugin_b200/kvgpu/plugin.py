@@ -659,48 +659,67 @@ def _rebuild_pci_maps(maps: Maps, res: PciResult, snap, name_of) -> PciMapsTouch
     return _rebuild_into(maps, lambda m: pci_maps_from_result(res, snap, m, name_of=name_of))
 
 
-def _patch_pci_maps(maps: Maps, dev: PciResult, grp: PciResult, delta) -> PciMapsTouched:
-    """The numeric patch of apply_pci_delta: deviceMap keys from `dev`, iommuMap keys from `grp` (each result's
-    permutation indexes its own survivors), bdfToIommuMap from the changes."""
+def _pci_names(snap: PciSnapshot | None):
+    """The strings behind a snapshot's handles: (address, device key, group) of a handle; None is fully numeric."""
+    addr = format_bdf if snap is None or snap.packed_addr else (lambda a: snap.names[int(a)])
+    dev = (lambda d: "%04x" % int(d)) if snap is None or snap.device_names is None else \
+        (lambda d: snap.device_names[int(d)])
+    grp = (lambda g: str(int(g))) if snap is None or snap.group_names is None else (lambda g: snap.group_names[int(g)])
+    return addr, dev, grp
+
+
+def _patch_pci_maps(maps: Maps, dev: PciResult, grp: PciResult, delta, snap: PciSnapshot | None = None,
+                    prev_snap: PciSnapshot | None = None, name_of=None) -> PciMapsTouched:
+    """The patch of apply_pci_delta: deviceMap keys from `dev`, iommuMap keys from `grp` (each result's permutation
+    indexes its own survivors), bdfToIommuMap from the changes.  Handles of the new side are named through `snap`,
+    those of the previous side (removed addresses, gone keys) through `prev_snap`; None is a numeric snapshot."""
+    addr_of, dev_of, grp_of = _pci_names(snap)
+    prev_addr_of, prev_dev_of, prev_grp_of = _pci_names(prev_snap)
+    dev_index = snap is not None and snap.device_names is not None
+
     def members(res, perm, off, k):
         s = res.survivors
         idx = perm[off[k]:off[k + 1]]
-        return [NvidiaGpuDevice(format_bdf(int(s["addr"][i])), int(s["numa"][i])) for i in idx]
+        return [NvidiaGpuDevice(addr_of(int(s["addr"][i])), int(s["numa"][i])) for i in idx]
 
     t = PciMapsTouched([], [], [], [])
     for k in delta.dev_dirty:
-        key = "%04x" % int(dev.dev_keys[k])
+        key = dev_of(dev.dev_keys[k])
         maps.deviceMap[key] = members(dev, dev.dev_perm, dev.dev_off, k)
-        maps.deviceNames[key] = dev.name_at(int(dev.dev_name_slot[k]))
+        maps.deviceNames[key] = name_of(key) if dev_index else dev.name_at(int(dev.dev_name_slot[k]))
         t.dev_dirty.append(key)
     for d in delta.dev_gone:
-        key = "%04x" % int(d)
+        key = prev_dev_of(d)
         maps.deviceMap.pop(key, None)
         maps.deviceNames.pop(key, None)
         t.dev_gone.append(key)
     for k in delta.grp_dirty:
-        key = str(int(grp.grp_keys[k]))
+        key = grp_of(grp.grp_keys[k])
         maps.iommuMap[key] = members(grp, grp.grp_perm, grp.grp_off, k)
         t.grp_dirty.append(key)
     for g in delta.grp_gone:
-        key = str(int(g))
+        key = prev_grp_of(g)
         maps.iommuMap.pop(key, None)
         t.grp_gone.append(key)
     for c in delta.changes:
-        addr = format_bdf(int(c["addr"]))
         if c["what"] & L.CH_REMOVED:
-            maps.bdfToIommuMap.pop(addr, None)
+            maps.bdfToIommuMap.pop(prev_addr_of(int(c["addr"])), None)
         else:
-            maps.bdfToIommuMap[addr] = str(int(c["now_group"]))
+            maps.bdfToIommuMap[addr_of(int(c["addr"]))] = grp_of(c["now_group"])
     return t
 
 
 def apply_pci_delta(maps: Maps, res: PciResult, delta, snap: PciSnapshot | None = None,
                     prev_snap: PciSnapshot | None = None, name_of=None) -> PciMapsTouched:
     """Patch deviceMap, iommuMap and bdfToIommuMap of `maps` (built from the previous delta scan's result) into
-    what pci_maps_from_result(res) builds, touching only dirty or gone keys and changed addresses.  A snapshot
-    that is not fully numeric (index-mode addresses, groups or device strings) has no stable handles: the maps are
-    then rebuilt and every key is reported."""
+    what pci_maps_from_result(res) builds, touching only dirty or gone keys and changed addresses.  A delta keyed by
+    entry name (Context.scan_pci_raw_delta) is patched in every snapshot mode, naming each side's handles through
+    its own snapshot.  Otherwise a snapshot that is not fully numeric (index-mode addresses, groups or device strings)
+    has no stable handles: the maps are then rebuilt and every key is reported."""
+    if getattr(delta, "by_name", False):
+        if snap is not None and snap.device_names is not None and name_of is None:
+            raise ValueError("snapshot carries device strings in index mode: pass name_of (Context.name_lookup)")
+        return _patch_pci_maps(maps, res, res, delta, snap, prev_snap, name_of)
     if not (_fully_numeric(snap) and _fully_numeric(prev_snap)):
         return _rebuild_pci_maps(maps, res, snap, name_of)
     return _patch_pci_maps(maps, res, res, delta)
@@ -765,22 +784,39 @@ def apply_mdev_delta(maps: Maps, res: MdevResult, delta, snap: MdevSnapshot | No
     """Patch vGpuMap, gpuVgpuMap and the label entries of deviceNames of `maps` (built from the previous delta scan's
     result) IN PLACE into what mdev_maps_from_result(res) builds, touching only dirty or gone keys: whoever holds
     maps.gpuVgpuMap (XidEventRouter) sees the new vGPUs.  A snapshot whose UUIDs are not canonical or whose parents are
-    not packed BDFs has no stable handles: the maps are then rebuilt (in place as well) and every key is reported."""
+    not packed BDFs has no stable handles: the maps are then rebuilt (in place as well) and every key is reported.  A
+    delta keyed by entry name (Context.scan_mdev_raw_delta) is patched in every snapshot mode, naming each side's
+    UUIDs and parents through its own snapshot."""
+    if getattr(delta, "by_name", False):
+        return _patch_mdev_maps(maps, res, res, delta, snap, prev_snap)
     if not (_numeric_mdev(snap) and _numeric_mdev(prev_snap)):
         return _rebuild_mdev_maps(maps, res, snap)
     return _patch_mdev_maps(maps, res, res, delta)
 
 
-def _patch_mdev_maps(maps: Maps, by_type: MdevResult, by_par: MdevResult, delta) -> MdevMapsTouched:
-    """The numeric patch of apply_mdev_delta: vGpuMap keys from `by_type`, gpuVgpuMap keys from `by_par` (each result's
-    permutation indexes its own survivors)."""
+def _mdev_names(snap: MdevSnapshot | None):
+    """(UUID of survivor i of survivors s, parent key of a handle) of a snapshot; None is fully numeric"""
+    uid = (lambda s, i: format_uuid(s["uuid"][i])) if snap is None or snap.uuid_ok else \
+        (lambda s, i: snap.names[int(s["src"][i])])
+    par = (lambda p: format_bdf(int(p))) if snap is None or snap.parent_names is None else \
+        (lambda p: snap.parent_names[int(p)])
+    return uid, par
+
+
+def _patch_mdev_maps(maps: Maps, by_type: MdevResult, by_par: MdevResult, delta, snap: MdevSnapshot | None = None,
+                     prev_snap: MdevSnapshot | None = None) -> MdevMapsTouched:
+    """The patch of apply_mdev_delta: vGpuMap keys from `by_type`, gpuVgpuMap keys from `by_par` (each result's
+    permutation indexes its own survivors).  The new side is named through `snap`, gone parents through `prev_snap`;
+    None is a numeric snapshot."""
+    uid_of, par_of = _mdev_names(snap)
+    _, prev_par_of = _mdev_names(prev_snap)
     t = MdevMapsTouched([], [], [], [])
     s = by_type.survivors
     for k in delta.type_dirty:
         c = int(by_type.type_keys[k])
         label = by_type.labels[c].decode("latin-1")
         idx = by_type.type_perm[by_type.type_off[k]:by_type.type_off[k + 1]]
-        maps.vGpuMap[label] = [NvidiaGpuDevice(format_uuid(s["uuid"][i]), int(s["numa"][i])) for i in idx]
+        maps.vGpuMap[label] = [NvidiaGpuDevice(uid_of(s, i), int(s["numa"][i])) for i in idx]
         maps.deviceNames[label] = by_type.type_names[c]
         t.type_dirty.append(label)
     for g in delta.type_gone:
@@ -791,12 +827,12 @@ def _patch_mdev_maps(maps: Maps, by_type: MdevResult, by_par: MdevResult, delta)
         t.type_gone.append(label)
     s = by_par.survivors
     for k in delta.par_dirty:
-        key = format_bdf(int(by_par.par_keys[k]))
+        key = par_of(by_par.par_keys[k])
         idx = by_par.par_perm[by_par.par_off[k]:by_par.par_off[k + 1]]
-        maps.gpuVgpuMap[key] = [format_uuid(s["uuid"][i]) for i in idx]
+        maps.gpuVgpuMap[key] = [uid_of(s, i) for i in idx]
         t.par_dirty.append(key)
     for p in delta.par_gone:
-        key = format_bdf(int(p))
+        key = prev_par_of(p)
         maps.gpuVgpuMap.pop(key, None)
         t.par_gone.append(key)
     return t
@@ -852,6 +888,8 @@ class DiscoveryScan:
         self.maps = Maps()
         self._loaded_path = None
         self._prev_pci_snap = None   # snapshot of the last rescan_iommu_device_map
+        self._prev_pci_raw_snap = None   # ... and of the last rescan_iommu_device_map(raw=True)
+        self._prev_mdev_raw_snap = None  # ... and of the last rescan_vgpu_id_map(raw=True)
         self._prev_mdev_snap = None  # snapshot of the last rescan_vgpu_id_map
 
     def close(self):
@@ -883,10 +921,18 @@ class DiscoveryScan:
         res = self.ctx.scan_pci(snap.recs)
         return pci_maps_from_result(res, snap, self.maps, name_of=self.ctx.name_lookup)
 
-    def rescan_iommu_device_map(self) -> PciMapsTouched:
+    def rescan_iommu_device_map(self, raw: bool = False) -> PciMapsTouched:
         """Re-walk the tree and bring deviceMap / iommuMap / bdfToIommuMap up to date through the re-scan delta.
-        The first call has no previous delta scan to diff against: it rebuilds the maps and reports every key."""
+        The first call has no previous delta scan to diff against: it rebuilds the maps and reports every key.
+        raw=True: the walk reads everything, the GPU decodes the reads and diffs by entry name
+        (Context.scan_pci_raw_delta), so the maps are patched, not rebuilt, in every snapshot mode."""
         self._ensure_table()
+        if raw:
+            res, snap, delta = self.ctx.scan_pci_raw_delta(read_pci_tree_raw(self.basePath))
+            prev, self._prev_pci_raw_snap = self._prev_pci_raw_snap, snap
+            if prev is None:
+                return _rebuild_pci_maps(self.maps, res, snap, self.ctx.name_lookup)
+            return apply_pci_delta(self.maps, res, delta, snap, prev, name_of=self.ctx.name_lookup)
         snap = snapshot_pci_tree(self.basePath)
         res, delta = self.ctx.scan_pci_delta(snap.recs)
         prev, self._prev_pci_snap = self._prev_pci_snap, snap
@@ -906,10 +952,18 @@ class DiscoveryScan:
         res = self.ctx.scan_mdev(snap.recs, snap.raw_types)
         return mdev_maps_from_result(res, snap, self.maps)
 
-    def rescan_vgpu_id_map(self) -> MdevMapsTouched:
+    def rescan_vgpu_id_map(self, raw: bool = False) -> MdevMapsTouched:
         """Re-walk the mdev tree and bring vGpuMap / gpuVgpuMap up to date through the re-scan delta.  The first call
-        has no previous delta scan to diff against: it rebuilds the maps and reports every key."""
+        has no previous delta scan to diff against: it rebuilds the maps and reports every key.  raw=True: the walk
+        reads everything, the GPU decodes the reads and diffs by entry name (Context.scan_mdev_raw_delta), so the maps
+        are patched, not rebuilt, in every snapshot mode."""
         self._ensure_table()
+        if raw:
+            res, snap, delta = self.ctx.scan_mdev_raw_delta(read_mdev_tree_raw(self.vGpuBasePath, self.basePath))
+            prev, self._prev_mdev_raw_snap = self._prev_mdev_raw_snap, snap
+            if prev is None:
+                return _rebuild_mdev_maps(self.maps, res, snap)
+            return apply_mdev_delta(self.maps, res, delta, snap, prev)
         snap = snapshot_mdev_tree(self.vGpuBasePath, self.basePath)
         res, delta = self.ctx.scan_mdev_delta(snap.recs, snap.raw_types)
         prev, self._prev_mdev_snap = self._prev_mdev_snap, snap

@@ -926,18 +926,28 @@ class PciRescanFeed(_RescanFeed):
     to running plugins and `make_plugin(spec)` builds one for a new key.  Each tick patches `maps` in place (Allocate
     reads iommuMap / bdfToIommuMap from it, so it sees a moved device at once), gives every plugin whose key is
     dirty its new device list, starts and registers a plugin for every new key, and stops the plugin of every key
-    that went.  The first tick has no previous snapshot: it rebuilds the maps and treats every key as dirty."""
+    that went.  The first tick has no previous snapshot: it rebuilds the maps and treats every key as dirty.
 
-    def __init__(self, scan_delta, snapshot, maps: Maps, plugins: dict, make_plugin, period_s: float = 0.01):
+    raw=True runs the feed from raw reads: `snapshot()` returns a PciRaw (plugin.read_pci_tree_raw) and
+    `scan_delta(raw)` is Context.scan_pci_raw_delta, whose delta is keyed by entry name, so a tick patches the maps
+    and re-sends only the dirty keys in every snapshot mode.  name_of (Context.name_lookup) names device keys when
+    the snapshot carries device strings in index mode."""
+
+    def __init__(self, scan_delta, snapshot, maps: Maps, plugins: dict, make_plugin, period_s: float = 0.01,
+                 raw: bool = False, name_of=None):
         super().__init__(scan_delta, snapshot, maps, plugins, make_plugin, period_s)
+        self.raw, self.name_of = raw, name_of
 
     def tick(self):
-        snap = self.snapshot()
-        res, delta = self.scan_delta(snap.recs)
-        if self._prev_snap is None:
-            touched = _rebuild_pci_maps(self.maps, res, snap, None)
+        if self.raw:
+            res, snap, delta = self.scan_delta(self.snapshot())
         else:
-            touched = apply_pci_delta(self.maps, res, delta, snap, self._prev_snap)
+            snap = self.snapshot()
+            res, delta = self.scan_delta(snap.recs)
+        if self._prev_snap is None:
+            touched = _rebuild_pci_maps(self.maps, res, snap, self.name_of)
+        else:
+            touched = apply_pci_delta(self.maps, res, delta, snap, self._prev_snap, name_of=self.name_of)
         self._prev_snap = snap
         self._follow(Maps(deviceMap={k: self.maps.deviceMap[k] for k in touched.dev_dirty},
                           deviceNames=self.maps.deviceNames), touched.dev_gone)
@@ -952,14 +962,23 @@ class MdevRescanFeed(_RescanFeed):
     Each tick patches vGpuMap / gpuVgpuMap of `maps` in place (an XidEventRouter holding maps.gpuVgpuMap sees a new
     vGPU at once), re-sends the device list of every plugin whose label is dirty (a NUMA move re-sends topology),
     starts and registers a plugin for every new label, and stops the plugin of every label that went.  The first
-    tick has no previous snapshot: it rebuilds the maps and treats every key as dirty."""
+    tick has no previous snapshot: it rebuilds the maps and treats every key as dirty.
 
-    def __init__(self, scan_delta, snapshot, maps: Maps, plugins: dict, make_plugin, period_s: float = 0.01):
+    raw=True runs the feed from raw reads: `snapshot()` returns an MdevRaw (plugin.read_mdev_tree_raw) and
+    `scan_delta(raw)` is Context.scan_mdev_raw_delta, whose delta is keyed by entry name, so a tick patches the maps
+    and re-sends only the dirty labels in every snapshot mode."""
+
+    def __init__(self, scan_delta, snapshot, maps: Maps, plugins: dict, make_plugin, period_s: float = 0.01,
+                 raw: bool = False):
         super().__init__(scan_delta, snapshot, maps, plugins, make_plugin, period_s)
+        self.raw = raw
 
     def tick(self):
-        snap = self.snapshot()
-        res, delta = self.scan_delta(snap.recs, snap.raw_types)
+        if self.raw:
+            res, snap, delta = self.scan_delta(self.snapshot())
+        else:
+            snap = self.snapshot()
+            res, delta = self.scan_delta(snap.recs, snap.raw_types)
         if self._prev_snap is None:
             touched = _rebuild_mdev_maps(self.maps, res, snap)
         else:

@@ -1,8 +1,9 @@
 // delta_emu.cpp — K7, the re-scan deltas of csrc/kvg_delta.cuh, compiled for the CPU from their real source on top
 // of warp_emu.h.  The launch arguments come from the builders of kvg_delta.cuh that kvg_api_delta.inc uses, in its
 // launch order: k_delta_merge<PciDeltaRec> then k_delta_lists (kvg_scan_pci_delta), k_mdev_delta_types,
-// k_delta_merge<MdevDeltaRec>, k_delta_lists (kvg_scan_mdev_delta), and the sharded forms through
-// k_delta_merge_shard<PciDeltaRec> / <MdevDeltaRec>.
+// k_delta_merge<MdevDeltaRec>, k_delta_lists (kvg_scan_mdev_delta), the sharded forms through
+// k_delta_merge_shard<PciDeltaRec> / <MdevDeltaRec>, and kvg_scan_pci_raw_delta's k_raw_rekey, k_raw_xlate,
+// k_delta_merge<PciRawDeltaRec>, k_delta_lists.
 #define KVG_HOST_EMU 1
 #include "warp_emu.h"
 #include "../../kubevirt-gpu-device-plugin_b200/csrc/kvg_delta.cuh"
@@ -122,6 +123,41 @@ int emu_mdev_shard_delta(const uint4* const* prev, const uint32_t* n_prev, const
                                            {n_now[1], n_now[2]});
     emu_launch(k_delta_merge_shard<MdevDeltaRec>, dim3(cols, 3), DELTA_THREADS, a, state);
   });
+  return 0;
+}
+
+// kvg_scan_pci_raw_delta's delta of two snapshots, chosen by raw_rekey_needed as run_raw_delta chooses: both sides
+// fully numeric, the merge of emu_delta on the survivors; otherwise the re-key first, its arguments from
+// raw_rekey_args as the library builds them.  sides[0] / [1]: the previous and the new side (kvg_delta.cuh
+// RawDeltaSide).  table: raw_rekey_table_words of the new keys, zero before the first call; xlate: RAW_XLATE_GROUP + the previous group keys; rekeyed: room for both sides' survivors.  flags,
+// tag, changes, the four lists and counts as for emu_delta; *launches: the kernels run.
+int emu_pci_raw_delta(const RawDeltaSide* sides, uint64_t* table, uint32_t* xlate, uint4* rekeyed, uint32_t* flags,
+                      uint32_t flag_cap, uint32_t tag, uint4* changes, uint32_t* dev_dirty, uint16_t* dev_gone,
+                      uint32_t* grp_dirty, uint32_t* grp_gone, uint32_t* counts, uint32_t* launches) {
+  Call c(flags, flag_cap);
+  const RawDeltaSide &pv = sides[0], &nw = sides[1];
+  const uint32_t* keys[4] = {nw.keys[0], pv.keys[0], nw.keys[1], pv.keys[1]};
+  const uint32_t n_keys[4] = {nw.n_keys[0], pv.n_keys[0], nw.n_keys[1], pv.n_keys[1]};
+  if (!raw_rekey_needed(pv.numeric, nw.numeric, RAW_NUM_ADDR | RAW_NUM_DEVICE | RAW_NUM_GROUP)) {
+    const auto op = delta_merge_op<PciDeltaRec>(pv.surv, pv.n, nw.surv, nw.n, changes, &c.ctrl, keys, n_keys, c.flag,
+                                                nullptr, tag);
+    c.run(op, {dev_dirty, dev_gone, grp_dirty, grp_gone}, true, counts, [&](uint64_t* state) {
+      emu_launch(k_delta_merge<PciDeltaRec>, dim3(delta_merge_tiles(op.n)), DELTA_THREADS, op, state);
+    });
+    *launches = 2;
+    return 0;
+  }
+  uint32_t g_rekey, g_xlate;
+  const RawRekeyArgs a = raw_rekey_args<false>(pv, nw, rekeyed, table, xlate, tag, &c.ctrl, &g_rekey, &g_xlate);
+  emu_launch(k_raw_rekey<false>, dim3(g_rekey), REKEY_THREADS, a);
+  emu_launch(k_raw_xlate<false>, dim3(g_xlate), REKEY_THREADS, a);
+  auto op = delta_merge_op<PciRawDeltaRec>(a.out[0], pv.n, a.out[1], nw.n, changes, &c.ctrl, keys, n_keys, c.flag,
+                                           xlate, tag);
+  op.k1.xlate = xlate + RAW_XLATE_GROUP;
+  c.run(op, {dev_dirty, dev_gone, grp_dirty, grp_gone}, true, counts, [&](uint64_t* state) {
+    emu_launch(k_delta_merge<PciRawDeltaRec>, dim3(delta_merge_tiles(op.n)), DELTA_THREADS, op, state);
+  });
+  *launches = 4;
   return 0;
 }
 
