@@ -236,31 +236,44 @@ class Context:
 
     def _scan_pci_raw(self, raw, dl):
         """kvg_scan_pci_raw, or kvg_scan_pci_raw_delta into `dl` -> (PciResult, PciSnapshot)"""
-        from .plugin import PciSnapshot, ReferencePanic
+        from .plugin import PciSnapshot
+
+        def table(n, off_p, bytes_p):
+            return [b.decode("latin-1") for b in self._table(n, off_p, bytes_p)]
+
+        return self._scan_raw(
+            "kvg_scan_pci_raw", L.PciRawC, L.PciResultC, L.PciSnapC, self._take_pci, raw, dl,
+            lambda sn: PciSnapshot(
+                L._arr(sn.recs, int(sn.n_records), L.PCI_REC), list(raw.names), bool(sn.packed_addr),
+                None if sn.groups_numeric else table(sn.n_group_names, sn.group_off, sn.group_bytes),
+                None if sn.devices_numeric else table(sn.n_device_names, sn.device_off, sn.device_bytes)))
+
+    def _scan_raw(self, entry: str, arg_t, res_t, snap_t, take, raw, dl, snapshot):
+        """`entry` (kvg_scan_<kind>_raw), or `entry`_delta into `dl`, on the raw reads `raw` (a PciRaw or MdevRaw,
+        passed as an arg_t) -> (take(result), snapshot(decoded snapshot)).  KVG_EPANIC raises plugin.ReferencePanic."""
+        from .plugin import ReferencePanic
         off = np.ascontiguousarray(raw.off, dtype=np.uint32)
         state = np.ascontiguousarray(raw.state, dtype=np.uint16)
         blob = np.frombuffer(bytes(raw.bytes) + b"\0", dtype=np.uint8)
-        arg = L.PciRawC(len(state), off.ctypes.data, blob.ctypes.data, state.ctypes.data)
-        res, snap = C.POINTER(L.PciResultC)(), C.POINTER(L.PciSnapC)()
+        arg = arg_t(len(state), off.ctypes.data, blob.ctypes.data, state.ctypes.data)
+        res, snap = C.POINTER(res_t)(), C.POINTER(snap_t)()
         if dl is None:
-            rc = self._lib.kvg_scan_pci_raw(self._h, C.byref(arg), C.byref(res), C.byref(snap))
+            rc = getattr(self._lib, entry)(self._h, C.byref(arg), C.byref(res), C.byref(snap))
         else:
-            rc = self._lib.kvg_scan_pci_raw_delta(self._h, C.byref(arg), C.byref(res), C.byref(snap), C.byref(dl))
+            rc = getattr(self._lib, entry + "_delta")(self._h, C.byref(arg), C.byref(res), C.byref(snap), C.byref(dl))
         if rc == L.KVG_EPANIC:
             raise ReferencePanic((self._lib.kvg_last_error(self._h) or b"").decode("latin-1"))
         self._ck(rc)
-        sn = snap.contents
-
-        def table(n, off_p, bytes_p):
-            o = L._arr(off_p, int(n) + 1, np.uint32)
-            b = C.string_at(bytes_p, int(o[-1])) if o[-1] else b""
-            return [b[o[k]:o[k + 1]].decode("latin-1") for k in range(int(n))]
-
-        out = PciSnapshot(L._arr(sn.recs, int(sn.n_records), L.PCI_REC), list(raw.names), bool(sn.packed_addr),
-                          None if sn.groups_numeric else table(sn.n_group_names, sn.group_off, sn.group_bytes),
-                          None if sn.devices_numeric else table(sn.n_device_names, sn.device_off, sn.device_bytes))
+        out = snapshot(snap.contents)
         self._lib.kvg_result_free(snap)
-        return self._take_pci(res), out
+        return take(res), out
+
+    @staticmethod
+    def _table(n, off_p, bytes_p) -> list:
+        """The n strings (bytes) of a snapshot string table."""
+        o = L._arr(off_p, int(n) + 1, np.uint32)
+        b = C.string_at(bytes_p, int(o[-1])) if o[-1] else b""
+        return [b[o[k]:o[k + 1]] for k in range(int(n))]
 
     @staticmethod
     def _type_dict(raw_types):
@@ -325,32 +338,15 @@ class Context:
 
     def _scan_mdev_raw(self, raw, dl):
         """kvg_scan_mdev_raw, or kvg_scan_mdev_raw_delta into `dl` -> (MdevResult, MdevSnapshot)"""
-        from .plugin import MdevSnapshot, ReferencePanic
-        off = np.ascontiguousarray(raw.off, dtype=np.uint32)
-        state = np.ascontiguousarray(raw.state, dtype=np.uint16)
-        blob = np.frombuffer(bytes(raw.bytes) + b"\0", dtype=np.uint8)
-        arg = L.MdevRawC(len(state), off.ctypes.data, blob.ctypes.data, state.ctypes.data)
-        res, snap = C.POINTER(L.MdevResultC)(), C.POINTER(L.MdevSnapC)()
-        if dl is None:
-            rc = self._lib.kvg_scan_mdev_raw(self._h, C.byref(arg), C.byref(res), C.byref(snap))
-        else:
-            rc = self._lib.kvg_scan_mdev_raw_delta(self._h, C.byref(arg), C.byref(res), C.byref(snap), C.byref(dl))
-        if rc == L.KVG_EPANIC:
-            raise ReferencePanic((self._lib.kvg_last_error(self._h) or b"").decode("latin-1"))
-        self._ck(rc)
-        sn = snap.contents
-
-        def table(n, off_p, bytes_p):
-            o = L._arr(off_p, int(n) + 1, np.uint32)
-            b = C.string_at(bytes_p, int(o[-1])) if o[-1] else b""
-            return [b[o[k]:o[k + 1]] for k in range(int(n))]
-
-        parents = None if sn.parents_packed else [p.decode("latin-1") for p in
-                                                  table(sn.n_parent_names, sn.parent_off, sn.parent_bytes)]
-        out = MdevSnapshot(L._arr(sn.recs, int(sn.n_records), L.MDEV_REC), list(raw.names),
-                           table(sn.n_types, sn.type_off, sn.type_bytes), parents, bool(sn.uuid_ok))
-        self._lib.kvg_result_free(snap)
-        return self._take_mdev(res), out
+        from .plugin import MdevSnapshot
+        return self._scan_raw(
+            "kvg_scan_mdev_raw", L.MdevRawC, L.MdevResultC, L.MdevSnapC, self._take_mdev, raw, dl,
+            lambda sn: MdevSnapshot(
+                L._arr(sn.recs, int(sn.n_records), L.MDEV_REC), list(raw.names),
+                self._table(sn.n_types, sn.type_off, sn.type_bytes),
+                None if sn.parents_packed else
+                [p.decode("latin-1") for p in self._table(sn.n_parent_names, sn.parent_off, sn.parent_bytes)],
+                bool(sn.uuid_ok)))
 
     def mdev_label_match(self, raw_files: list, name) -> np.ndarray:
         r"""The vGPU plugin's Allocate-time re-check (include/kvgpu.h kvg_mdev_label_match), one launch: element i is

@@ -24,9 +24,9 @@ from dataclasses import dataclass
 import numpy as np
 
 from . import _lib as L
-from .context import Context, MdevShardResult, PciResult, PciShardResult
-from .plugin import (Maps, MdevMapsTouched, PciMapsTouched, _fully_numeric, _numeric_mdev, _patch_mdev_maps,
-                     _patch_pci_maps, _rebuild_into, mdev_maps_from_result, pci_maps_from_result)
+from .context import Context, MdevShardResult, PciShardResult
+from .plugin import (Maps, MdevMapsTouched, PciMapsTouched, _fully_numeric, _mdev_maps, _numeric_mdev, _patch_mdev_maps,
+                     _patch_pci_maps, _pci_maps, _rebuild_into, _rebuild_mdev_maps)
 
 
 def shard_range(n: int, rank: int, world: int) -> tuple[int, int]:
@@ -72,21 +72,12 @@ def allgatherv_torch(local, dist_mod=None):
 def pci_maps_from_shard(sh: PciShardResult) -> Maps:
     """This rank's part of the three PCI maps: deviceMap / iommuMap for the keys it owns (all members),
     bdfToIommuMap for its own shard's survivors."""
-    m = pci_maps_from_result(sh.dev)
-    part = Maps(deviceMap=m.deviceMap, deviceNames=m.deviceNames)
-    part.iommuMap = pci_maps_from_result(sh.grp).iommuMap
-    e = sh.dev.grp_perm[:0]
-    local = PciResult(sh.n_records, sh.local, sh.dev.dev_keys[:0], sh.dev.grp_off[:1], e, e, sh.dev.grp_keys[:0],
-                      sh.dev.grp_off[:1], e, b"")
-    part.bdfToIommuMap = pci_maps_from_result(local).bdfToIommuMap
-    return part
+    return _pci_maps(Maps(), sh.dev, sh.grp, sh.local)
 
 
 def mdev_maps_from_shard(sh: MdevShardResult) -> Maps:
     """This rank's part of vGpuMap (type labels it owns) and gpuVgpuMap (parents it owns)."""
-    a = mdev_maps_from_result(sh.by_type)
-    b = mdev_maps_from_result(sh.by_parent)
-    return Maps(vGpuMap=a.vGpuMap, gpuVgpuMap=b.gpuVgpuMap, deviceNames=a.deviceNames)
+    return _mdev_maps(Maps(), sh.by_type, sh.by_parent)
 
 
 def apply_pci_shard_delta(part: Maps, res: PciShardResult, delta, snap=None, prev_snap=None) -> PciMapsTouched:
@@ -183,18 +174,7 @@ def apply_mdev_shard_delta(part: Maps, res: MdevShardResult, delta, snap=None, p
     else.  As in apply_mdev_delta, a snapshot without canonical UUIDs and packed-BDF parents has no stable handles: the
     part is then rebuilt (in place) and every key is reported."""
     if not (_numeric_mdev(snap) and _numeric_mdev(prev_snap)):
-        a, b = mdev_maps_from_result(res.by_type, snap), mdev_maps_from_result(res.by_parent, snap)
-        type_gone = sorted(set(part.vGpuMap) - set(a.vGpuMap))
-        par_gone = sorted(set(part.gpuVgpuMap) - set(b.gpuVgpuMap))
-        for label in type_gone:
-            if label not in part.deviceMap:
-                part.deviceNames.pop(label, None)
-        part.vGpuMap.clear()
-        part.vGpuMap.update(a.vGpuMap)
-        part.gpuVgpuMap.clear()
-        part.gpuVgpuMap.update(b.gpuVgpuMap)
-        part.deviceNames.update(a.deviceNames)
-        return MdevMapsTouched(list(a.vGpuMap), type_gone, list(b.gpuVgpuMap), par_gone)
+        return _rebuild_mdev_maps(part, res.by_type, res.by_parent, snap)
     return _patch_mdev_maps(part, res.by_type, res.by_parent, delta)
 
 

@@ -100,8 +100,12 @@ def _walk(root: str):
     yield from rec(root, os.path.basename(root), st)
 
 
-def _read_file(path):
+def _read_raw(path, link: bool = False):
+    """The contents of the file `path`, or the target of the link `path` (link=True), as read; None when the read
+    fails."""
     try:
+        if link:
+            return os.readlink(path)
         with open(path, "rb") as f:
             return f.read()
     except OSError:
@@ -110,7 +114,7 @@ def _read_file(path):
 
 def _read_id(base, addr, prop):
     """readIDFromFileFunc :294-302 -> (string, err)"""
-    data = _read_file(os.path.join(base, addr, prop))
+    data = _read_raw(os.path.join(base, addr, prop))
     if data is None:
         return "", True
     if len(data) < 2:
@@ -134,7 +138,7 @@ _GO_SPACE = "\t\n\v\f\r \u0085\u00a0\u1680\u2028\u2029\u202f\u205f\u3000" + "".j
 
 def _read_numa(base, addr):
     """readNUMANodeFunc :304-320 -> (raw value, err).  The clamp (<0 -> 0) is left to the GPU."""
-    data = _read_file(os.path.join(base, addr, "numa_node"))
+    data = _read_raw(os.path.join(base, addr, "numa_node"))
     if data is None:
         return 0, True
     try:
@@ -194,6 +198,32 @@ def _read_pci_entry(base_path: str, name: str):
     return vendor, device, group, driver, flags, numa
 
 
+def _pci_records(names, rows, ascending: bool, group_of):
+    """The records of the entries `names` from what _read_pci_entry returned for each (rows) -> (recs, packed_addr,
+    device_names).  addr is the packed BDF when every name parses (and the values ascend, if `ascending`), else the
+    index; group_of(group string) -> the group handle.  `device`: "%04x" strings travel as the number; anything else
+    switches the column to index mode (interned strings, like the groups): the GPU groups by the interned id, the host
+    keeps the strings and asks getDeviceName with the exact bytes."""
+    packed = [parse_bdf(n) for n in names]
+    packed_ok = all(p is not None for p in packed) and (
+        not ascending or all(packed[i] < packed[i + 1] for i in range(len(packed) - 1)))
+    devices_numeric = all(len(r[1]) == 4 and all(c in HEXD for c in r[1]) for r in rows if isinstance(r[1], str))
+    dintern = {}
+    recs = np.zeros(len(rows), dtype=L.PCI_REC)
+    for i, (vendor, device, group, driver, flags, numa) in enumerate(rows):
+        if isinstance(device, str):
+            if devices_numeric:
+                device = int(device, 16)
+            else:
+                device = dintern.setdefault(device, len(dintern))
+                if device > 0xFFFF:
+                    raise L.KvgError(L.KVG_ERANGE, "more than 65536 distinct non-canonical device strings")
+        if not -32768 <= numa <= 32767:
+            raise L.KvgError(L.KVG_ERANGE, "numa_node %d of %s does not fit int16" % (numa, names[i]))
+        recs[i] = (packed[i] if packed_ok else i, vendor, device, group_of(group), driver, flags, numa)
+    return recs, packed_ok, None if devices_numeric else list(dintern)
+
+
 def snapshot_pci_tree(base_path: str) -> PciSnapshot:
     """Walk `base_path` like createIommuDeviceMap and record what each reader returned."""
     rows, names = [], []
@@ -202,47 +232,20 @@ def snapshot_pci_tree(base_path: str) -> PciSnapshot:
             break
         if is_dir:   # :197-200
             continue
-        rows.append((name,) + _read_pci_entry(base_path, name))
+        rows.append(_read_pci_entry(base_path, name))
         names.append(name)
-    packed = [parse_bdf(n) for n in names]
-    packed_ok = all(p is not None for p in packed) and all(
-        packed[i] < packed[i + 1] for i in range(len(packed) - 1))
 
     def canon_dec(s):
         return s.isdigit() and s.isascii() and (s == "0" or s[0] != "0") and int(s) < (1 << 32)
 
-    groups_numeric = all(canon_dec(r[3]) for r in rows if r[3] != "")
-    group_names, intern = (None, None) if groups_numeric else ([], {})
-    # `device`: "%04x" strings travel as the number; anything else switches the column to index mode (interned
-    # strings, like the groups): the GPU groups by the interned id, the host keeps the strings and asks
-    # getDeviceName with the exact bytes
-    devs = [r[2] for r in rows if isinstance(r[2], str)]
-    devices_numeric = all(len(d) == 4 and all(c in HEXD for c in d) for d in devs)
-    device_names, dintern = (None, None) if devices_numeric else ([], {})
-    recs = np.zeros(len(rows), dtype=L.PCI_REC)
-    for i, (name, vendor, device, group, driver, flags, numa) in enumerate(rows):
-        if isinstance(device, str):
-            if devices_numeric:
-                device = int(device, 16)
-            else:
-                k = dintern.setdefault(device, len(dintern))
-                if k == len(device_names):
-                    device_names.append(device)
-                if k > 0xFFFF:
-                    raise L.KvgError(L.KVG_ERANGE, "more than 65536 distinct non-canonical device strings")
-                device = k
-        if group == "":
-            g = 0
-        elif groups_numeric:
-            g = int(group)
-        else:
-            g = intern.setdefault(group, len(intern))
-            if g == len(group_names):
-                group_names.append(group)
-        if not -32768 <= numa <= 32767:
-            raise L.KvgError(L.KVG_ERANGE, "numa_node %d of %s does not fit int16" % (numa, name))
-        recs[i] = (packed[i] if packed_ok else i, vendor, device, g, driver, flags, numa)
-    return PciSnapshot(recs, names, packed_ok, group_names, device_names)
+    # groups: the number itself when every group read is canonical decimal, else strings interned from 0
+    if all(canon_dec(r[2]) for r in rows if r[2] != ""):
+        intern, group_of = None, lambda g: int(g) if g else 0
+    else:
+        intern = {}
+        group_of = lambda g: intern.setdefault(g, len(intern)) if g else 0   # noqa: E731
+    recs, packed_ok, device_names = _pci_records(names, rows, True, group_of)
+    return PciSnapshot(recs, names, packed_ok, None if intern is None else list(intern), device_names)
 
 
 @dataclass
@@ -260,7 +263,7 @@ def read_pci_tree_raw(base_path: str) -> PciRaw:
     """The walk of snapshot_pci_tree with all five reads made for every entry and nothing decoded: file contents as
     read, link targets as os.readlink returns them.  Reading what the reference would not reach is allowed: the GPU
     decodes only what it reaches, so no panic is raised here."""
-    names, parts, state = [], [], []
+    names, fields, state = [], [], []
     bbase = os.fsencode(base_path)
     for name, is_dir, err in _walk(base_path):
         if err:
@@ -268,26 +271,26 @@ def read_pci_tree_raw(base_path: str) -> PciRaw:
         if is_dir:
             continue
         bname = os.fsencode(name)
-        st, row = 0, [bname]
+        st = 0
+        fields.append(bname)
         for f, prop in ((L.RAW_VENDOR, b"vendor"), (L.RAW_DRIVER, b"driver"), (L.RAW_GROUP, b"iommu_group"),
                         (L.RAW_NUMA, b"numa_node"), (L.RAW_DEVICE, b"device")):
-            path = os.path.join(bbase, bname, prop)
-            try:
-                data = os.readlink(path) if f in (L.RAW_DRIVER, L.RAW_GROUP) else open(path, "rb").read()
-            except OSError:
-                data, st = b"", st | (1 << (8 + f))
-            st |= 1 << f
-            row.append(data)
+            data = _read_raw(os.path.join(bbase, bname, prop), f in (L.RAW_DRIVER, L.RAW_GROUP))
+            st |= 1 << f | (1 << (8 + f) if data is None else 0)
+            fields.append(data or b"")
         names.append(name)
-        parts.append(row)
         state.append(st)
-    lens = np.array([len(x) for row in parts for x in row], dtype=np.int64)
-    off = np.zeros(len(lens) + 1, dtype=np.int64)
-    np.cumsum(lens, out=off[1:])
+    return PciRaw(names, *_pack_raw(fields, state, "the raw reads of %s" % base_path))
+
+
+def _pack_raw(fields, state, what: str):
+    """Byte fields, entry after entry, and the read bits of each entry (bit f: read f was made, bit 8 + f: it failed)
+    -> (u32 offsets, the fields joined, u16 state): field j is bytes[off[j]:off[j + 1]]."""
+    off = np.zeros(len(fields) + 1, dtype=np.int64)
+    np.cumsum([len(x) for x in fields], out=off[1:])
     if off[-1] > 0xFFFFFFFF:
-        raise ValueError("the raw reads of %s exceed 4 GiB" % base_path)
-    return PciRaw(names, off.astype(np.uint32), b"".join(x for row in parts for x in row),
-                  np.array(state, dtype=np.uint16))
+        raise ValueError("%s exceed 4 GiB" % what)
+    return off.astype(np.uint32), b"".join(fields), np.array(state, dtype=np.uint16)
 
 
 NOT_READ = "not read"   # a read that was not made (pack_alloc_raw); the library refuses one the reference reaches
@@ -310,14 +313,6 @@ class AllocRaw:
     egm_off: np.ndarray     # u32 [n_egm * AEGM_FIELDS + 1]
     egm_bytes: bytes
     egm_state: np.ndarray   # u16 [n_egm]
-
-
-def _offsets(parts) -> np.ndarray:
-    off = np.zeros(len(parts) + 1, dtype=np.int64)
-    np.cumsum([len(p) for p in parts], out=off[1:])
-    if off[-1] > 0xFFFFFFFF:
-        raise ValueError("the raw reads exceed 4 GiB")
-    return off.astype(np.uint32)
 
 
 def pack_alloc_raw(requests, egm_entries) -> AllocRaw:
@@ -350,9 +345,10 @@ def pack_alloc_raw(requests, egm_entries) -> AllocRaw:
             st |= 1 << L.AEGM_STAT | (0 if stat else 1 << (8 + L.AEGM_STAT))
         eparts += [enc(name), enc(gpus) if isinstance(gpus, (bytes, str)) else b""]
         estate.append(st)
-    return AllocRaw(np.array(n_members, dtype=np.uint32), np.array(n_ids, dtype=np.uint32), _offsets(mparts),
-                    b"".join(mparts), np.array(mstate, dtype=np.uint16), _offsets(iparts), b"".join(iparts),
-                    _offsets(eparts), b"".join(eparts), np.array(estate, dtype=np.uint16))
+    what = "the raw reads"
+    return AllocRaw(np.array(n_members, dtype=np.uint32), np.array(n_ids, dtype=np.uint32),
+                    *_pack_raw(mparts, mstate, what), *_pack_raw(iparts, (), what)[:2],
+                    *_pack_raw(eparts, estate, what))
 
 
 def snapshot_pci_ids(base_path: str, bdfs, intern: dict) -> PciSnapshot:
@@ -366,26 +362,8 @@ def snapshot_pci_ids(base_path: str, bdfs, intern: dict) -> PciSnapshot:
     The `device` column follows snapshot_pci_tree: "%04x" strings as the number, otherwise interned strings."""
     names = list(bdfs)
     rows = [_read_pci_entry(base_path, name) for name in names]
-    packed = [parse_bdf(n) for n in names]
-    packed_ok = all(p is not None for p in packed)
-    devs = [r[1] for r in rows if isinstance(r[1], str)]
-    devices_numeric = all(len(d) == 4 and all(c in HEXD for c in d) for d in devs)
-    device_names, dintern = (None, None) if devices_numeric else ([], {})
-    recs = np.zeros(len(names), dtype=L.PCI_REC)
-    for i, (vendor, device, group, driver, flags, numa) in enumerate(rows):
-        if isinstance(device, str):
-            if devices_numeric:
-                device = int(device, 16)
-            else:
-                device = dintern.setdefault(device, len(dintern))
-                if device == len(device_names):
-                    device_names.append(rows[i][1])
-                if device > 0xFFFF:
-                    raise L.KvgError(L.KVG_ERANGE, "more than 65536 distinct non-canonical device strings")
-        if not -32768 <= numa <= 32767:
-            raise L.KvgError(L.KVG_ERANGE, "numa_node %d of %s does not fit int16" % (numa, names[i]))
-        g = intern.setdefault(group, len(intern) + 1) if group else 0
-        recs[i] = (packed[i] if packed_ok else i, vendor, device, g, driver, flags, numa)
+    recs, packed_ok, device_names = _pci_records(names, rows, False,
+                                                 lambda g: intern.setdefault(g, len(intern) + 1) if g else 0)
     return PciSnapshot(recs, names, packed_ok, [""] + sorted(intern, key=intern.get), device_names)
 
 
@@ -401,7 +379,7 @@ def group_nodes(device_path: str, intern: dict) -> np.ndarray:
 
 
 def _read_vgpu_raw(base, addr, prop):
-    data = _read_file(os.path.join(base, addr, prop))
+    data = _read_raw(os.path.join(base, addr, prop))
     return (None, True) if data is None else (data, False)
 
 
@@ -417,6 +395,34 @@ def _read_gpu_id_for_vgpu(base, addr):
     return parts[-2].strip("\n"), False
 
 
+def _uuid_bytes(s: str):
+    """The 16 bytes of `s` when it is a UUID in canonical form (lower-case 8-4-4-4-12 hex), else None."""
+    h = s.replace("-", "")
+    if len(s) == 36 and len(h) == 32 and all(c in HEXD for c in h) and format_uuid(bytes.fromhex(h)) == s:
+        return bytes.fromhex(h)
+    return None
+
+
+def _read_mdev_entry(vgpu_base: str, pci_base: str, name: str, type_ids: dict):
+    """What the readers of createVgpuIDMap's walk callback return for one entry -> (type index, parent, flags, numa):
+    the type file, then the parent link only when the type read succeeded (:275), then the parent's numa_node only when
+    the link read succeeded.  A type file content not in `type_ids` (content -> index) gets the next index."""
+    flags, tidx, parent, numa = 0, 0, "", 0
+    raw, e = _read_vgpu_raw(vgpu_base, name, "mdev_type/name")
+    if e:
+        flags |= L.MF_TYPE_ERR
+    else:
+        tidx = type_ids.setdefault(raw, len(type_ids))
+        parent, e = _read_gpu_id_for_vgpu(vgpu_base, name)
+        if e:
+            flags |= L.MF_PARENT_ERR
+        else:
+            numa, e = _read_numa(pci_base, parent)
+            if e:
+                flags |= L.MF_NUMA_ERR
+    return tidx, parent, flags, numa
+
+
 @dataclass
 class MdevSnapshot:
     recs: np.ndarray
@@ -427,46 +433,21 @@ class MdevSnapshot:
 
 
 def snapshot_mdev_tree(vgpu_base: str, pci_base: str) -> MdevSnapshot:
-    rows, names = [], []
-    type_ids, raw_types = {}, []
+    rows, names, type_ids = [], [], {}
     for name, is_dir, err in _walk(vgpu_base):
         if err:
             break
         if is_dir:
             continue
-        flags, tidx, parent, numa = 0, 0, "", 0
-        raw, e = _read_vgpu_raw(vgpu_base, name, "mdev_type/name")
-        if e:
-            flags |= L.MF_TYPE_ERR
-        else:
-            tidx = type_ids.setdefault(raw, len(type_ids))
-            if tidx == len(raw_types):
-                raw_types.append(raw)
-        if not e:  # :275 is only reached when the type read succeeded
-            parent, e2 = _read_gpu_id_for_vgpu(vgpu_base, name)
-            if e2:
-                flags |= L.MF_PARENT_ERR
-            else:
-                numa, e3 = _read_numa(pci_base, parent)
-                if e3:
-                    flags |= L.MF_NUMA_ERR
-        rows.append((name, parent, tidx, flags, numa))
+        rows.append(_read_mdev_entry(vgpu_base, pci_base, name, type_ids))
         names.append(name)
     ppacked = [parse_bdf(r[1]) for r in rows if r[1] != ""]
     parents_packed = all(p is not None for p in ppacked)
     parent_names, intern = (None, None) if parents_packed else ([], {})
-
-    def uuid_bytes(s):
-        h = s.replace("-", "")
-        if len(s) == 36 and len(h) == 32 and all(c in HEXD for c in h) and format_uuid(
-                bytes.fromhex(h)) == s:
-            return bytes.fromhex(h)
-        return None
-
-    ub = [uuid_bytes(n) for n in names]
+    ub = [_uuid_bytes(n) for n in names]
     uuid_ok = all(u is not None for u in ub) and all(ub[i] < ub[i + 1] for i in range(len(ub) - 1))
     recs = np.zeros(len(rows), dtype=L.MDEV_REC)
-    for i, (name, parent, tidx, flags, numa) in enumerate(rows):
+    for i, (tidx, parent, flags, numa) in enumerate(rows):
         if parent == "":
             p = 0
         elif parents_packed:
@@ -481,7 +462,7 @@ def snapshot_mdev_tree(vgpu_base: str, pci_base: str) -> MdevSnapshot:
             recs[i]["uuid"][:4] = np.frombuffer(int(i).to_bytes(4, "big"), dtype=np.uint8)
         recs[i]["parent"], recs[i]["type_idx"], recs[i]["flags"] = p, tidx, flags
         recs[i]["parent_numa"] = numa
-    return MdevSnapshot(recs, names, raw_types, parent_names, uuid_ok)
+    return MdevSnapshot(recs, names, list(type_ids), parent_names, uuid_ok)
 
 
 @dataclass
@@ -507,7 +488,7 @@ def read_mdev_tree_raw(vgpu_base: str, pci_base: str) -> MdevRaw:
     """The walk of snapshot_mdev_tree with every read it can make and nothing decoded: the type file as read, the link
     target as os.readlink returns it, and <pci_base>/<parent>/numa_node for the parent of that target (not made when
     the link is unreadable or has no '/').  The GPU decodes only what the reference reaches."""
-    names, parts, state = [], [], []
+    names, fields, state = [], [], []
     vbase, pbase = os.fsencode(vgpu_base), os.fsencode(pci_base)
     for name, is_dir, err in _walk(vgpu_base):
         if err:
@@ -517,29 +498,21 @@ def read_mdev_tree_raw(vgpu_base: str, pci_base: str) -> MdevRaw:
         bname = os.fsencode(name)
         st, row = 0, [bname, b"", b"", b""]
 
-        def take(f, read):
+        def take(f, path, link=False):
             nonlocal st
-            st |= 1 << f
-            try:
-                row[f] = read()
-            except OSError:
-                st |= 1 << (8 + f)
+            data = _read_raw(path, link)
+            st |= 1 << f | (1 << (8 + f) if data is None else 0)
+            row[f] = data or b""
 
-        take(L.MRAW_TYPE, lambda: open(os.path.join(vbase, bname, b"mdev_type", b"name"), "rb").read())
-        take(L.MRAW_LINK, lambda: os.readlink(os.path.join(vbase, bname)))
+        take(L.MRAW_TYPE, os.path.join(vbase, bname, b"mdev_type", b"name"))
+        take(L.MRAW_LINK, os.path.join(vbase, bname), link=True)
         parent = mdev_numa_parent(row[L.MRAW_LINK]) if not (st >> (8 + L.MRAW_LINK)) & 1 else None
         if parent is not None:
-            take(L.MRAW_NUMA, lambda: open(os.path.join(pbase, parent, b"numa_node"), "rb").read())
+            take(L.MRAW_NUMA, os.path.join(pbase, parent, b"numa_node"))
         names.append(name)
-        parts.append(row)
+        fields += row
         state.append(st)
-    lens = np.array([len(x) for row in parts for x in row], dtype=np.int64)
-    off = np.zeros(len(lens) + 1, dtype=np.int64)
-    np.cumsum(lens, out=off[1:])
-    if off[-1] > 0xFFFFFFFF:
-        raise ValueError("the raw reads of %s exceed 4 GiB" % vgpu_base)
-    return MdevRaw(names, off.astype(np.uint32), b"".join(x for row in parts for x in row),
-                   np.array(state, dtype=np.uint16))
+    return MdevRaw(names, *_pack_raw(fields, state, "the raw reads of %s" % vgpu_base))
 
 
 def snapshot_mdev_ids(vgpu_base: str, pci_base: str, uuids, intern: dict) -> MdevSnapshot:
@@ -552,34 +525,20 @@ def snapshot_mdev_ids(vgpu_base: str, pci_base: str, uuids, intern: dict) -> Mde
     parent_names[h] = the string of handle h."""
     uuids = list(uuids)
     recs = np.zeros(len(uuids), dtype=L.MDEV_REC)
-    type_ids, raw_types, uuid_ok = {}, [], True
+    type_ids, uuid_ok = {}, True
     for i, name in enumerate(uuids):
-        flags, tidx, parent, numa = 0, 0, "", 0
-        raw, e = _read_vgpu_raw(vgpu_base, name, "mdev_type/name")
-        if e:
-            flags |= L.MF_TYPE_ERR
-        else:
-            tidx = type_ids.setdefault(raw, len(type_ids))
-            if tidx == len(raw_types):
-                raw_types.append(raw)
-            parent, e2 = _read_gpu_id_for_vgpu(vgpu_base, name)
-            if e2:
-                flags |= L.MF_PARENT_ERR
-            else:
-                numa, e3 = _read_numa(pci_base, parent)
-                if e3:
-                    flags |= L.MF_NUMA_ERR
+        tidx, parent, flags, numa = _read_mdev_entry(vgpu_base, pci_base, name, type_ids)
         if not -32768 <= numa <= 32767:
             raise L.KvgError(L.KVG_ERANGE, "numa_node %d of %s does not fit int16" % (numa, parent))
         h = intern.setdefault(parent, len(intern) + 1) if parent else 0
-        hx = name.replace("-", "")
-        if len(name) == 36 and len(hx) == 32 and all(c in HEXD for c in hx) and format_uuid(bytes.fromhex(hx)) == name:
-            recs[i]["uuid"] = np.frombuffer(bytes.fromhex(hx), dtype=np.uint8)
+        u = _uuid_bytes(name)
+        if u is not None:
+            recs[i]["uuid"] = np.frombuffer(u, dtype=np.uint8)
         else:
             uuid_ok = False
             recs[i]["uuid"][:4] = np.frombuffer(int(i).to_bytes(4, "big"), dtype=np.uint8)
         recs[i]["parent"], recs[i]["type_idx"], recs[i]["flags"], recs[i]["parent_numa"] = h, tidx, flags, numa
-    return MdevSnapshot(recs, uuids, raw_types, [""] + sorted(intern, key=intern.get), uuid_ok)
+    return MdevSnapshot(recs, uuids, list(type_ids), [""] + sorted(intern, key=intern.get), uuid_ok)
 
 
 # ------------------------------------------------------------------------------------------------
@@ -605,31 +564,18 @@ def pci_maps_from_result(res: PciResult, snap: PciSnapshot | None = None, maps: 
                          name_of=None) -> Maps:
     """name_of(key) -> getDeviceName(key): needed (and only used) when the snapshot carries the `device`
     strings in index mode — the GPU's per-survivor join is keyed by the numeric id and does not apply."""
-    m = maps or Maps()
+    return _pci_maps(maps or Maps(), res, res, res.survivors, snap, name_of)
+
+
+def _pci_maps(m: Maps, dev: PciResult, grp: PciResult, local: np.ndarray, snap: PciSnapshot | None = None,
+              name_of=None) -> Maps:
+    """New deviceMap, iommuMap and bdfToIommuMap dicts in `m`: every key of `dev` and of `grp` (_put_pci_keys), and
+    the survivors `local` in their order."""
     m.iommuMap, m.deviceMap, m.bdfToIommuMap = {}, {}, {}  # :188-190
-    s = res.survivors
-    if snap is None or snap.packed_addr:
-        addr = [format_bdf(int(a)) for a in s["addr"]]
-    else:
-        addr = [snap.names[int(a)] for a in s["addr"]]
-    if snap is None or snap.group_names is None:
-        gname = lambda g: str(int(g))
-    else:
-        gname = lambda g: snap.group_names[int(g)]
-    numa = s["numa"]
-    dev_index = snap is not None and snap.device_names is not None
-    if dev_index and name_of is None:
-        raise ValueError("snapshot carries device strings in index mode: pass name_of (Context.name_lookup)")
-    for k in range(len(res.dev_keys)):
-        key = snap.device_names[int(res.dev_keys[k])] if dev_index else "%04x" % int(res.dev_keys[k])
-        idx = res.dev_perm[res.dev_off[k]:res.dev_off[k + 1]]
-        m.deviceMap[key] = [NvidiaGpuDevice(addr[i], int(numa[i])) for i in idx]
-        m.deviceNames[key] = name_of(key) if dev_index else res.name_at(int(res.dev_name_slot[k]))
-    for k in range(len(res.grp_keys)):
-        idx = res.grp_perm[res.grp_off[k]:res.grp_off[k + 1]]
-        m.iommuMap[gname(res.grp_keys[k])] = [NvidiaGpuDevice(addr[i], int(numa[i])) for i in idx]
-    for i in range(len(s)):
-        m.bdfToIommuMap[addr[i]] = gname(s["iommu_group"][i])
+    _put_pci_keys(m, dev, grp, range(len(dev.dev_keys)), range(len(grp.grp_keys)), snap, name_of)
+    addr_of, _, grp_of = _pci_names(snap)
+    for a, g in zip(local["addr"], local["iommu_group"]):
+        m.bdfToIommuMap[addr_of(int(a))] = grp_of(g)
     return m
 
 
@@ -668,39 +614,48 @@ def _pci_names(snap: PciSnapshot | None):
     return addr, dev, grp
 
 
-def _patch_pci_maps(maps: Maps, dev: PciResult, grp: PciResult, delta, snap: PciSnapshot | None = None,
-                    prev_snap: PciSnapshot | None = None, name_of=None) -> PciMapsTouched:
-    """The patch of apply_pci_delta: deviceMap keys from `dev`, iommuMap keys from `grp` (each result's permutation
-    indexes its own survivors), bdfToIommuMap from the changes.  Handles of the new side are named through `snap`,
-    those of the previous side (removed addresses, gone keys) through `prev_snap`; None is a numeric snapshot."""
+def _put_pci_keys(maps: Maps, dev: PciResult, grp: PciResult, dev_ks, grp_ks, snap: PciSnapshot | None = None,
+                  name_of=None) -> tuple:
+    """Set the deviceMap key dev.dev_keys[k] and its deviceNames entry for every k of dev_ks, and the iommuMap key
+    grp.grp_keys[k] for every k of grp_ks (each result's permutation indexes its own survivors), named through `snap`
+    (None is fully numeric) -> (the device keys, the group keys) set, in that order."""
     addr_of, dev_of, grp_of = _pci_names(snap)
-    prev_addr_of, prev_dev_of, prev_grp_of = _pci_names(prev_snap)
     dev_index = snap is not None and snap.device_names is not None
+    if dev_index and name_of is None:
+        raise ValueError("snapshot carries device strings in index mode: pass name_of (Context.name_lookup)")
 
     def members(res, perm, off, k):
-        s = res.survivors
-        idx = perm[off[k]:off[k + 1]]
-        return [NvidiaGpuDevice(addr_of(int(s["addr"][i])), int(s["numa"][i])) for i in idx]
+        s = res.survivors[perm[off[k]:off[k + 1]]]
+        return [NvidiaGpuDevice(addr_of(a), n) for a, n in zip(s["addr"].tolist(), s["numa"].tolist())]
 
-    t = PciMapsTouched([], [], [], [])
-    for k in delta.dev_dirty:
+    dev_keys, grp_keys = [], []
+    for k in dev_ks:
         key = dev_of(dev.dev_keys[k])
         maps.deviceMap[key] = members(dev, dev.dev_perm, dev.dev_off, k)
         maps.deviceNames[key] = name_of(key) if dev_index else dev.name_at(int(dev.dev_name_slot[k]))
-        t.dev_dirty.append(key)
-    for d in delta.dev_gone:
-        key = prev_dev_of(d)
-        maps.deviceMap.pop(key, None)
-        maps.deviceNames.pop(key, None)
-        t.dev_gone.append(key)
-    for k in delta.grp_dirty:
+        dev_keys.append(key)
+    for k in grp_ks:
         key = grp_of(grp.grp_keys[k])
         maps.iommuMap[key] = members(grp, grp.grp_perm, grp.grp_off, k)
-        t.grp_dirty.append(key)
-    for g in delta.grp_gone:
-        key = prev_grp_of(g)
+        grp_keys.append(key)
+    return dev_keys, grp_keys
+
+
+def _patch_pci_maps(maps: Maps, dev: PciResult, grp: PciResult, delta, snap: PciSnapshot | None = None,
+                    prev_snap: PciSnapshot | None = None, name_of=None) -> PciMapsTouched:
+    """The patch of apply_pci_delta: deviceMap keys from `dev`, iommuMap keys from `grp` (_put_pci_keys),
+    bdfToIommuMap from the changes.  Handles of the new side are named through `snap`, those of the previous side
+    (removed addresses, gone keys) through `prev_snap`; None is a numeric snapshot."""
+    addr_of, _, grp_of = _pci_names(snap)
+    prev_addr_of, prev_dev_of, prev_grp_of = _pci_names(prev_snap)
+    dev_dirty, grp_dirty = _put_pci_keys(maps, dev, grp, delta.dev_dirty, delta.grp_dirty, snap, name_of)
+    t = PciMapsTouched(dev_dirty, [prev_dev_of(d) for d in delta.dev_gone], grp_dirty,
+                       [prev_grp_of(g) for g in delta.grp_gone])
+    for key in t.dev_gone:
+        maps.deviceMap.pop(key, None)
+        maps.deviceNames.pop(key, None)
+    for key in t.grp_gone:
         maps.iommuMap.pop(key, None)
-        t.grp_gone.append(key)
     for c in delta.changes:
         if c["what"] & L.CH_REMOVED:
             maps.bdfToIommuMap.pop(prev_addr_of(int(c["addr"])), None)
@@ -717,8 +672,6 @@ def apply_pci_delta(maps: Maps, res: PciResult, delta, snap: PciSnapshot | None 
     its own snapshot.  Otherwise a snapshot that is not fully numeric (index-mode addresses, groups or device strings)
     has no stable handles: the maps are then rebuilt and every key is reported."""
     if getattr(delta, "by_name", False):
-        if snap is not None and snap.device_names is not None and name_of is None:
-            raise ValueError("snapshot carries device strings in index mode: pass name_of (Context.name_lookup)")
         return _patch_pci_maps(maps, res, res, delta, snap, prev_snap, name_of)
     if not (_fully_numeric(snap) and _fully_numeric(prev_snap)):
         return _rebuild_pci_maps(maps, res, snap, name_of)
@@ -726,26 +679,13 @@ def apply_pci_delta(maps: Maps, res: PciResult, delta, snap: PciSnapshot | None 
 
 
 def mdev_maps_from_result(res: MdevResult, snap: MdevSnapshot | None = None, maps: Maps | None = None) -> Maps:
-    m = maps or Maps()
+    return _mdev_maps(maps or Maps(), res, res, snap)
+
+
+def _mdev_maps(m: Maps, by_type: MdevResult, by_par: MdevResult, snap: MdevSnapshot | None = None) -> Maps:
+    """New vGpuMap and gpuVgpuMap dicts in `m`: every key of `by_type` and of `by_par` (_put_mdev_keys)."""
     m.vGpuMap, m.gpuVgpuMap = {}, {}  # :256-257
-    s = res.survivors
-    if snap is None or snap.uuid_ok:
-        uid = [format_uuid(u) for u in s["uuid"]]
-    else:
-        uid = [snap.names[int(i)] for i in s["src"]]
-    if snap is None or snap.parent_names is None:
-        pname = lambda p: format_bdf(int(p))
-    else:
-        pname = lambda p: snap.parent_names[int(p)]
-    for k in range(len(res.type_keys)):
-        t = int(res.type_keys[k])
-        label = res.labels[t].decode("latin-1")
-        idx = res.type_perm[res.type_off[k]:res.type_off[k + 1]]
-        m.vGpuMap[label] = [NvidiaGpuDevice(uid[i], int(s["numa"][i])) for i in idx]
-        m.deviceNames[label] = res.type_names[t]
-    for k in range(len(res.par_keys)):
-        idx = res.par_perm[res.par_off[k]:res.par_off[k + 1]]
-        m.gpuVgpuMap[pname(res.par_keys[k])] = [uid[i] for i in idx]
+    _put_mdev_keys(m, by_type, by_par, range(len(by_type.type_keys)), range(len(by_par.par_keys)), snap)
     return m
 
 
@@ -762,10 +702,10 @@ def _numeric_mdev(snap: MdevSnapshot | None) -> bool:
     return snap is None or (snap.uuid_ok and snap.parent_names is None)
 
 
-def _rebuild_mdev_maps(maps: Maps, res: MdevResult, snap) -> MdevMapsTouched:
-    """mdev_maps_from_result into the dicts `maps` already holds (they are shared), reporting every key of the new
-    maps and every key that went."""
-    fresh = mdev_maps_from_result(res, snap)
+def _rebuild_mdev_maps(maps: Maps, by_type: MdevResult, by_par: MdevResult, snap) -> MdevMapsTouched:
+    """_mdev_maps into the dicts `maps` already holds (they are shared), reporting every key of the new maps and
+    every key that went."""
+    fresh = _mdev_maps(Maps(), by_type, by_par, snap)
     type_gone = sorted(set(maps.vGpuMap) - set(fresh.vGpuMap))
     par_gone = sorted(set(maps.gpuVgpuMap) - set(fresh.gpuVgpuMap))
     for label in type_gone:
@@ -790,51 +730,54 @@ def apply_mdev_delta(maps: Maps, res: MdevResult, delta, snap: MdevSnapshot | No
     if getattr(delta, "by_name", False):
         return _patch_mdev_maps(maps, res, res, delta, snap, prev_snap)
     if not (_numeric_mdev(snap) and _numeric_mdev(prev_snap)):
-        return _rebuild_mdev_maps(maps, res, snap)
+        return _rebuild_mdev_maps(maps, res, res, snap)
     return _patch_mdev_maps(maps, res, res, delta)
 
 
 def _mdev_names(snap: MdevSnapshot | None):
-    """(UUID of survivor i of survivors s, parent key of a handle) of a snapshot; None is fully numeric"""
-    uid = (lambda s, i: format_uuid(s["uuid"][i])) if snap is None or snap.uuid_ok else \
-        (lambda s, i: snap.names[int(s["src"][i])])
+    """(UUIDs of the survivors s, parent key of a handle) of a snapshot; None is fully numeric"""
+    uids = (lambda s: [format_uuid(u) for u in s["uuid"]]) if snap is None or snap.uuid_ok else \
+        (lambda s: [snap.names[i] for i in s["src"].tolist()])
     par = (lambda p: format_bdf(int(p))) if snap is None or snap.parent_names is None else \
         (lambda p: snap.parent_names[int(p)])
-    return uid, par
+    return uids, par
+
+
+def _put_mdev_keys(maps: Maps, by_type: MdevResult, by_par: MdevResult, type_ks, par_ks,
+                   snap: MdevSnapshot | None = None) -> tuple:
+    """Set the vGpuMap key of by_type.type_keys[k] and its deviceNames entry for every k of type_ks, and the gpuVgpuMap
+    key by_par.par_keys[k] for every k of par_ks (each result's permutation indexes its own survivors), named through
+    `snap` (None is fully numeric) -> (the labels, the parent keys) set, in that order."""
+    uids_of, par_of = _mdev_names(snap)
+    labels, parents = [], []
+    for k in type_ks:
+        c = int(by_type.type_keys[k])
+        label = by_type.labels[c].decode("latin-1")
+        s = by_type.survivors[by_type.type_perm[by_type.type_off[k]:by_type.type_off[k + 1]]]
+        maps.vGpuMap[label] = [NvidiaGpuDevice(u, n) for u, n in zip(uids_of(s), s["numa"].tolist())]
+        maps.deviceNames[label] = by_type.type_names[c]
+        labels.append(label)
+    for k in par_ks:
+        key = par_of(by_par.par_keys[k])
+        maps.gpuVgpuMap[key] = uids_of(by_par.survivors[by_par.par_perm[by_par.par_off[k]:by_par.par_off[k + 1]]])
+        parents.append(key)
+    return labels, parents
 
 
 def _patch_mdev_maps(maps: Maps, by_type: MdevResult, by_par: MdevResult, delta, snap: MdevSnapshot | None = None,
                      prev_snap: MdevSnapshot | None = None) -> MdevMapsTouched:
-    """The patch of apply_mdev_delta: vGpuMap keys from `by_type`, gpuVgpuMap keys from `by_par` (each result's
-    permutation indexes its own survivors).  The new side is named through `snap`, gone parents through `prev_snap`;
-    None is a numeric snapshot."""
-    uid_of, par_of = _mdev_names(snap)
+    """The patch of apply_mdev_delta: vGpuMap keys from `by_type`, gpuVgpuMap keys from `by_par` (_put_mdev_keys).
+    The new side is named through `snap`, gone parents through `prev_snap`; None is a numeric snapshot."""
     _, prev_par_of = _mdev_names(prev_snap)
-    t = MdevMapsTouched([], [], [], [])
-    s = by_type.survivors
-    for k in delta.type_dirty:
-        c = int(by_type.type_keys[k])
-        label = by_type.labels[c].decode("latin-1")
-        idx = by_type.type_perm[by_type.type_off[k]:by_type.type_off[k + 1]]
-        maps.vGpuMap[label] = [NvidiaGpuDevice(uid_of(s, i), int(s["numa"][i])) for i in idx]
-        maps.deviceNames[label] = by_type.type_names[c]
-        t.type_dirty.append(label)
-    for g in delta.type_gone:
-        label = g.decode("latin-1")
+    type_dirty, par_dirty = _put_mdev_keys(maps, by_type, by_par, delta.type_dirty, delta.par_dirty, snap)
+    t = MdevMapsTouched(type_dirty, [g.decode("latin-1") for g in delta.type_gone], par_dirty,
+                        [prev_par_of(p) for p in delta.par_gone])
+    for label in t.type_gone:
         maps.vGpuMap.pop(label, None)
         if label not in maps.deviceMap:
             maps.deviceNames.pop(label, None)
-        t.type_gone.append(label)
-    s = by_par.survivors
-    for k in delta.par_dirty:
-        key = par_of(by_par.par_keys[k])
-        idx = by_par.par_perm[by_par.par_off[k]:by_par.par_off[k + 1]]
-        maps.gpuVgpuMap[key] = [uid_of(s, i) for i in idx]
-        t.par_dirty.append(key)
-    for p in delta.par_gone:
-        key = prev_par_of(p)
+    for key in t.par_gone:
         maps.gpuVgpuMap.pop(key, None)
-        t.par_gone.append(key)
     return t
 
 
@@ -898,7 +841,7 @@ class DiscoveryScan:
     def _ensure_table(self):
         if self._loaded_path == self.pciIdsFilePath:
             return
-        data = _read_file(self.pciIdsFilePath)
+        data = _read_raw(self.pciIdsFilePath)
         # unreadable file -> getDeviceName returns "" for every key (:373-377): an empty table
         self.ctx.pciids_load(data if data is not None else b"")
         self._loaded_path = self.pciIdsFilePath
@@ -962,13 +905,13 @@ class DiscoveryScan:
             res, snap, delta = self.ctx.scan_mdev_raw_delta(read_mdev_tree_raw(self.vGpuBasePath, self.basePath))
             prev, self._prev_mdev_raw_snap = self._prev_mdev_raw_snap, snap
             if prev is None:
-                return _rebuild_mdev_maps(self.maps, res, snap)
+                return _rebuild_mdev_maps(self.maps, res, res, snap)
             return apply_mdev_delta(self.maps, res, delta, snap, prev)
         snap = snapshot_mdev_tree(self.vGpuBasePath, self.basePath)
         res, delta = self.ctx.scan_mdev_delta(snap.recs, snap.raw_types)
         prev, self._prev_mdev_snap = self._prev_mdev_snap, snap
         if prev is None:
-            return _rebuild_mdev_maps(self.maps, res, snap)
+            return _rebuild_mdev_maps(self.maps, res, res, snap)
         return apply_mdev_delta(self.maps, res, delta, snap, prev)
 
     def create_device_plugins(self) -> list:
@@ -979,20 +922,13 @@ def plugin_specs_from_maps(maps: Maps) -> list:
     """createDevicePlugins' payload half (device_plugin.go:99-157): one PluginSpec per deviceMap key,
     then one per vGpuMap key; name falls back to the key when getDeviceName returned ""."""
     specs = []
-    for key, devs in maps.deviceMap.items():
-        name = maps.deviceNames.get(key, "") or key
-        specs.append(PluginSpec(
-            key, name, "%s/%s" % (DEVICE_NAMESPACE, name),
-            "%skubevirt-%s.sock" % (DEVICE_PLUGIN_PATH, name),
-            "%s_%s" % (GPU_PREFIX, name.upper()),
-            [{"ID": d.addr, "Health": HEALTHY, "Topology": {"Nodes": [{"ID": d.numaNode}]}}
-             for d in devs]))
-    for key, devs in maps.vGpuMap.items():
-        name = maps.deviceNames.get(key, "") or key
-        specs.append(PluginSpec(
-            key, name, "%s/%s" % (DEVICE_NAMESPACE, name),
-            "%skubevirt-%s.sock" % (DEVICE_PLUGIN_PATH, name),
-            "%s_%s" % (VGPU_PREFIX, name.upper()),
-            [{"ID": d.addr, "Health": HEALTHY, "Topology": {"Nodes": [{"ID": d.numaNode}]}}
-             for d in devs], vgpu=True))
+    for devices, prefix, vgpu in ((maps.deviceMap, GPU_PREFIX, False), (maps.vGpuMap, VGPU_PREFIX, True)):
+        for key, devs in devices.items():
+            name = maps.deviceNames.get(key, "") or key
+            specs.append(PluginSpec(
+                key, name, "%s/%s" % (DEVICE_NAMESPACE, name),
+                "%skubevirt-%s.sock" % (DEVICE_PLUGIN_PATH, name),
+                "%s_%s" % (prefix, name.upper()),
+                [{"ID": d.addr, "Health": HEALTHY, "Topology": {"Nodes": [{"ID": d.numaNode}]}}
+                 for d in devs], vgpu=vgpu))
     return specs

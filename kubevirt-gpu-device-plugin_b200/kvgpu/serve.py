@@ -38,7 +38,7 @@ import numpy as np
 from . import _lib as L
 from . import dpapi
 from .plugin import (DEVICE_NAMESPACE, GPU_PREFIX, VGPU_PREFIX, Maps, PluginSpec, ReferencePanic, _read_id,
-                     _read_link, _read_vgpu_raw, _rebuild_mdev_maps, _rebuild_pci_maps, apply_mdev_delta,
+                     _read_link, _read_raw, _read_vgpu_raw, _rebuild_mdev_maps, _rebuild_pci_maps, apply_mdev_delta,
                      apply_pci_delta, format_uuid, pack_alloc_raw, parse_bdf, plugin_specs_from_maps)
 
 VFIO_DEVICE_PATH = "/dev/vfio"      # generic_device_plugin.go:54
@@ -413,14 +413,7 @@ class AllocateRawCheck:
         self.call, self.base_path = call, base_path
 
     def _read(self, addr, prop, link):
-        path = os.path.join(os.fsencode(self.base_path), os.fsencode(addr), prop)
-        try:
-            if link:
-                return os.readlink(path)
-            with open(path, "rb") as f:
-                return f.read()
-        except OSError:
-            return None
+        return _read_raw(os.path.join(os.fsencode(self.base_path), os.fsencode(addr), prop), link)
 
     def __call__(self, requests, egm_entries) -> list:
         """requests: [(pairs, devices_ids)] as for AllocateCheck; egm_entries: discover_egm_raw's entries (None or []
@@ -980,7 +973,7 @@ class MdevRescanFeed(_RescanFeed):
             snap = self.snapshot()
             res, delta = self.scan_delta(snap.recs, snap.raw_types)
         if self._prev_snap is None:
-            touched = _rebuild_mdev_maps(self.maps, res, snap)
+            touched = _rebuild_mdev_maps(self.maps, res, res, snap)
         else:
             touched = apply_mdev_delta(self.maps, res, delta, snap, self._prev_snap)
         self._prev_snap = snap
