@@ -121,6 +121,27 @@ struct ArawKeysArgs {
   uint32_t seq;
 };
 
+// k_araw_keys' work for n_egm entries spanning nb_egm bytes (host side): a field takes a byte and a space at least, a
+// list not kept one handle, so nb_egm + n_egm bounds the list positions (n_list); the key table has `slots` words.
+struct ArawKeysSize {
+  size_t n_list, slots;
+};
+inline ArawKeysSize araw_keys_size(uint32_t n_egm, size_t nb_egm) {
+  const size_t n_list = n_egm ? nb_egm + n_egm : 0;
+  return {n_list, raw_slots(n_list)};
+}
+// k_araw_keys' arguments: the EGM and ID tables where the kernel reads them, work arrays of araw_keys_size, the host
+// outputs, and the sequence word, which the key kernel writes only when no request follows it to the check kernel
+inline ArawKeysArgs araw_keys_args(const ArawKeysSize& ks, const uint32_t* egm_off, const uint16_t* egm_state,
+                                   const uint8_t* egm_bytes, uint32_t n_egm, const uint32_t* id_off,
+                                   const uint8_t* id_bytes, uint32_t n_ids, uint32_t* list_off, uint32_t* list,
+                                   uint2* tok, uint32_t* tok_entry, uint32_t* rank, uint64_t* table, uint32_t* ids_out,
+                                   uint8_t* kept_host, unsigned long long* verdict_host, uint32_t n_reqs,
+                                   uint32_t* seq_word, uint32_t seq) {
+  return {egm_off, egm_state, egm_bytes, n_egm, id_off, id_bytes, n_ids, list_off, list, tok, tok_entry, rank, table,
+          (uint32_t)(ks.slots - 1), ids_out, kept_host, verdict_host, n_reqs ? nullptr : seq_word, seq};
+}
+
 // discoverEGMDevicesFunc's rule for entry e: the number of fields of a kept entry, 0 for any other.  `miss` (NULL: do
 // not note) receives the reads it reaches that were not made.
 __device__ __forceinline__ uint32_t araw_egm_entry(const ArawKeysArgs& a, uint32_t e, unsigned long long* miss) {

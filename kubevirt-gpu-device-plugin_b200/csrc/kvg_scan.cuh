@@ -725,6 +725,14 @@ __global__ void __launch_bounds__(GROUP_CHECK_THREADS) k_pci_allocate_check(
     *((volatile uint32_t*)seq_host) = seq;
   }
 }
+// k_pci_allocate_check's req table (host side): the requests' members and IDs lie one request after another
+inline void allocate_check_reqs(const kvg_alloc_req* reqs, uint32_t n_reqs, uint4* req) {
+  for (uint32_t r = 0, rec_at = 0, id_at = 0; r < n_reqs; r++) {
+    req[r] = make_uint4(rec_at, reqs[r].n_members, id_at, reqs[r].n_ids);
+    rec_at += reqs[r].n_members;
+    id_at += reqs[r].n_ids;
+  }
+}
 // canonical id = smallest raw index with an identical label: hash + length first (independent,
 // pipelined loads), bytes only on a hash match
 __global__ void k_mdev_canon(const uint8_t* __restrict__ label, const uint32_t* __restrict__ raw_off,

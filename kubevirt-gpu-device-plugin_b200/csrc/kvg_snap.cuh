@@ -513,4 +513,138 @@ __global__ void __launch_bounds__(RAW_THREADS) k_mraw_pack(RawPackArgs a, uint4*
   recs[2 * (size_t)i + 1] = r;
 }
 
+// ---- the launch plan of both raw scans (host side; kvg_api_snap.inc and the CPU emulator build it alike) ---------
+// What differs between the two walks: a record of rec_words uint4; column c is interned when interned(broken, c), a
+// handle above max_hnd[c] being the range error of field range_field[c]; broken & bad_addr puts the names in index
+// mode.  The snapshot's mode flag mode[m] is 1 iff bit m of broken is clear, and column c's string table is
+// n_names[c], names_off[c], names_bytes[c].  empty_result and scan (the scan and fetch of the packed records) are the
+// library's, defined in kvg_api_snap.inc.
+template <class S, class T>
+using Member = T S::*;
+struct PciWalk {
+  using Raw = kvg_pci_raw;
+  using Snap = kvg_pci_snap;
+  using Result = kvg_pci_result;
+  static constexpr uint32_t fields = KVG_RAW_FIELDS, rec_words = 1;
+  static constexpr auto decode = k_raw_decode;
+  static constexpr auto pack = k_raw_pack;
+  static constexpr const char *decode_label = "raw_decode", *intern_label = "raw_intern", *pack_label = "raw_pack";
+  static bool interned(uint32_t broken, uint32_t c) {
+    return broken & (c == RAW_COL_GROUP ? RAW_BAD_GROUP : RAW_BAD_DEVICE);
+  }
+  static constexpr uint32_t bad_addr = RAW_BAD_ADDR;
+  static constexpr uint32_t max_hnd[2] = {0xffffffffu, 0xffffu}, range_field[2] = {KVG_RAW_DEVICE, KVG_RAW_DEVICE};
+  static constexpr Member<Snap, uint8_t> mode[3] = {&Snap::packed_addr, &Snap::groups_numeric,
+                                                     &Snap::devices_numeric};
+  static constexpr Member<Snap, uint32_t> n_names[2] = {&Snap::n_group_names, &Snap::n_device_names};
+  static constexpr Member<Snap, const uint32_t*> names_off[2] = {&Snap::group_off, &Snap::device_off};
+  static constexpr Member<Snap, const uint8_t*> names_bytes[2] = {&Snap::group_bytes, &Snap::device_bytes};
+  // kvg_last_error: "<fn>: a read ... at <where>", "<panic_at><where>", "<range_at><where>" (numa_field: its own)
+  static constexpr const char* fn = "kvg_scan_pci_raw";
+  static constexpr const char* panic_at = "the reference panics (slice bounds out of range, data[2:]) at ";
+  static constexpr const char* range_at = "more than 65536 distinct device strings at ";
+  static constexpr uint32_t numa_field = KVG_RAW_NUMA;
+  static constexpr const char* field_name[KVG_RAW_FIELDS] = {"name",        "vendor",    "driver",
+                                                             "iommu_group", "numa_node", "device"};
+  static int empty_result(kvg_ctx* ctx, void** blk, Result** res);
+  static int scan(kvg_ctx* ctx, const Snap* s, Result** res);
+};
+struct MdevWalk {
+  using Raw = kvg_mdev_raw;
+  using Snap = kvg_mdev_snap;
+  using Result = kvg_mdev_result;
+  static constexpr uint32_t fields = KVG_MRAW_FIELDS, rec_words = 2;
+  static constexpr auto decode = k_mraw_decode;
+  static constexpr auto pack = k_mraw_pack;
+  static constexpr const char *decode_label = "mraw_decode", *intern_label = "mraw_intern", *pack_label = "mraw_pack";
+  // the types always; the parents when one is not a canonical BDF
+  static bool interned(uint32_t broken, uint32_t c) { return c == MRAW_COL_TYPE || (broken & MRAW_BAD_PARENT); }
+  static constexpr uint32_t bad_addr = MRAW_BAD_UUID;
+  // 65,535 types at most (load_type_dict)
+  static constexpr uint32_t max_hnd[2] = {65534u, 0xffffffffu}, range_field[2] = {KVG_MRAW_TYPE, KVG_MRAW_LINK};
+  static constexpr Member<Snap, uint8_t> mode[2] = {&Snap::uuid_ok, &Snap::parents_packed};
+  static constexpr Member<Snap, uint32_t> n_names[2] = {&Snap::n_types, &Snap::n_parent_names};
+  static constexpr Member<Snap, const uint32_t*> names_off[2] = {&Snap::type_off, &Snap::parent_off};
+  static constexpr Member<Snap, const uint8_t*> names_bytes[2] = {&Snap::type_bytes, &Snap::parent_bytes};
+  static constexpr const char* fn = "kvg_scan_mdev_raw";
+  static constexpr const char* panic_at = "the reference panics (index out of range, a link target without '/') at ";
+  static constexpr const char* range_at = "more than 65535 distinct mdev_type/name contents at ";
+  static constexpr uint32_t numa_field = KVG_MRAW_NUMA;
+  static constexpr const char* field_name[KVG_MRAW_FIELDS] = {"name", "mdev_type/name", "link", "numa_node"};
+  static int empty_result(kvg_ctx* ctx, void** blk, Result** res);
+  static int scan(kvg_ctx* ctx, const Snap* s, Result** res);
+};
+
+// the snapshot's mode flags from the walk's broken bits, and back
+template <class W>
+inline void raw_snap_modes(typename W::Snap* s, uint32_t broken) {
+  uint32_t m = 0;
+  for (auto flag : W::mode) s->*flag = !((broken >> m++) & 1u);
+}
+template <class W>
+inline uint32_t raw_snap_broken(const typename W::Snap& s) {
+  uint32_t broken = 0, m = 0;
+  for (auto flag : W::mode) broken |= (s.*flag ? 0u : 1u) << m++;
+  return broken;
+}
+
+// The probe table of each column holds raw_slots(n) words, at least twice as many as entries
+inline size_t raw_slots(size_t n) {
+  size_t slots = 64;
+  while (slots < 2 * n) slots <<= 1;
+  return slots;
+}
+// The index-mode work of both columns, column after column: probe tables, then slots, handles and handle spans per
+// entry
+struct RawWork {
+  uint64_t* table;
+  uint32_t *slot_of, *hnd;
+  uint2* tab;
+};
+// column c of it, with the probe mask k_raw_probe takes
+struct RawColumn {
+  uint64_t* table;
+  uint32_t mask;
+  uint32_t *slot_of, *hnd;
+  uint2* tab;
+};
+inline RawColumn raw_column(const RawWork& w, size_t n, uint32_t c) {
+  const size_t slots = raw_slots(n);
+  return {w.table + c * slots, (uint32_t)(slots - 1), w.slot_of + c * n, w.hnd + c * n, w.tab + c * n};
+}
+template <class W>
+inline RawInternOp raw_intern_op(const RawColumn& col, const uint2* span, uint32_t n, uint32_t c, RawCtrl* ctrl) {
+  RawInternOp op;
+  op.table = col.table;
+  op.slot_of = col.slot_of;
+  op.span = span;
+  op.n = n;
+  op.col = c;
+  op.max_hnd = W::max_hnd[c];
+  op.range_field = W::range_field[c];
+  op.hnd = col.hnd;
+  op.tab = col.tab;
+  op.ctrl = ctrl;
+  return op;
+}
+// the pack runs iff the names are in index mode or a column is interned
+template <class W>
+inline bool raw_pack_needed(uint32_t broken) {
+  return (broken & W::bad_addr) || W::interned(broken, 0) || W::interned(broken, 1);
+}
+template <class W>
+inline RawPackArgs raw_pack_args(const RawWork& w, uint32_t n, uint32_t broken) {
+  RawPackArgs a = {};
+  a.n = n;
+  a.index_addr = (broken & W::bad_addr) ? 1u : 0u;
+  for (uint32_t c = 0; c < 2; c++)
+    if (W::interned(broken, c)) {
+      const RawColumn col = raw_column(w, n, c);
+      a.table[c] = col.table;
+      a.slot_of[c] = col.slot_of;
+      a.hnd[c] = col.hnd;
+    }
+  return a;
+}
+
 }  // namespace kvg

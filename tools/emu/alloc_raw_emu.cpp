@@ -1,6 +1,8 @@
 // alloc_raw_emu.cpp — kvg_pci_allocate_raw's kernels (csrc/kvg_alloc_raw.cuh) compiled for the CPU from their real
 // source on top of warp_emu.h, in the library's order and launch shapes: k_araw_members, k_araw_keys, then
-// k_pci_allocate_check on what they wrote; and unicode.ToLower of the device (case_lower) over any runes.
+// k_pci_allocate_check on what they wrote, the key kernel sized and its arguments built by araw_keys_size /
+// araw_keys_args (kvg_alloc_raw.cuh) and the request table by allocate_check_reqs (kvg_scan.cuh), as the library
+// builds them; and unicode.ToLower of the device (case_lower) over any runes.
 #define KVG_HOST_EMU 1
 #include <algorithm>
 #include <vector>
@@ -27,42 +29,19 @@ int emu_pci_allocate_raw(const uint32_t* reqs, uint32_t n_reqs, const uint32_t* 
   if (n_mem)
     emu_launch(k_araw_members, dim3((n_mem + ARAW_THREADS - 1) / ARAW_THREADS), ARAW_THREADS, moff, mst, mb, n_mem,
                recs.data(), want.data(), code_out);
-  const size_t n_list = n_egm ? eoff[(size_t)n_egm * KVG_AEGM_FIELDS] + n_egm : 0;
-  size_t slots = 64;
-  while (slots < 2 * n_list) slots <<= 1;
+  const ArawKeysSize ks = araw_keys_size(n_egm, n_egm ? eoff[(size_t)n_egm * KVG_AEGM_FIELDS] : 0);
+  const size_t n_list = ks.n_list;
   std::vector<uint32_t> list_off(n_egm + 1), list(n_list + 1), tok_entry(n_list + 1), rank(n_list + 1, 0xdeadbeefu);
   std::vector<uint2> tok(n_list + 1);
-  std::vector<uint64_t> table(slots, 0x5a5a5a5a5a5a5a5aull);  // the kernel clears its table
-  if (n_egm) {
-    ArawKeysArgs a;
-    a.egm_off = eoff;
-    a.egm_state = est;
-    a.egm_bytes = eb;
-    a.n_egm = n_egm;
-    a.id_off = ioff;
-    a.id_bytes = ib;
-    a.n_ids = n_ids;
-    a.list_off = list_off.data();
-    a.list = list.data();
-    a.tok = tok.data();
-    a.tok_entry = tok_entry.data();
-    a.rank = rank.data();
-    a.table = table.data();
-    a.mask = (uint32_t)(slots - 1);
-    a.ids_out = ids.data();
-    a.kept_host = kept_out;
-    a.verdict_host = (unsigned long long*)verdict_out;
-    a.seq_host = n_reqs ? nullptr : &seq;
-    a.seq = 7;
-    emu_launch(k_araw_keys, dim3(1), ARAW_KEY_THREADS, a);
-  }
+  std::vector<uint64_t> table(ks.slots, 0x5a5a5a5a5a5a5a5aull);  // the kernel clears its table
+  if (n_egm)
+    emu_launch(k_araw_keys, dim3(1), ARAW_KEY_THREADS,
+               araw_keys_args(ks, eoff, est, eb, n_egm, ioff, ib, n_ids, list_off.data(), list.data(), tok.data(),
+                              tok_entry.data(), rank.data(), table.data(), ids.data(), kept_out,
+                              (unsigned long long*)verdict_out, n_reqs, &seq, 7));
   if (n_reqs) {
     std::vector<uint4> req(n_reqs);
-    for (uint32_t r = 0, rec_at = 0, id_at = 0; r < n_reqs; r++) {
-      req[r] = make_uint4(rec_at, reqs[2 * r], id_at, reqs[2 * r + 1]);
-      rec_at += reqs[2 * r];
-      id_at += reqs[2 * r + 1];
-    }
+    allocate_check_reqs((const kvg_alloc_req*)reqs, n_reqs, req.data());
     uint32_t done = 0;
     emu_launch(k_pci_allocate_check, dim3(std::min(n_reqs, ALLOC_CHECK_MAX_GRID)), GROUP_CHECK_THREADS,
                (const uint4*)req.data(), (const uint4*)recs.data(), (const uint32_t*)want.data(),

@@ -228,17 +228,14 @@ int emu_mdev_label_match(const uint8_t* raw, const uint32_t* raw_off, uint32_t n
 // kvg_pci_allocate_check's kernel in its launch shape (min(n_reqs, ALLOC_CHECK_MAX_GRID) CTAs of GROUP_CHECK_THREADS):
 // reqs: n_reqs x {n_members, n_ids}; recs / want: the requests' members one after another; ids: their EGM handles;
 // egm_off: n_egm + 1 offsets into egm_gpu.  first_bad_out: n_reqs words; take_out: n_reqs x n_egm bytes; seq_out: the
-// sequence word (7 when done).  The CTA counter and the request offsets are the harness's, as the library's are its own.
+// sequence word (7 when done).  The request table comes from allocate_check_reqs (kvg_scan.cuh), as in the library;
+// the CTA counter is the harness's.
 int emu_pci_allocate_check(const uint32_t* reqs, uint32_t n_reqs, const uint4* recs, const uint32_t* want,
                            const uint32_t* ids, const uint32_t* egm_off, const uint32_t* egm_gpu, uint32_t n_egm,
                            uint32_t n_egm_gpus, uint32_t* first_bad_out, uint8_t* take_out, uint32_t* seq_out) {
   if (n_reqs == 0) return -1;
   std::vector<uint4> req(n_reqs);
-  for (uint32_t r = 0, rec_at = 0, id_at = 0; r < n_reqs; r++) {
-    req[r] = make_uint4(rec_at, reqs[2 * r], id_at, reqs[2 * r + 1]);
-    rec_at += reqs[2 * r];
-    id_at += reqs[2 * r + 1];
-  }
+  allocate_check_reqs((const kvg_alloc_req*)reqs, n_reqs, req.data());
   uint32_t done = 0;
   const uint32_t grid = std::min(n_reqs, ALLOC_CHECK_MAX_GRID);
   emu_launch(k_pci_allocate_check, dim3(grid), GROUP_CHECK_THREADS, (const uint4*)req.data(), recs, want, ids, egm_off,
