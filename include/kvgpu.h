@@ -21,6 +21,10 @@
  *   kvg_health_rescan_*_keyed             <- the same two checks with the state kept per UUID / address, so it
  *                                            survives re-scans that change the device list (the reference never
  *                                            re-scans)
+ *   kvg_health_rescan_*_raw               <- the same two checks from the raw reads of the advertised devices,
+ *                                            state kept per entry name, groups and parents compared as strings:
+ *                                            generic_device_plugin.go:611-690, generic_vgpu_device_plugin.go:280-385,
+ *                                            readers device_plugin.go:202-238, :269-284
  *   kvg_scan_pci_raw                      <- createIommuDeviceMap from the raw reads of its walk callback:
  *                                            readIDFromFileFunc :294-302, readNUMANodeFunc :304-320,
  *                                            readLinkFunc :323-331, isSupportedVfioDriver :249-252
@@ -753,6 +757,58 @@ int kvg_health_rescan_mdev_keyed(kvg_ctx *ctx, const kvg_mdev_rec *recs, size_t 
                                  const uint32_t *xid_parents, size_t n_xid, kvg_health_delta **delta);
 int kvg_health_rescan_groups_keyed(kvg_ctx *ctx, const kvg_pci_rec *recs, size_t n,
                                    const uint32_t *group_nodes, size_t n_nodes, kvg_health_delta **delta);
+
+/* Health re-scans from raw reads: the two checks of the keyed calls (generic_device_plugin.go:611-690,
+ * generic_vgpu_device_plugin.go:280-385) on the raw reads of the advertised devices, decoded on the GPU by the
+ * decoders of kvg_scan_pci_raw / kvg_scan_mdev_raw (the readers of device_plugin.go:202-238 and :269-284), with the
+ * state kept per ENTRY NAME and every identity compared as bytes, so nothing is interned on the host.
+ *
+ * Entries: one per advertised device, in the kvg_pci_raw / kvg_mdev_raw layout and with its conventions (offsets,
+ * the made / failed bits, a read the reference does not reach may be made or skipped).  The entry name
+ * (KVG_RAW_NAME / KVG_MRAW_NAME) is the device's ID as advertised, in any form; names must ascend strictly byte-wise
+ * across all entries, alive or not (checked on the device).
+ *
+ * Sets: `nodes` and `xid_parents` use the layout of kvg_type_dict as a list of byte strings (NULL = empty list), in
+ * any order, duplicates allowed.  `nodes` is one raw listing of the VFIO device directory (a standing set);
+ * `xid_parents` holds the bus ids of the GPUs that reported a critical XID since the previous call (events).
+ *
+ * Rules, for entry i decoded as the raw scans decode it:
+ *   groups  h' = the record passes createIommuDeviceMap's filter && the iommu_group link basename equals one of the
+ *           node names byte for byte ("042" is not "42"; `vfio` or `devices` match only a group so named; an empty
+ *           listing means no node exists): kvg_health_rescan_groups with string membership
+ *   mdev    p' = the mdev_type/name and link reads succeeded; m' = p' && (the decoded parent,
+ *           Split(target, "/")[len-2] trimmed, equals one of the XID bus ids || (p && m)); an empty parent is marked by
+ *           nothing.  healthy = p && !m: the two-bit rule of kvg_health_rescan_mdev
+ *
+ * State: each kind keeps a list of (name, state byte), byte-wise ascending.  prior_i = the byte of entry i's name in
+ * the previous list, or 0; record i is listed iff bit 0 of its new byte and of prior_i differ; the list then becomes
+ * this call's names and bytes.  The previous names stay on the device (double-buffered, adopted only on success).
+ * Each kind has a slot of its own: no scan, delta, Allocate, kvg_pciids_load or other health call (nor its reset)
+ * touches it, and these calls touch none of theirs.  A refused call hands out nothing and leaves the list unchanged.
+ *
+ * The delta is kvg_health_delta: changed[] holds (i << 1) | healthy_now in ascending i; n_alive counts the entries
+ * healthy now.  n = 0 empties the list and returns an empty delta (the reset), with nothing launched.
+ *
+ * Refused, in this precedence:
+ *   KVG_EINVAL  nothing launched: ctx, raw or delta NULL; off or state NULL with n > 0; bytes NULL with bytes to read;
+ *               off[0] != 0 or decreasing offsets; n above 2^31 - 1; more than KVG_HEALTH_MAX_GROUPS node names or
+ *               KVG_HEALTH_MAX_XID bus ids; a set with n_types > 0 and off NULL (or bytes NULL with bytes), off[0] != 0
+ *               or decreasing offsets; the entries' and the set's bytes together above 4 GiB.  No byte cap applies to
+ *               the set: the per-CTA table holds hashes and indices, the strings stay in device memory.
+ *   KVG_EINVAL  found by the decode: a read the reference reaches was not made (kvg_last_error names the entry)
+ *   KVG_EPANIC  the reference would panic (data[2:] of a short vendor / device file; a link target without '/')
+ *   KVG_ERANGE  a reached numa_node that parses but does not fit int16
+ *   KVG_EINVAL  the names do not ascend strictly byte-wise
+ *
+ * Cost: the raw bytes, offsets, states and the set are staged in one host-to-device copy.  Up to 32,768 entries and
+ * with kernel timing off, one kernel launch (one CTA: the set table, the decode, the join by name and the transition
+ * list written into mapped host memory) and one host synchronisation (a flag in that memory).  Above that, one launch
+ * of the look-back form (k_compact over 2048-entry tiles, one set table per CTA), one copy of the counters and the
+ * verdicts with one synchronisation, and one copy of the list with another. */
+int kvg_health_rescan_groups_raw(kvg_ctx *ctx, const kvg_pci_raw *raw, const kvg_type_dict *nodes,
+                                 kvg_health_delta **delta);
+int kvg_health_rescan_mdev_raw(kvg_ctx *ctx, const kvg_mdev_raw *raw, const kvg_type_dict *xid_parents,
+                               kvg_health_delta **delta);
 
 /* Scan `recs` and diff the result against the previous one, keyed by survivor address.
  *

@@ -256,11 +256,13 @@ struct PciHealthRule {
 // Per record two bits, p (present: mdev_record_alive) and m (marked), m => p.  A tick with the sorted, deduplicated
 // parent handles X:  p' = alive,  m' = p' && (parent in X || (p && m)),  healthy = p && !m.  The state byte keeps them
 // as bit 0 = healthy (p && !m), bit 1 = marked (p && m).  The rule reads the second unit of the 32-byte record.
+// `in_x()` is the membership test of the record's parent, asked only of a present, unmarked record: the handle in X
+// here, the parent string among the XID bus ids in the raw rule (kvg_snap.cuh).
 constexpr uint32_t HEALTH_MDEV_HEALTHY = 1u, HEALTH_MDEV_MARKED = 2u;
-__device__ __forceinline__ uint32_t health_mdev_next(const uint4& hi, uint32_t s, uint32_t n_types, const uint32_t* xs,
-                                                     uint32_t n_xid) {
+template <class InX>
+__device__ __forceinline__ uint32_t health_mdev_next(const uint4& hi, uint32_t s, uint32_t n_types, InX&& in_x) {
   if (!mdev_record_alive(hi, n_types)) return 0;
-  const bool marked = (s & HEALTH_MDEV_MARKED) || sorted_has<KVG_HEALTH_MAX_XID>(xs, n_xid, hi.x);
+  const bool marked = (s & HEALTH_MDEV_MARKED) || in_x();
   return marked ? HEALTH_MDEV_MARKED : HEALTH_MDEV_HEALTHY;
 }
 struct MdevHealthRule {
@@ -268,22 +270,25 @@ struct MdevHealthRule {
   const uint32_t* set;  // X
   uint32_t n_set, n_types;
   __device__ __forceinline__ uint32_t next(const uint4& r, uint32_t s, const uint32_t* xs) const {
-    return health_mdev_next(r, s, n_types, xs, n_set);
+    return health_mdev_next(r, s, n_types, [&] { return sorted_has<KVG_HEALTH_MAX_XID>(xs, n_set, r.x); });
   }
 };
 
 // passthrough GPUs by IOMMU group (kvg_health_rescan_groups): healthy = alive and the group's VFIO node exists.  One
 // bit per record, as for PCI.  A tick with the sorted, deduplicated handles G of the groups whose node exists now (the
-// encoding of kvg_pci_rec.iommu_group, r.z of the record):  h' = pci_record_alive(r) && r.z in G.
-__device__ __forceinline__ uint32_t health_group_next(const uint4& r, const uint32_t* gs, uint32_t n_groups) {
-  return pci_record_alive(r) && sorted_has<KVG_HEALTH_MAX_GROUPS>(gs, n_groups, r.z) ? 1u : 0u;
+// encoding of kvg_pci_rec.iommu_group, r.z of the record):  h' = pci_record_alive(r) && r.z in G.  `in_g()` is the
+// membership test of the record's group, asked only of an alive record (the raw rule: the group string among the
+// node names).
+template <class InG>
+__device__ __forceinline__ uint32_t health_group_next(const uint4& r, InG&& in_g) {
+  return pci_record_alive(r) && in_g() ? 1u : 0u;
 }
 struct GroupHealthRule {
   static constexpr uint32_t UNITS = 1, UNIT = 0, STAGE_ROWS = 12, SET_CAP = KVG_HEALTH_MAX_GROUPS, STATE_BITS = 1;
   const uint32_t* set;  // G
   uint32_t n_set;
   __device__ __forceinline__ uint32_t next(const uint4& r, uint32_t, const uint32_t* gs) const {
-    return health_group_next(r, gs, n_set);
+    return health_group_next(r, [&] { return sorted_has<KVG_HEALTH_MAX_GROUPS>(gs, n_set, r.z); });
   }
 };
 
@@ -456,6 +461,48 @@ constexpr uint32_t HEALTH_SMALL_MAX = HEALTH_SMALL_THREADS * HEALTH_SMALL_ROWS; 
 constexpr uint32_t HEALTH_STAGE_BYTES = 192u << 10;                               // one TMA round
 template <class Rule>
 constexpr uint32_t HEALTH_SMALL_SMEM = HEALTH_STAGE_BYTES + Rule::SET_CAP * 4 + KEYED_SMEM<Rule>;
+// The end of both one-CTA health kernels (k_health_small, k_health_raw_small of kvg_snap.cuh), once every row has
+// left its ballots in s_bal ("changed") and s_now ("healthy now") behind a block barrier, and each thread its count of
+// healthy records in n_alive: 32 rows x 32 warps = one counter per thread, in record order, so ONE block scan places
+// every transition; the list goes to changed_host, and every thread gets the totals.  Returns after the block barrier
+// that follows the list's system fence, so thread 0 may publish the header and the flag.
+constexpr uint32_t HEALTH_SMALL_NW = HEALTH_SMALL_THREADS / 32;
+__device__ __forceinline__ void health_small_list(uint32_t rows, uint32_t n_alive,
+                                                  uint32_t (*s_bal)[HEALTH_SMALL_NW],
+                                                  uint32_t (*s_now)[HEALTH_SMALL_NW], uint32_t* s_scan,
+                                                  uint32_t* s_alv, uint32_t* __restrict__ changed_host,
+                                                  uint32_t& alive, uint32_t& total) {
+  constexpr uint32_t NW = HEALTH_SMALL_NW;
+  const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const uint32_t crow = tid >> 5, cw = tid & 31;
+  const uint32_t mybal = crow < rows ? s_bal[crow][cw] : 0;
+  const uint32_t mycnt = __popc(mybal);
+  const uint32_t incl = warp_incl_sum(mycnt);
+  const uint32_t wal = warp_sum(n_alive);
+  if (lane == 31) s_scan[warp] = incl;
+  if (lane == 0) s_alv[warp] = wal;
+  __syncthreads();
+  uint32_t base = 0;
+  total = 0;
+  alive = 0;
+#pragma unroll
+  for (uint32_t w = 0; w < NW; w++) {
+    const uint32_t c = s_scan[w];
+    if (w < warp) base += c;
+    total += c;
+    alive += s_alv[w];
+  }
+  // thread (crow, cw) writes the transitions of warp cw in row crow: lane order == record order
+  uint32_t pos = base + incl - mycnt;
+  const uint32_t nowb = crow < rows ? s_now[crow][cw] : 0;
+  for (uint32_t m = mybal; m; m &= m - 1) {
+    const uint32_t l = (uint32_t)__ffs((int)m) - 1;
+    const uint32_t i = crow * HEALTH_SMALL_THREADS + cw * 32 + l;
+    changed_host[pos++] = (i << 1) | ((nowb >> l) & 1u);
+  }
+  __threadfence_system();  // the list entries of every thread are on their way before the flag
+  __syncthreads();
+}
 template <class Rule>
 __global__ void __launch_bounds__(HEALTH_SMALL_THREADS) k_health_small(Rule rule, const uint4* __restrict__ recs,
                                                                        uint32_t n, uint8_t* __restrict__ state,
@@ -552,33 +599,8 @@ __global__ void __launch_bounds__(HEALTH_SMALL_THREADS) k_health_small(Rule rule
     }
     __syncthreads();  // every read of the stage is done before the next round's copy lands in it
   }
-  // 32 rows x 32 warps = one counter per thread, in record order: ONE block scan places every transition
-  const uint32_t crow = tid >> 5, cw = tid & 31;
-  const uint32_t mybal = crow < rows ? s_bal[crow][cw] : 0;
-  const uint32_t mycnt = __popc(mybal);
-  const uint32_t incl = warp_incl_sum(mycnt);
-  const uint32_t wal = warp_sum(n_alive);
-  if (lane == 31) s_scan[warp] = incl;
-  if (lane == 0) s_alv[warp] = wal;
-  __syncthreads();
-  uint32_t base = 0, total = 0, alive = 0;
-#pragma unroll
-  for (uint32_t w = 0; w < NW; w++) {
-    const uint32_t c = s_scan[w];
-    if (w < warp) base += c;
-    total += c;
-    alive += s_alv[w];
-  }
-  // thread (crow, cw) writes the transitions of warp cw in row crow: lane order == record order
-  uint32_t pos = base + incl - mycnt;
-  const uint32_t nowb = crow < rows ? s_now[crow][cw] : 0;
-  for (uint32_t m = mybal; m; m &= m - 1) {
-    const uint32_t l = (uint32_t)__ffs((int)m) - 1;
-    const uint32_t i = crow * HEALTH_SMALL_THREADS + cw * 32 + l;
-    changed_host[pos++] = (i << 1) | ((nowb >> l) & 1u);
-  }
-  __threadfence_system();  // the list entries of every thread are on their way before the flag
-  __syncthreads();
+  uint32_t alive, total;
+  health_small_list(rows, n_alive, s_bal, s_now, s_scan, s_alv, changed_host, alive, total);
   if (tid == 0) {
     hdr_host[0] = alive;
     hdr_host[1] = total;

@@ -16,6 +16,12 @@
 //                  writes the record as the numeric snapshot has it, the type and parent spans, and the verdicts
 //   k_raw_probe, k_compact<RawInternOp>  as above: column 0 = the type contents (always), 1 = the parent (index mode)
 //   k_mraw_pack    type handles, parent handles (index mode) and the Walk index (names not canonical) into the records
+//
+// and the health re-scans from raw reads (kvg_health_rescan_groups_raw / kvg_health_rescan_mdev_raw): the entries
+// decoded as above, the state joined by entry name, groups and parents matched as strings:
+//
+//   k_health_raw_small<Rule>                        poll-loop sizes: one CTA, the list into mapped host memory
+//   k_compact<RawHealthOp<Rule>, KVG_BLOCK, C_ROWS>  above them
 #pragma once
 #include "../../include/kvgpu.h"
 #include "kvg_common.cuh"
@@ -511,6 +517,252 @@ __global__ void __launch_bounds__(RAW_THREADS) k_mraw_pack(RawPackArgs a, uint4*
   r.y = (r.y & 0xffff0000u) | (h[MRAW_COL_TYPE] & 0xffffu);
   if (a.table[MRAW_COL_PARENT]) r.x = h[MRAW_COL_PARENT];
   recs[2 * (size_t)i + 1] = r;
+}
+
+// ---- K6 from raw reads (kvg_health_rescan_groups_raw / kvg_health_rescan_mdev_raw) ------------------------------
+// The health rules of kvg_scan.cuh on entries decoded by the scans' own decoders (raw_decode_entry,
+// mraw_decode_entry), with every identity a string compared byte for byte: an entry is its name, a group or parent
+// is its string, the tick's set is a list of strings.
+//   RawNameSet<CAP>   the set (VFIO node names / XID bus ids) as a per-CTA open-addressed table in shared memory, built
+//                     once per call: one word per slot, tag (19 hash bits) << 13 | index + 1; the strings stay in
+//                     global memory, behind the entries' bytes
+//   RawNameJoin       the prior state byte of a name: the same position of the previous list first, then a binary
+//                     search of its names (Keyed<Rule>::find with a byte-wise compare)
+//   raw_health_step   one entry: the name-ascent check, the join, the rule, this call's byte
+//   k_health_raw_small<Rule>             poll-loop sizes: one CTA, the transition list into mapped host memory
+//   k_compact<RawHealthOp<Rule>, KVG_BLOCK, C_ROWS>  above them (or with kernel timing on)
+
+// byte-wise order of a[x.x, x.y) and c[y.x, y.y): <0, 0, >0
+__device__ __forceinline__ int raw_cmp(const uint8_t* a, uint2 x, const uint8_t* c, uint2 y) {
+  const uint32_t la = x.y - x.x, lc = y.y - y.x, m = min(la, lc);
+  for (uint32_t k = 0; k < m; k++) {
+    const uint32_t p = a[x.x + k], q = c[y.x + k];
+    if (p != q) return p < q ? -1 : 1;
+  }
+  return la < lc ? -1 : la > lc ? 1 : 0;
+}
+
+constexpr uint32_t RAW_SET_IDX_BITS = 13;
+static_assert(KVG_HEALTH_MAX_GROUPS < (1u << RAW_SET_IDX_BITS) && KVG_HEALTH_MAX_XID < (1u << RAW_SET_IDX_BITS),
+              "index + 1 of every set string fits the slot word");
+template <uint32_t CAP>
+struct RawNameSet {
+  static constexpr uint32_t SLOTS = 2 * CAP, MASK = SLOTS - 1;  // at most half full
+  uint32_t* slot;                                               // shared memory, [SLOTS]
+  const uint8_t* bytes;                                         // string k = bytes[off[k], off[k + 1])
+  const uint32_t* off;
+  __device__ __forceinline__ static uint32_t tag(uint64_t h) { return (uint32_t)(h >> 45); }
+  // every thread of the CTA: clear the table, then place its share of the n strings (duplicates take a slot each)
+  __device__ __forceinline__ void build(uint32_t n) {
+    for (uint32_t k = threadIdx.x; k < SLOTS; k += blockDim.x) slot[k] = 0;
+    __syncthreads();
+    for (uint32_t k = threadIdx.x; k < n; k += blockDim.x) {
+      const uint64_t h = raw_fnv(bytes, make_uint2(__ldg(&off[k]), __ldg(&off[k + 1])));
+      const uint32_t w = tag(h) << RAW_SET_IDX_BITS | (k + 1);
+      for (uint32_t s = (uint32_t)h & MASK;; s = (s + 1) & MASK)
+        if (atomicCAS(&slot[s], 0u, w) == 0u) break;
+    }
+    __syncthreads();
+  }
+  // is bytes[x) one of the strings?
+  __device__ __forceinline__ bool has(uint2 x) const {
+    const uint64_t h = raw_fnv(bytes, x);
+    const uint32_t t = tag(h);
+    for (uint32_t s = (uint32_t)h & MASK;; s = (s + 1) & MASK) {
+      const uint32_t w = slot[s];
+      if (!w) return false;
+      const uint32_t k = (w & ((1u << RAW_SET_IDX_BITS) - 1)) - 1;
+      if ((w >> RAW_SET_IDX_BITS) == t && raw_same(bytes, x, make_uint2(__ldg(&off[k]), __ldg(&off[k + 1]))))
+        return true;
+    }
+  }
+};
+
+// The previous call's list: its names (field 0 of each entry of its staged walk, `fields` offsets per entry) ascending
+// byte-wise, and its state bytes.
+struct RawNameJoin {
+  const uint32_t* off;
+  const uint8_t* bytes;
+  const uint8_t* state;
+  uint32_t n, fields;
+  __device__ __forceinline__ uint2 name(uint32_t j) const {
+    return make_uint2(__ldg(&off[(size_t)j * fields]), __ldg(&off[(size_t)j * fields + 1]));
+  }
+  // the prior byte of the name b[k), entry i of this call; 0 for a name the previous list lacks
+  __device__ __forceinline__ uint32_t find(const uint8_t* b, uint2 k, uint32_t i) const {
+    if (i < n && raw_cmp(bytes, name(i), b, k) == 0) return __ldg(&state[i]);
+    uint32_t lo = 0, hi = n;
+    while (lo < hi) {
+      const uint32_t mid = (lo + hi) >> 1;
+      if (raw_cmp(bytes, name(mid), b, k) < 0)
+        lo = mid + 1;
+      else
+        hi = mid;
+    }
+    return lo < n && raw_cmp(bytes, name(lo), b, k) == 0 ? (uint32_t)__ldg(&state[lo]) : 0u;
+  }
+};
+
+// passthrough GPUs by IOMMU group: h' = pci_record_alive(decoded record) && the iommu_group link basename is one of
+// the node names.  An alive record has read its link; a basename left without a span is the empty string.
+struct GroupRawRule {
+  static constexpr uint32_t FIELDS = KVG_RAW_FIELDS, SET_CAP = KVG_HEALTH_MAX_GROUPS, STATE_BITS = 1;
+  __device__ __forceinline__ static uint32_t next(const RawIn& in, uint32_t i, uint32_t, RawCtrl* ctrl,
+                                                  const RawNameSet<SET_CAP>& set) {
+    const RawEntry e = raw_decode_entry(in, i, ctrl);
+    const uint2 g = e.span[RAW_COL_GROUP];
+    return health_group_next(e.rec, [&] { return set.has(g.y >= g.x ? g : make_uint2(0, 0)); });
+  }
+};
+// vGPUs: present = the type and link reads succeeded (the raw dictionary always holds the type: one entry, index 0),
+// marked by a non-empty decoded parent that is one of the XID bus ids.
+struct MdevRawRule {
+  static constexpr uint32_t FIELDS = KVG_MRAW_FIELDS, SET_CAP = KVG_HEALTH_MAX_XID, STATE_BITS = 2;
+  __device__ __forceinline__ static uint32_t next(const RawIn& in, uint32_t i, uint32_t s, RawCtrl* ctrl,
+                                                  const RawNameSet<SET_CAP>& set) {
+    const MRawEntry e = mraw_decode_entry(in, i, ctrl);
+    const uint2 p = e.span[MRAW_COL_PARENT];
+    return health_mdev_next(e.rec[1], s, 1u, [&] { return p.y > p.x && set.has(p); });
+  }
+};
+
+// One call: this call's entries (the set's strings behind their bytes: set_off indexes in.bytes), the previous list,
+// and where this call's state bytes go.
+struct RawHealthArgs {
+  RawIn in;
+  const uint32_t* set_off;  // [n_set + 1]
+  uint32_t n_set;
+  RawNameJoin prev;
+  uint8_t* state;  // [in.n]
+};
+
+// Entry i: its name must exceed entry i - 1's (else *name_err = 1), its prior byte comes from the previous list by
+// name, the rule gives its new byte, which goes to this call's slot.  Returns the new byte; *was = the prior one.
+template <class Rule>
+__device__ __forceinline__ uint32_t raw_health_step(const RawHealthArgs& a, const RawNameSet<Rule::SET_CAP>& set,
+                                                    uint32_t i, RawCtrl* ctrl, uint32_t* name_err, uint32_t* was) {
+  const uint8_t* b = a.in.bytes;
+  const uint32_t* o = a.in.off + (size_t)i * Rule::FIELDS;
+  const uint2 nm = make_uint2(o[0], o[1]);
+  if (i > 0 && raw_cmp(b, make_uint2(o[-(int)Rule::FIELDS], o[1 - (int)Rule::FIELDS]), b, nm) >= 0) *name_err = 1u;
+  *was = a.prev.find(b, nm, i);
+  const uint32_t s = Rule::next(a.in, i, *was, ctrl, set);
+  a.state[i] = (uint8_t)s;
+  return s;
+}
+
+// Poll-loop sizes (n <= HEALTH_SMALL_MAX): ONE CTA, one launch.  Thread t takes entries t, t + 1024, ... (a row of
+// 1024 per step); the verdicts of the decode and the name check collect in shared memory; the list, the counters,
+// the verdicts and last the sequence word go straight into the host-visible result block: hdr_host = {n_alive,
+// n_changed, seq, name_err} then {miss, panic, range} as u64.
+template <class Rule>
+__global__ void __launch_bounds__(HEALTH_SMALL_THREADS) k_health_raw_small(RawHealthArgs a,
+                                                                           uint32_t* __restrict__ changed_host,
+                                                                           uint32_t* __restrict__ hdr_host,
+                                                                           uint32_t seq) {
+  pdl_enter();
+  constexpr uint32_t NW = HEALTH_SMALL_NW;
+  __shared__ uint32_t s_set[RawNameSet<Rule::SET_CAP>::SLOTS];
+  __shared__ RawCtrl s_ctrl;
+  __shared__ uint32_t s_err;
+  __shared__ uint32_t s_bal[HEALTH_SMALL_ROWS][NW];  // "changed" ballot of (row, warp)
+  __shared__ uint32_t s_now[HEALTH_SMALL_ROWS][NW];  // "healthy now" ballot of (row, warp)
+  __shared__ uint32_t s_scan[NW], s_alv[NW];
+  const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, n = a.in.n;
+  if (tid == 0) {
+    s_ctrl.miss = s_ctrl.panic = s_ctrl.range = ~0ull;
+    s_err = 0;
+  }
+  RawNameSet<Rule::SET_CAP> set = {s_set, a.in.bytes, a.set_off};
+  set.build(a.n_set);  // (its barriers also publish s_ctrl and s_err)
+  const uint32_t rows = (n + HEALTH_SMALL_THREADS - 1) / HEALTH_SMALL_THREADS;
+  uint32_t n_alive = 0;
+#pragma unroll 1
+  for (uint32_t r = 0; r < rows; r++) {  // uniform
+    const uint32_t i = r * HEALTH_SMALL_THREADS + tid;
+    const bool in = i < n;
+    uint32_t s = 0, was = 0;
+    if (in) s = raw_health_step<Rule>(a, set, i, &s_ctrl, &s_err, &was);
+    const bool now = in && (s & 1u) != 0;
+    const bool chg = in && (now ? 1u : 0u) != (was & 1u);
+    const uint32_t bc = __ballot_sync(KVG_FULL, chg), bn = __ballot_sync(KVG_FULL, now);
+    if (lane == 0) {
+      s_bal[r][warp] = bc;
+      s_now[r][warp] = bn;
+    }
+    n_alive += now ? 1u : 0u;
+  }
+  __syncthreads();  // every row's ballots are in place before any thread reads another warp's
+  uint32_t alive, total;
+  health_small_list(rows, n_alive, s_bal, s_now, s_scan, s_alv, changed_host, alive, total);
+  if (tid == 0) {
+    hdr_host[0] = alive;
+    hdr_host[1] = total;
+    hdr_host[3] = s_err;
+    unsigned long long* v = reinterpret_cast<unsigned long long*>(hdr_host + 4);
+    v[0] = s_ctrl.miss;
+    v[1] = s_ctrl.panic;
+    v[2] = s_ctrl.range;
+    __threadfence_system();
+    *((volatile uint32_t*)&hdr_host[2]) = seq;  // the host polls this word
+  }
+}
+
+// The look-back form: k_compact<RawHealthOp<Rule>, KVG_BLOCK, C_ROWS>.  Item = new byte | prior byte << W; a change of
+// bit 0 is listed.  The verdicts go to ctrl (RawCtrl), the name check to sc->key_err, the counters to sc.
+template <class Rule>
+struct RawHealthOp {
+  using Item = uint32_t;
+  static constexpr uint32_t W = Rule::STATE_BITS;
+  RawHealthArgs a;
+  RawNameSet<Rule::SET_CAP> set;  // slot: compact_enter
+  uint32_t n;
+  RawCtrl* ctrl;
+  ScanCtrl* sc;
+  uint32_t* changed;
+  uint32_t local_alive;
+  __device__ __forceinline__ Item load(uint32_t i, bool ok) const {
+    if (!ok) return 0;
+    uint32_t was;
+    const uint32_t s = raw_health_step<Rule>(a, set, i, ctrl, &sc->key_err, &was);
+    return s | was << W;
+  }
+  __device__ __forceinline__ bool pred(const Item& x, uint32_t) {
+    const uint32_t now = x & ((1u << W) - 1), was = x >> W;
+    local_alive += now & 1u;
+    return ((now ^ was) & 1u) != 0;
+  }
+  __device__ __forceinline__ uint32_t prepare(const Item&) const { return 0; }
+  __device__ __forceinline__ void emit(uint32_t pos, const Item& x, uint32_t i, uint32_t) {
+    changed[pos] = (i << 1) | (x & 1u);
+  }
+  __device__ __forceinline__ void tile_epilogue() {
+    const uint32_t s = warp_sum(local_alive);
+    if (lane_id() == 0 && s) atomicAdd(&sc->n_alive, s);
+    local_alive = 0;
+  }
+  __device__ __forceinline__ void finish(uint32_t total) { sc->n_changed = total; }
+};
+template <class Rule>
+__device__ __forceinline__ void compact_enter(RawHealthOp<Rule>& op) {
+  __shared__ uint32_t s_set[RawNameSet<Rule::SET_CAP>::SLOTS];
+  op.set.slot = s_set;
+  op.set.build(op.a.n_set);
+}
+// without the bound ptxas holds the vGPU instantiation to 40 registers and spills
+template <class Rule>
+constexpr int COMPACT_MIN_BLOCKS<RawHealthOp<Rule>> = 1;
+template <class Rule>
+inline RawHealthOp<Rule> raw_health_op(const RawHealthArgs& a, RawCtrl* ctrl, ScanCtrl* sc, uint32_t* changed) {
+  RawHealthOp<Rule> op;
+  op.a = a;
+  op.set = {nullptr, a.in.bytes, a.set_off};
+  op.n = a.in.n;
+  op.ctrl = ctrl;
+  op.sc = sc;
+  op.changed = changed;
+  op.local_alive = 0;
+  return op;
 }
 
 // ---- the launch plan of both raw scans (host side; kvg_api_snap.inc and the CPU emulator build it alike) ---------

@@ -214,6 +214,8 @@ def load() -> C.CDLL:
         "kvg_health_groups_reset": (C.c_int, [vp]),
         "kvg_health_rescan_mdev_keyed": (C.c_int, [vp, vp, sz, u32, vp, sz, P(P(HealthDeltaC))]),
         "kvg_health_rescan_groups_keyed": (C.c_int, [vp, vp, sz, vp, sz, P(P(HealthDeltaC))]),
+        "kvg_health_rescan_groups_raw": (C.c_int, [vp, P(PciRawC), P(TypeDict), P(P(HealthDeltaC))]),
+        "kvg_health_rescan_mdev_raw": (C.c_int, [vp, P(MdevRawC), P(TypeDict), P(P(HealthDeltaC))]),
         "kvg_scan_pci_delta": (C.c_int, [vp, vp, sz, P(P(PciResultC)), P(P(PciDeltaC))]),
         "kvg_scan_pci_delta_reset": (C.c_int, [vp]),
         "kvg_scan_pci_raw_delta": (C.c_int, [vp, P(PciRawC), P(P(PciResultC)), P(P(PciSnapC)), P(P(PciDeltaC))]),

@@ -2,6 +2,7 @@
 from __future__ import annotations
 
 import ctypes as C
+import os
 import threading
 from dataclasses import dataclass
 
@@ -517,6 +518,36 @@ class Context:
         res = C.POINTER(L.HealthDeltaC)()
         self._ck(self._lib.kvg_health_rescan_groups_keyed(self._h, recs.ctypes.data, len(recs),
                                                           g.ctypes.data if len(g) else None, len(g), C.byref(res)))
+        return self._take_health(res)
+
+    def health_rescan_groups_raw(self, raw, nodes=()) -> HealthDelta:
+        """Passthrough health re-scan by IOMMU group from raw reads (include/kvgpu.h kvg_health_rescan_groups_raw):
+        `raw` is a PciRaw of the advertised devices (plugin.read_pci_ids_raw), names ascending byte-wise; `nodes` the
+        names (bytes) of one listing of the VFIO directory (plugin.list_nodes_raw).  The state is kept per entry name;
+        `changed` indexes this call's entries.  An empty `raw` resets.  Raises plugin.ReferencePanic where the Go
+        reference would panic."""
+        return self._health_raw("kvg_health_rescan_groups_raw", L.PciRawC, raw, nodes)
+
+    def health_rescan_mdev_raw(self, raw, xid_parents=()) -> HealthDelta:
+        """vGPU health re-scan from raw reads (include/kvgpu.h kvg_health_rescan_mdev_raw): `raw` is an MdevRaw of the
+        advertised vGPUs (plugin.read_mdev_ids_raw), names ascending byte-wise; `xid_parents` the bus ids (bytes) of
+        the GPUs that reported a critical XID since the previous call, matched against the decoded parent strings.
+        The state is kept per entry name.  An empty `raw` resets."""
+        return self._health_raw("kvg_health_rescan_mdev_raw", L.MdevRawC, raw, xid_parents)
+
+    def _health_raw(self, entry: str, arg_t, raw, strs) -> HealthDelta:
+        from .plugin import ReferencePanic
+        off = np.ascontiguousarray(raw.off, dtype=np.uint32)
+        state = np.ascontiguousarray(raw.state, dtype=np.uint16)
+        blob = np.frombuffer(bytes(raw.bytes) + b"\0", dtype=np.uint8)
+        arg = arg_t(len(state), off.ctypes.data, blob.ctypes.data, state.ctypes.data)
+        td, keep = self._type_dict([os.fsencode(x) if isinstance(x, str) else bytes(x) for x in strs])
+        res = C.POINTER(L.HealthDeltaC)()
+        rc = getattr(self._lib, entry)(self._h, C.byref(arg), C.byref(td), C.byref(res))
+        del keep
+        if rc == L.KVG_EPANIC:
+            raise ReferencePanic((self._lib.kvg_last_error(self._h) or b"").decode("latin-1"))
+        self._ck(rc)
         return self._take_health(res)
 
     def _take_pci_delta(self, dl) -> PciDelta:

@@ -263,24 +263,47 @@ def read_pci_tree_raw(base_path: str) -> PciRaw:
     """The walk of snapshot_pci_tree with all five reads made for every entry and nothing decoded: file contents as
     read, link targets as os.readlink returns them.  Reading what the reference would not reach is allowed: the GPU
     decodes only what it reaches, so no panic is raised here."""
-    names, fields, state = [], [], []
-    bbase = os.fsencode(base_path)
+    names = []
     for name, is_dir, err in _walk(base_path):
         if err:
             break
-        if is_dir:
-            continue
-        bname = os.fsencode(name)
-        st = 0
-        fields.append(bname)
-        for f, prop in ((L.RAW_VENDOR, b"vendor"), (L.RAW_DRIVER, b"driver"), (L.RAW_GROUP, b"iommu_group"),
-                        (L.RAW_NUMA, b"numa_node"), (L.RAW_DEVICE, b"device")):
-            data = _read_raw(os.path.join(bbase, bname, prop), f in (L.RAW_DRIVER, L.RAW_GROUP))
-            st |= 1 << f | (1 << (8 + f) if data is None else 0)
-            fields.append(data or b"")
-        names.append(name)
+        if not is_dir:
+            names.append(name)
+    return read_pci_ids_raw(base_path, names)
+
+
+def _read_pci_entry_raw(bbase: bytes, name: str):
+    """The five reads of one entry, raw -> (fields: name, vendor, driver target, iommu_group target, numa_node, device;
+    state bits)."""
+    bname = os.fsencode(name)
+    st, row = 0, [bname]
+    for f, prop in ((L.RAW_VENDOR, b"vendor"), (L.RAW_DRIVER, b"driver"), (L.RAW_GROUP, b"iommu_group"),
+                    (L.RAW_NUMA, b"numa_node"), (L.RAW_DEVICE, b"device")):
+        data = _read_raw(os.path.join(bbase, bname, prop), f in (L.RAW_DRIVER, L.RAW_GROUP))
+        st |= 1 << f | (1 << (8 + f) if data is None else 0)
+        row.append(data or b"")
+    return row, st
+
+
+def read_pci_ids_raw(base_path: str, names) -> PciRaw:
+    """The reads of read_pci_tree_raw for the entries `names` in THAT order (a health re-scan's advertised devices,
+    any form of name; an entry that is gone reads as failed reads)."""
+    names, fields, state = list(names), [], []
+    bbase = os.fsencode(base_path)
+    for name in names:
+        row, st = _read_pci_entry_raw(bbase, name)
+        fields += row
         state.append(st)
     return PciRaw(names, *_pack_raw(fields, state, "the raw reads of %s" % base_path))
+
+
+def list_nodes_raw(device_path: str) -> list:
+    """One listing of the VFIO device directory (/dev/vfio, generic_device_plugin.go:611-690) as the names' bytes, in
+    listing order: every name, `vfio` and `devices` included; a missing directory means no node exists."""
+    try:
+        return os.listdir(os.fsencode(device_path))
+    except FileNotFoundError:
+        return []
 
 
 def _pack_raw(fields, state, what: str):
@@ -488,28 +511,41 @@ def read_mdev_tree_raw(vgpu_base: str, pci_base: str) -> MdevRaw:
     """The walk of snapshot_mdev_tree with every read it can make and nothing decoded: the type file as read, the link
     target as os.readlink returns it, and <pci_base>/<parent>/numa_node for the parent of that target (not made when
     the link is unreadable or has no '/').  The GPU decodes only what the reference reaches."""
-    names, fields, state = [], [], []
-    vbase, pbase = os.fsencode(vgpu_base), os.fsencode(pci_base)
+    names = []
     for name, is_dir, err in _walk(vgpu_base):
         if err:
             break
-        if is_dir:
-            continue
-        bname = os.fsencode(name)
-        st, row = 0, [bname, b"", b"", b""]
+        if not is_dir:
+            names.append(name)
+    return read_mdev_ids_raw(vgpu_base, pci_base, names)
 
-        def take(f, path, link=False):
-            nonlocal st
-            data = _read_raw(path, link)
-            st |= 1 << f | (1 << (8 + f) if data is None else 0)
-            row[f] = data or b""
 
-        take(L.MRAW_TYPE, os.path.join(vbase, bname, b"mdev_type", b"name"))
-        take(L.MRAW_LINK, os.path.join(vbase, bname), link=True)
-        parent = mdev_numa_parent(row[L.MRAW_LINK]) if not (st >> (8 + L.MRAW_LINK)) & 1 else None
-        if parent is not None:
-            take(L.MRAW_NUMA, os.path.join(pbase, parent, b"numa_node"))
-        names.append(name)
+def _read_mdev_entry_raw(vbase: bytes, pbase: bytes, name: str):
+    """The reads of one mdev entry, raw -> (fields: name, mdev_type/name, link target, parent numa_node; state bits)."""
+    bname = os.fsencode(name)
+    st, row = 0, [bname, b"", b"", b""]
+
+    def take(f, path, link=False):
+        nonlocal st
+        data = _read_raw(path, link)
+        st |= 1 << f | (1 << (8 + f) if data is None else 0)
+        row[f] = data or b""
+
+    take(L.MRAW_TYPE, os.path.join(vbase, bname, b"mdev_type", b"name"))
+    take(L.MRAW_LINK, os.path.join(vbase, bname), link=True)
+    parent = mdev_numa_parent(row[L.MRAW_LINK]) if not (st >> (8 + L.MRAW_LINK)) & 1 else None
+    if parent is not None:
+        take(L.MRAW_NUMA, os.path.join(pbase, parent, b"numa_node"))
+    return row, st
+
+
+def read_mdev_ids_raw(vgpu_base: str, pci_base: str, names) -> MdevRaw:
+    """The reads of read_mdev_tree_raw for the entries `names` in THAT order (a health re-scan's advertised vGPUs, any
+    form of name; an entry that is gone reads as a failed type read)."""
+    names, fields, state = list(names), [], []
+    vbase, pbase = os.fsencode(vgpu_base), os.fsencode(pci_base)
+    for name in names:
+        row, st = _read_mdev_entry_raw(vbase, pbase, name)
         fields += row
         state.append(st)
     return MdevRaw(names, *_pack_raw(fields, state, "the raw reads of %s" % vgpu_base))

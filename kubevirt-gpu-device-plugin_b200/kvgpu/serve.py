@@ -1207,9 +1207,28 @@ class KeyedVgpuHealthFeed(VgpuHealthFeed):
     transition of a UUID that was advertised on the previous tick; a new UUID is sent only when the kernel's health
     differs from what its plugin advertises.  Every advertised ID must be a canonical UUID (ValueError names the first
     that is not): a Walk-index handle is not a stable identity, so names that are not UUIDs need VgpuHealthFeed, whose
-    state follows the record index."""
+    state follows the record index.
+
+    raw=True runs the feed from raw reads, with no intern dict: `health_rescan_mdev(raw, xid_parents)` is
+    Context.health_rescan_mdev_raw, `snapshot(names)` returns an MdevRaw of `names` in that order
+    (plugin.read_mdev_ids_raw over the sysfs paths).  The advertised IDs are ordered by os.fsencode(ID) and may take
+    any form; the state is kept per name.  The queued bus ids go to the call as strings, matched byte for byte against
+    the parents the GPU decodes from the link targets, as the reference's gpuVgpuMap[busID] lookup matches them."""
+
+    def __init__(self, health_rescan_mdev, snapshot, plugins, gpus, period_s: float = 0.001, raw: bool = False):
+        super().__init__(health_rescan_mdev, snapshot, plugins, gpus, period_s)
+        self.raw = raw
 
     def tick(self) -> int:
+        if self.raw:
+            devs = _by_key(self.plugins, os.fsencode)
+            names = [d.ID for d, _ in devs]
+            raw = self.snapshot(names)
+            with self._lock:
+                buses, self._queued = self._queued, []
+            delta = self.health_rescan_mdev(raw, buses)
+            prev, self._uuids = self._uuids or frozenset(), frozenset(names)
+            return _send_keyed_health(devs, delta, prev)
         devs = _by_key(self.plugins, _uuid_key)
         uuids = [d.ID for d, _ in devs]
         snap = self.snapshot(uuids, self.intern)
@@ -1229,9 +1248,27 @@ class KeyedGroupHealthFeed(GroupHealthFeed):
     the advertised devices by packed BDF, snapshot them in that order, list the nodes, one keyed call, then each
     transition of an address advertised on the previous tick; a new address is sent only when the kernel's health
     differs from what its plugin advertises.  Every advertised ID must be a canonical BDF (ValueError names the first
-    that is not); other names need GroupHealthFeed."""
+    that is not); other names need GroupHealthFeed.
+
+    raw=True runs the feed from raw reads, with no intern dict: `health_rescan_groups(raw, nodes)` is
+    Context.health_rescan_groups_raw, `snapshot(names)` returns a PciRaw of `names` in that order
+    (plugin.read_pci_ids_raw over the sysfs tree) and `list_nodes()` the raw names of one listing of the VFIO directory
+    (plugin.list_nodes_raw).  The advertised IDs are ordered by os.fsencode(ID) and may take any form; the state is
+    kept per name, and a group's node is matched by its name's bytes, as the reference joins the directory with the
+    group string (generic_device_plugin.go:639-676)."""
+
+    def __init__(self, health_rescan_groups, snapshot, list_nodes, plugins, period_s: float = 0.001,
+                 raw: bool = False):
+        super().__init__(health_rescan_groups, snapshot, list_nodes, plugins, period_s)
+        self.raw = raw
 
     def tick(self) -> int:
+        if self.raw:
+            devs = _by_key(self.plugins, os.fsencode)
+            names = [d.ID for d, _ in devs]
+            delta = self.health_rescan_groups(self.snapshot(names), self.list_nodes())
+            prev, self._bdfs = self._bdfs or frozenset(), frozenset(names)
+            return _send_keyed_health(devs, delta, prev)
         devs = _by_key(self.plugins, _bdf_key)
         bdfs = [d.ID for d, _ in devs]
         snap = self.snapshot(bdfs, self.intern)

@@ -52,5 +52,5 @@ def build_delta(force: bool = False) -> str:
 
 
 if __name__ == "__main__":
-    for name in ("radix", "shard", "classify", "names", "delta"):
+    for name in ("radix", "shard", "classify", "names", "delta", "health_raw"):
         print(build(name, force=True))

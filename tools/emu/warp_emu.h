@@ -181,6 +181,10 @@ static inline uint32_t atomicMin(uint32_t* p, uint32_t v) {
   }
   return old;
 }
+static inline uint32_t atomicCAS(uint32_t* p, uint32_t cmp, uint32_t v) {
+  __atomic_compare_exchange_n(p, &cmp, v, false, __ATOMIC_SEQ_CST, __ATOMIC_SEQ_CST);
+  return cmp;  // the old value either way
+}
 static inline unsigned long long atomicCAS(unsigned long long* p, unsigned long long cmp, unsigned long long v) {
   __atomic_compare_exchange_n(p, &cmp, v, false, __ATOMIC_SEQ_CST, __ATOMIC_SEQ_CST);
   return cmp;  // the old value either way
