@@ -616,6 +616,82 @@ typedef struct kvg_alloc_raw {
 } kvg_alloc_raw;
 int kvg_pci_allocate_raw(kvg_ctx *ctx, const kvg_alloc_req *reqs, uint32_t n_reqs, const kvg_alloc_raw *raw,
                          uint32_t *first_bad, uint8_t *panic, uint8_t *egm_kept, uint8_t *egm_take);
+/* The passthrough plugin's AllocateResponse (generic_device_plugin.go:352-444) for every container request of one
+ * AllocateRequest, from the raw reads: kvg_pci_allocate_raw's decisions, then readVFIODev (:702-716) of every member,
+ * requestedDeviceFound, the device specs and the env value.  The host plans (bdfToIommu / iommuMap lookups), lists,
+ * reads and stats; it decides nothing.  `reqs` and `raw` are kvg_pci_allocate_raw's, with request r's members those of
+ * its visited IDs, ID after ID, each ID's group members in map order.
+ * Plan: request r visits its first in->n_visited[r] DevicesIDs; in->lookup_error[r] = 1 when its next ID misses
+ * bdfToIommu or has an empty iommuMap entry.  in->id_members[v] is the member count of visited ID v (request after
+ * request); the counts of request r add up to reqs[r].n_members.
+ * Members: addr_bytes[addr_off[i] .. addr_off[i + 1]) is dev.addr as the maps hold it.  The vfio-dev listing of member
+ * i is entries vfio_first[i] .. vfio_first[i + 1], in any order: name vfio_bytes[vfio_off[e] .. vfio_off[e + 1]) and
+ * vfio_dir[e] = DirEntry.IsDir() (a link is not a directory).  vfio_state[i]: KVG_AVFIO_MADE when the listing was
+ * made, | KVG_AVFIO_FAILED when os.ReadDir failed (the host keeps the OS error text).  It is reached when iommufd = 1
+ * (supportsIOMMUFD; its other errors are raised by the host before the call) and the member passed the re-check.
+ * Rules, per request in the reference's order (visited ID k, then its members):
+ *   member    the re-check of kvg_pci_allocate_raw fails it: UNKNOWN_MEMBER, or PANIC for the vendor read's panic;
+ *             then, with iommufd, readVFIODev: a failed listing is VFIO_READ; else the byte-wise least name with the
+ *             prefix "vfio" among the entries that are directories, none being VFIO_NONE ("no iommufd device found")
+ *   ID        after its members: no member whose dev.addr equals the ID byte for byte is UNKNOWN_ID
+ *   request   after the visited IDs: lookup_error is UNKNOWN_ID at n_visited
+ *   specs     per visited ID: /dev/vfio/devices/<name> per member (iommufd), /dev/vfio/vfio,
+ *             filepath.Join("/dev/vfio", group) ("" and "." give /dev/vfio, ".." gives /dev), /dev/iommu (iommufd);
+ *             then /dev/<name> of the EGM entries the request takes (kvg_pci_allocate_raw's rule), ascending.  A host
+ *             path is kept at its first occurrence (appendDeviceSpec); container path = host path, permissions "mrw".
+ *   env       envList outlives the request loop (:361): response r's value is the addresses of every member of
+ *             requests 0..r joined by ',' (duplicates kept), a prefix of env_bytes of env_len[r] bytes; env_key[r] = 1
+ *             iff requests 0..r visited an ID (else envs is empty).
+ * Requests are decided independently; the caller returns the error of the first request whose error is not OK.
+ * error_at[r]: the ID index within the request for UNKNOWN_ID, the member position within the request for the
+ * other errors, 0 for OK.
+ * Output: *res, library-owned (kvg_result_free).  Request r's specs are spec_span[2s] (offset into spec_bytes) and
+ * spec_span[2s + 1] (length) for s in spec_first[r] .. spec_first[r] + n_specs[r]; an erring request has none.
+ * Launches: k_araw_members when there are members; k_aresp_members when there are members or two EGM entries;
+ * k_araw_keys when there are EGM entries; k_pci_allocate_check and k_aresp_requests when there are requests, so at
+ * most five, none for a call with no requests and no EGM entries (*res is an empty result) or one refused before
+ * launch.  One host synchronisation per call that launches; the outputs land in mapped host memory sized on the host
+ * from the inputs.  The call uses buffers of its own: no scan, fetch, delta, health or name-table state changes, and
+ * it does not wait for a pci.ids parse.
+ * Errors (*res unwritten):
+ *   KVG_EINVAL  before launch: every argument refusal of kvg_pci_allocate_raw; in or res NULL; a plan or listing table
+ *               NULL with entries; vfio_first or vfio_off not starting at 0 or decreasing; visit counts that do not
+ *               add up; n_visited + lookup_error > n_ids; a visited ID with no members.  Found on the device, in this
+ *               order: members of one visited ID with different group strings, or a group string holding '/'; EGM
+ *               entry names that do not ascend strictly byte-wise; then kvg_pci_allocate_raw's refusals in its order,
+ *               a reached listing that was not made taking its place beside a request's missing member read
+ *               (kvg_last_error names the entry).
+ *   KVG_ERANGE  kvg_pci_allocate_raw's key cap; a response of more than 2^32 - 1 spec slots or pool bytes. */
+enum { KVG_ARESP_OK, KVG_ARESP_UNKNOWN_ID, KVG_ARESP_UNKNOWN_MEMBER, KVG_ARESP_PANIC, KVG_ARESP_VFIO_READ,
+       KVG_ARESP_VFIO_NONE };
+enum { KVG_AVFIO_MADE = 1, KVG_AVFIO_FAILED = 2 };
+typedef struct kvg_alloc_resp_in {
+  uint32_t iommufd;             /* supportsIOMMUFD: 0 or 1 */
+  const uint32_t *n_visited;    /* [n_reqs] */
+  const uint8_t *lookup_error;  /* [n_reqs] */
+  const uint32_t *id_members;   /* [sum of n_visited] */
+  const uint32_t *addr_off;     /* [n_members + 1] */
+  const uint8_t *addr_bytes;
+  const uint32_t *vfio_first;   /* [n_members + 1] */
+  const uint32_t *vfio_off;     /* [vfio_first[n_members] + 1] */
+  const uint8_t *vfio_bytes;
+  const uint8_t *vfio_dir;      /* [vfio_first[n_members]] */
+  const uint8_t *vfio_state;    /* [n_members] */
+} kvg_alloc_resp_in;
+typedef struct kvg_alloc_resp {
+  uint32_t n_reqs;
+  const uint8_t *error;         /* [n_reqs] KVG_ARESP_* */
+  const uint32_t *error_at;     /* [n_reqs] */
+  const uint32_t *spec_first;   /* [n_reqs] */
+  const uint32_t *n_specs;      /* [n_reqs] */
+  const uint32_t *spec_span;    /* [2 * spec slots] */
+  const uint8_t *spec_bytes;
+  const uint32_t *env_len;      /* [n_reqs] */
+  const uint8_t *env_key;       /* [n_reqs] */
+  const uint8_t *env_bytes;
+} kvg_alloc_resp;
+int kvg_pci_allocate_response(kvg_ctx *ctx, const kvg_alloc_req *reqs, uint32_t n_reqs, const kvg_alloc_raw *raw,
+                              const kvg_alloc_resp_in *in, kvg_alloc_resp **res);
 /* GetPreferredAllocation of the passthrough plugin (generic_device_plugin.go:470-608): the NUMA packing of every
  * container request of one PreferredAllocationRequest, in one launch.
  * Entries: request r's entries follow those of requests 0..r-1 in `ids`, its n_must must-include IDs first, then its

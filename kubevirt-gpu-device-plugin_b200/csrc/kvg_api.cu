@@ -35,6 +35,7 @@
 #include "kvg_alloc.cuh"
 #include "kvg_snap.cuh"
 #include "kvg_alloc_raw.cuh"
+#include "kvg_alloc_resp.cuh"
 
 using namespace kvg;
 

@@ -1170,3 +1170,216 @@ func vendorPanic(data []byte) (p interface{}) {
 	_ = strings.Trim(string(data[2:]), "\n")
 	return nil
 }
+
+// allocVisit is one DevicesID a container request visits: the ID, the group bdfToIommu holds for it and that
+// group's iommuMap members in map order.
+type allocVisit struct {
+	bdf, group string
+	addrs      []string
+}
+
+// allocPlan is one container request's plan from the map lookups: its DevicesIDs, the IDs visited in order, and
+// whether the ID after them misses the maps (the reference's first "unknown device" before any read).
+type allocPlan struct {
+	ids       []string
+	visits    []allocVisit
+	lookupErr bool
+}
+
+// allocateResponseGPU is the passthrough plugin's whole Allocate (generic_device_plugin.go:352-444) after the map
+// lookups, in one kvg_pci_allocate_response call (Python twin: kvgpu/serve.py AllocateResponder, tested against the
+// replay with AllocateRawCheck by tests/test_serve_allocate_response.py).  Every planned member's iommu_group link
+// target, vendor contents and, with iommufd, vfio-dev listing (os.ReadDir; each entry's DirEntry.IsDir(), which does
+// not follow links) are read raw; the library decides the re-check, readVFIODev, requestedDeviceFound, the device
+// specs with appendDeviceSpec's de-duplication, the env value and the EGM paths.  Go formats the first failing
+// request's error, re-raises a reported vendor panic as the runtime.Error vendorPanic recovers from the same bytes,
+// and otherwise builds the ContainerAllocateResponses.  iommufd is supportsIOMMUFD's result; its other errors stay
+// with the caller.  Like the rest of the file it is source only and has not been compiled.
+func allocateResponseGPU(deviceName string, plans []allocPlan, iommufd bool, egm []EGMEntryRaw) ([]*pluginapi.ContainerAllocateResponse, error) {
+	if len(plans) == 0 && len(egm) == 0 {
+		return nil, nil
+	}
+	var mOff, iOff, eOff, aOff, vFirst, vOff []uint32
+	var mBytes, iBytes, eBytes, aBytes, vBytes, vDir, vState []byte
+	var mState, eState []uint16
+	var vendors [][]byte   // per member, the vendor contents as read
+	var listErrs []error   // per member, the listing's error
+	var addrs [][]string   // per request, its members' addresses in order
+	push := func(off *[]uint32, b *[]byte, data []byte) {
+		if len(*off) == 0 {
+			*off = append(*off, 0)
+		}
+		*b = append(*b, data...)
+		*off = append(*off, uint32(len(*b)))
+	}
+	reqs := make([]C.kvg_alloc_req, len(plans))
+	nVisited := make([]uint32, len(plans))
+	lookup := make([]byte, len(plans))
+	var idMembers []uint32
+	vFirst = append(vFirst, 0)
+	for r, p := range plans {
+		var ra []string
+		for _, v := range p.visits {
+			idMembers = append(idMembers, uint32(len(v.addrs)))
+			for _, addr := range v.addrs {
+				st := uint16(1<<C.KVG_AMEM_LINK | 1<<C.KVG_AMEM_VENDOR)
+				target, err := os.Readlink(filepath.Join(basePath, addr, "iommu_group"))
+				if err != nil {
+					st |= 1 << (8 + C.KVG_AMEM_LINK)
+				}
+				vendor, err := os.ReadFile(filepath.Join(basePath, addr, "vendor"))
+				if err != nil {
+					st |= 1 << (8 + C.KVG_AMEM_VENDOR)
+				}
+				push(&mOff, &mBytes, []byte(target))
+				push(&mOff, &mBytes, vendor)
+				push(&mOff, &mBytes, []byte(v.group))
+				mState = append(mState, st)
+				vendors = append(vendors, vendor)
+				push(&aOff, &aBytes, []byte(addr))
+				var lerr error
+				ls := byte(0)
+				if iommufd {
+					ls = C.KVG_AVFIO_MADE
+					entries, err := os.ReadDir(filepath.Join(basePath, addr, "vfio-dev"))
+					if err != nil {
+						ls |= C.KVG_AVFIO_FAILED
+						lerr = err
+					}
+					for _, e := range entries {
+						push(&vOff, &vBytes, []byte(e.Name()))
+						d := byte(0)
+						if e.IsDir() {
+							d = 1
+						}
+						vDir = append(vDir, d)
+					}
+				}
+				vState = append(vState, ls)
+				vFirst = append(vFirst, uint32(len(vDir)))
+				listErrs = append(listErrs, lerr)
+				ra = append(ra, addr)
+			}
+		}
+		for _, id := range p.ids {
+			push(&iOff, &iBytes, []byte(id))
+		}
+		reqs[r] = C.kvg_alloc_req{n_members: C.uint32_t(len(ra)), n_ids: C.uint32_t(len(p.ids))}
+		nVisited[r] = uint32(len(p.visits))
+		if p.lookupErr {
+			lookup[r] = 1
+		}
+		addrs = append(addrs, ra)
+	}
+	for _, e := range egm {
+		st := uint16(1<<C.KVG_AEGM_GPUS | 1<<C.KVG_AEGM_STAT)
+		if e.GPUErr != nil {
+			st |= 1 << (8 + C.KVG_AEGM_GPUS)
+		}
+		if e.StatErr != nil {
+			st |= 1 << (8 + C.KVG_AEGM_STAT)
+		}
+		push(&eOff, &eBytes, []byte(e.Name))
+		push(&eOff, &eBytes, e.GPUDevices)
+		eState = append(eState, st)
+	}
+	// C copies of every table and byte array (cgo pointer rule): &raw and &in, Go values, hold no Go pointer
+	var cmem []unsafe.Pointer
+	defer func() {
+		for _, p := range cmem {
+			C.free(p)
+		}
+	}()
+	cCopy := func(b []byte) unsafe.Pointer {
+		if len(b) == 0 {
+			return nil
+		}
+		p := C.CBytes(b)
+		cmem = append(cmem, p)
+		return p
+	}
+	u32 := func(v []uint32) *C.uint32_t {
+		if len(v) == 0 {
+			return nil
+		}
+		return (*C.uint32_t)(cCopy(unsafe.Slice((*byte)(unsafe.Pointer(&v[0])), 4*len(v))))
+	}
+	u16 := func(v []uint16) *C.uint16_t {
+		if len(v) == 0 {
+			return nil
+		}
+		return (*C.uint16_t)(cCopy(unsafe.Slice((*byte)(unsafe.Pointer(&v[0])), 2*len(v))))
+	}
+	u8 := func(v []byte) *C.uint8_t { return (*C.uint8_t)(cCopy(v)) }
+	var raw C.kvg_alloc_raw
+	raw.n_members = C.size_t(len(mState))
+	raw.member_off, raw.member_state, raw.member_bytes = u32(mOff), u16(mState), u8(mBytes)
+	if len(iOff) > 0 {
+		raw.n_ids = C.size_t(len(iOff) - 1)
+	}
+	raw.id_off, raw.id_bytes = u32(iOff), u8(iBytes)
+	raw.n_egm = C.uint32_t(len(egm))
+	raw.egm_off, raw.egm_state, raw.egm_bytes = u32(eOff), u16(eState), u8(eBytes)
+	if len(vOff) == 0 {
+		vOff = append(vOff, 0)
+	}
+	var in C.kvg_alloc_resp_in
+	if iommufd {
+		in.iommufd = 1
+	}
+	in.n_visited, in.lookup_error, in.id_members = u32(nVisited), u8(lookup), u32(idMembers)
+	in.addr_off, in.addr_bytes = u32(aOff), u8(aBytes)
+	in.vfio_first, in.vfio_off, in.vfio_bytes = u32(vFirst), u32(vOff), u8(vBytes)
+	in.vfio_dir, in.vfio_state = u8(vDir), u8(vState)
+	kvgMu.Lock()
+	defer kvgMu.Unlock()
+	if err := kvgEnsure(); err != nil {
+		return nil, err
+	}
+	var reqPtr *C.kvg_alloc_req
+	if len(reqs) > 0 {
+		reqPtr = &reqs[0]
+	}
+	var res *C.kvg_alloc_resp
+	if rc := C.kvg_pci_allocate_response(kvgCtx, reqPtr, C.uint32_t(len(reqs)), &raw, &in, &res); rc != C.KVG_OK {
+		return nil, fmt.Errorf("kvg_pci_allocate_response: %d %s", int(rc), C.GoString(C.kvg_last_error(kvgCtx)))
+	}
+	defer C.kvg_result_free(unsafe.Pointer(res))
+	n := len(plans)
+	errKind := unsafe.Slice((*uint8)(unsafe.Pointer(res.error)), n)
+	errAt := unsafe.Slice((*uint32)(unsafe.Pointer(res.error_at)), n)
+	specFirst := unsafe.Slice((*uint32)(unsafe.Pointer(res.spec_first)), n)
+	nSpecs := unsafe.Slice((*uint32)(unsafe.Pointer(res.n_specs)), n)
+	envLen := unsafe.Slice((*uint32)(unsafe.Pointer(res.env_len)), n)
+	envKey := unsafe.Slice((*uint8)(unsafe.Pointer(res.env_key)), n)
+	key := fmt.Sprintf("%s_%s", gpuPrefix, strings.ToUpper(deviceName))
+	out := make([]*pluginapi.ContainerAllocateResponse, 0, n)
+	for r, m0 := 0, 0; r < n; m0, r = m0+len(addrs[r]), r+1 {
+		at := int(errAt[r])
+		switch errKind[r] {
+		case C.KVG_ARESP_UNKNOWN_ID:
+			return nil, fmt.Errorf("invalid allocation request: unknown device: %s", plans[r].ids[at])
+		case C.KVG_ARESP_UNKNOWN_MEMBER:
+			return nil, fmt.Errorf("invalid allocation request: unknown device: %s", addrs[r][at])
+		case C.KVG_ARESP_PANIC:
+			panic(vendorPanic(vendors[m0+at]))
+		case C.KVG_ARESP_VFIO_READ:
+			return nil, fmt.Errorf("could not determine iommufd device for device %s: %v", addrs[r][at], listErrs[m0+at])
+		case C.KVG_ARESP_VFIO_NONE:
+			return nil, fmt.Errorf("could not determine iommufd device for device %s: %v", addrs[r][at],
+				errors.New("no iommufd device found"))
+		}
+		specs := make([]*pluginapi.DeviceSpec, 0, int(nSpecs[r]))
+		spans := unsafe.Slice((*uint32)(unsafe.Pointer(res.spec_span)), 2*(int(specFirst[r])+int(nSpecs[r])))
+		for s := int(specFirst[r]); s < int(specFirst[r])+int(nSpecs[r]); s++ {
+			p := C.GoStringN((*C.char)(unsafe.Add(unsafe.Pointer(res.spec_bytes), spans[2*s])), C.int(spans[2*s+1]))
+			specs = append(specs, &pluginapi.DeviceSpec{HostPath: p, ContainerPath: p, Permissions: "mrw"})
+		}
+		envs := map[string]string{}
+		if envKey[r] != 0 {
+			envs[key] = C.GoStringN((*C.char)(unsafe.Pointer(res.env_bytes)), C.int(envLen[r]))
+		}
+		out = append(out, &pluginapi.ContainerAllocateResponse{Envs: envs, Devices: specs})
+	}
+	return out, nil
+}

@@ -22,6 +22,8 @@ MRAW_NAME, MRAW_TYPE, MRAW_LINK, MRAW_NUMA, MRAW_FIELDS = range(5)
 AMEM_LINK, AMEM_VENDOR, AMEM_GROUP, AMEM_FIELDS = range(4)
 AEGM_NAME, AEGM_GPUS, AEGM_FIELDS = range(3)
 AEGM_STAT = AEGM_FIELDS
+ARESP_OK, ARESP_UNKNOWN_ID, ARESP_UNKNOWN_MEMBER, ARESP_PANIC, ARESP_VFIO_READ, ARESP_VFIO_NONE = range(6)
+AVFIO_MADE, AVFIO_FAILED = 1, 2
 KVG_NO_NAME = 0xFFFFFFFF
 ERR_NAMES = {0: "KVG_OK", -1: "KVG_EINVAL", -2: "KVG_ECUDA", -3: "KVG_ENOMEM", -4: "KVG_ENCCL",
              -5: "KVG_ESTATE", -6: "KVG_ERANGE", -7: "KVG_EPANIC"}
@@ -88,6 +90,19 @@ class AllocRawC(C.Structure):
     _fields_ = [("n_members", C.c_size_t), ("member_off", C.c_void_p), ("member_bytes", C.c_void_p),
                 ("member_state", C.c_void_p), ("n_ids", C.c_size_t), ("id_off", C.c_void_p), ("id_bytes", C.c_void_p),
                 ("n_egm", C.c_uint32), ("egm_off", C.c_void_p), ("egm_bytes", C.c_void_p), ("egm_state", C.c_void_p)]
+
+
+class AllocRespInC(C.Structure):
+    _fields_ = [("iommufd", C.c_uint32), ("n_visited", C.c_void_p), ("lookup_error", C.c_void_p),
+                ("id_members", C.c_void_p), ("addr_off", C.c_void_p), ("addr_bytes", C.c_void_p),
+                ("vfio_first", C.c_void_p), ("vfio_off", C.c_void_p), ("vfio_bytes", C.c_void_p),
+                ("vfio_dir", C.c_void_p), ("vfio_state", C.c_void_p)]
+
+
+class AllocRespC(C.Structure):
+    _fields_ = [("n_reqs", C.c_uint32), ("error", C.c_void_p), ("error_at", C.c_void_p), ("spec_first", C.c_void_p),
+                ("n_specs", C.c_void_p), ("spec_span", C.c_void_p), ("spec_bytes", C.c_void_p),
+                ("env_len", C.c_void_p), ("env_key", C.c_void_p), ("env_bytes", C.c_void_p)]
 
 
 class PciSnapC(C.Structure):
@@ -206,6 +221,7 @@ def load() -> C.CDLL:
         "kvg_preferred_allocation": (C.c_int, [vp, vp, u32, vp, sz, vp, vp]),
         "kvg_pci_allocate_check": (C.c_int, [vp, vp, u32, vp, vp, sz, vp, sz, vp, vp, u32, u32, vp, vp]),
         "kvg_pci_allocate_raw": (C.c_int, [vp, vp, u32, P(AllocRawC), vp, vp, vp, vp]),
+        "kvg_pci_allocate_response": (C.c_int, [vp, vp, u32, P(AllocRawC), P(AllocRespInC), P(P(AllocRespC))]),
         "kvg_health_rescan": (C.c_int, [vp, vp, sz, P(P(HealthDeltaC))]),
         "kvg_health_reset": (C.c_int, [vp]),
         "kvg_health_rescan_mdev": (C.c_int, [vp, vp, sz, u32, vp, sz, P(P(HealthDeltaC))]),

@@ -430,6 +430,47 @@ class Context:
                                                 take.ctypes.data))
         return first_bad, panic.astype(bool), kept.astype(bool), take.astype(bool)
 
+    def pci_allocate_response(self, raw, resp) -> list:
+        """The passthrough plugin's AllocateResponse for every container request of one call, from the raw reads
+        (include/kvgpu.h kvg_pci_allocate_response; plugin.pack_alloc_response builds `raw` and `resp`).  Returns per
+        request (error, at, paths, env): error = ARESP_*, at = its DevicesID index (ARESP_UNKNOWN_ID) or member
+        position; paths = the device specs' host paths (bytes), in order; env = the env value (bytes), or None when
+        the key is absent.  Raises KvgError for a refusal (KVG_EINVAL, KVG_ERANGE)."""
+        arr = lambda a, t: np.ascontiguousarray(a, dtype=t)   # noqa: E731
+        blob = lambda b: np.frombuffer(bytes(b) + b"\0", dtype=np.uint8)   # noqa: E731
+        n_members, n_ids = arr(raw.n_members, np.uint32), arr(raw.n_ids, np.uint32)
+        moff, mst, ioff = arr(raw.member_off, np.uint32), arr(raw.member_state, np.uint16), arr(raw.id_off, np.uint32)
+        eoff, est = arr(raw.egm_off, np.uint32), arr(raw.egm_state, np.uint16)
+        mb, ib, eb = blob(raw.member_bytes), blob(raw.id_bytes), blob(raw.egm_bytes)
+        if not len(n_members) == len(n_ids) == len(resp.n_visited) == len(resp.lookup_error):
+            raise ValueError("pci_allocate_response: %d / %d / %d / %d per-request counts"
+                             % (len(n_members), len(n_ids), len(resp.n_visited), len(resp.lookup_error)))
+        reqs = np.zeros(len(n_members), dtype=L.ALLOC_REQ)
+        reqs["n_members"], reqs["n_ids"] = n_members, n_ids
+        arg = L.AllocRawC(len(mst), moff.ctypes.data, mb.ctypes.data, mst.ctypes.data, max(len(ioff) - 1, 0),
+                          ioff.ctypes.data, ib.ctypes.data, len(est), eoff.ctypes.data, eb.ctypes.data, est.ctypes.data)
+        keep = [arr(resp.n_visited, np.uint32), arr(resp.lookup_error, np.uint8), arr(resp.id_members, np.uint32),
+                arr(resp.addr_off, np.uint32), blob(resp.addr_bytes), arr(resp.vfio_first, np.uint32),
+                arr(resp.vfio_off, np.uint32), blob(resp.vfio_bytes), arr(resp.vfio_dir, np.uint8),
+                arr(resp.vfio_state, np.uint8)]
+        rin = L.AllocRespInC(int(resp.iommufd), *[a.ctypes.data for a in keep])
+        out = C.POINTER(L.AllocRespC)()
+        self._ck(self._lib.kvg_pci_allocate_response(self._h, reqs.ctypes.data, len(reqs), C.byref(arg),
+                                                     C.byref(rin), C.byref(out)))
+        o = out.contents
+        n = len(reqs)
+        error, at = L._arr(o.error, n, np.uint8), L._arr(o.error_at, n, np.uint32)
+        first, n_specs = L._arr(o.spec_first, n, np.uint32), L._arr(o.n_specs, n, np.uint32)
+        env_len, env_key = L._arr(o.env_len, n, np.uint32), L._arr(o.env_key, n, np.uint8)
+        res = []
+        for r in range(n):
+            span = L._arr(o.spec_span + 8 * int(first[r]), 2 * int(n_specs[r]), np.uint32) if n_specs[r] else []
+            paths = [C.string_at(o.spec_bytes + int(span[2 * k]), int(span[2 * k + 1])) for k in range(int(n_specs[r]))]
+            env = C.string_at(o.env_bytes, int(env_len[r])) if env_key[r] else None
+            res.append((int(error[r]), int(at[r]), paths, env))
+        self._lib.kvg_result_free(out)
+        return res
+
     def preferred_allocation(self, ids, n_must, n_avail, sizes) -> list:
         """GetPreferredAllocation's NUMA packing for every container request of one call, one launch
         (include/kvgpu.h kvg_preferred_allocation).  ids: PREF_ID entries, request after request, each request's

@@ -374,6 +374,60 @@ def pack_alloc_raw(requests, egm_entries) -> AllocRaw:
                     *_pack_raw(eparts, estate, what))
 
 
+@dataclass
+class AllocRespIn:
+    """The plan and the vfio-dev listings of one AllocateRequest (include/kvgpu.h kvg_alloc_resp_in): iommufd, then
+    per request the visited DevicesIDs and the lookup error after them, per visited ID its member count, per member
+    dev.addr, its listing's entries (name, IsDir) and the listing's made / failed bits."""
+    iommufd: int
+    n_visited: np.ndarray   # u32 [n_reqs]
+    lookup_error: np.ndarray  # u8 [n_reqs]
+    id_members: np.ndarray  # u32 [visited IDs]
+    addr_off: np.ndarray    # u32 [n + 1]
+    addr_bytes: bytes
+    vfio_first: np.ndarray  # u32 [n + 1]
+    vfio_off: np.ndarray    # u32 [entries + 1]
+    vfio_bytes: bytes
+    vfio_dir: np.ndarray    # u8 [entries]
+    vfio_state: np.ndarray  # u8 [n]
+
+
+def pack_alloc_response(requests, egm_entries, iommufd: bool):
+    """requests: [(ids, visits, lookup_error)] in request order: ids = the DevicesIDs, visits = per visited ID its
+    members in map order, each (addr, link target, vendor contents, group string, listing), lookup_error = the ID after
+    the visited ones misses the maps.  A listing is [(name, is_dir)] in any order, None (os.ReadDir failed) or
+    NOT_READ; the other reads as pack_alloc_raw takes them.  -> (AllocRaw, AllocRespIn)."""
+    enc = lambda v: os.fsencode(v) if isinstance(v, str) else v   # noqa: E731
+    raw_reqs, n_visited, lookup, id_members, addrs, first, names, dirs, state = [], [], [], [], [], [0], [], [], []
+    for ids, visits, lookup_error in requests:
+        members = []
+        for visit in visits:
+            id_members.append(len(visit))
+            for addr, link, vendor, group, listing in visit:
+                members.append((link, vendor, group))
+                addrs.append(enc(addr))
+                if listing is NOT_READ:
+                    state.append(0)
+                elif listing is None:
+                    state.append(L.AVFIO_MADE | L.AVFIO_FAILED)
+                else:
+                    state.append(L.AVFIO_MADE)
+                    for name, is_dir in listing:
+                        names.append(enc(name))
+                        dirs.append(1 if is_dir else 0)
+                first.append(len(names))
+        raw_reqs.append((members, list(ids)))
+        n_visited.append(len(visits))
+        lookup.append(1 if lookup_error else 0)
+    what = "the raw reads"
+    aoff, ab, _ = _pack_raw(addrs, (), what)
+    voff, vb, _ = _pack_raw(names, (), what)
+    return pack_alloc_raw(raw_reqs, egm_entries), AllocRespIn(
+        1 if iommufd else 0, np.array(n_visited, dtype=np.uint32), np.array(lookup, dtype=np.uint8),
+        np.array(id_members, dtype=np.uint32), aoff, ab, np.array(first, dtype=np.uint32), voff, vb,
+        np.array(dirs, dtype=np.uint8), np.array(state, dtype=np.uint8))
+
+
 def snapshot_pci_ids(base_path: str, bdfs, intern: dict) -> PciSnapshot:
     """Snapshot the PCI devices `bdfs` in THAT order (the health re-scan's fixed record order; a Walk would re-index
     when one vanishes), with the readers and flag rules of snapshot_pci_tree.  An address whose entry is gone reads as

@@ -37,9 +37,10 @@ import numpy as np
 
 from . import _lib as L
 from . import dpapi
-from .plugin import (DEVICE_NAMESPACE, GPU_PREFIX, VGPU_PREFIX, Maps, PluginSpec, ReferencePanic, _read_id,
+from .plugin import (DEVICE_NAMESPACE, GPU_PREFIX, NOT_READ, VGPU_PREFIX, Maps, PluginSpec, ReferencePanic, _read_id,
                      _read_link, _read_raw, _read_vgpu_raw, _rebuild_mdev_maps, _rebuild_pci_maps, apply_mdev_delta,
-                     apply_pci_delta, format_uuid, pack_alloc_raw, parse_bdf, plugin_specs_from_maps)
+                     apply_pci_delta, format_uuid, pack_alloc_raw, pack_alloc_response, parse_bdf,
+                     plugin_specs_from_maps)
 
 VFIO_DEVICE_PATH = "/dev/vfio"      # generic_device_plugin.go:54
 IOMMU_DEVICE_PATH = "/dev/iommu"    # :55
@@ -219,6 +220,17 @@ def read_vfio_dev(base_path: str, addr: str) -> str:
         if os.path.isdir(os.path.join(d, name)) and name.startswith("vfio"):
             return name
     raise OSError("no iommufd device found")
+
+
+def read_vfio_dev_raw(base_path: str, addr: str):
+    """The listing readVFIODev makes (:702-716), deciding nothing: ([(name bytes, IsDir)], None) in listing order,
+    IsDir not following links as DirEntry.IsDir() does, or (None, the error text) when the listing fails."""
+    d = os.path.join(os.fsencode(base_path), os.fsencode(addr), b"vfio-dev")
+    try:
+        with os.scandir(d) as it:
+            return [(e.name, e.is_dir(follow_symlinks=False)) for e in it], None
+    except OSError as e:     # the text read_vfio_dev's os.listdir raises for the same path
+        return None, str(OSError(e.errno, e.strerror, os.fsdecode(d)))
 
 
 # ------------------------------------------------------------------------------------------------
@@ -433,6 +445,65 @@ class AllocateRawCheck:
         return out
 
 
+class AllocateResponder:
+    """The passthrough plugin's whole Allocate (generic_device_plugin.go:352-444) after the plan, in ONE call
+    (Context.pci_allocate_response): a drop-in `allocate_response` for GenericDevicePlugin, whose `discover_egm` is
+    discover_egm_raw.  GenericDevicePlugin.Allocate's replay with AllocateRawCheck stays as the reference it is tested
+    against.
+
+    Every planned member's iommu_group link, vendor and (with iommufd) vfio-dev listing are read raw; with the plan,
+    the DevicesIDs and the EGM class entries they go to the call, which returns per request the reference's first
+    error or the device specs and the env value.  Here the error texts are formatted and the response is built;
+    nothing is decided."""
+
+    def __init__(self, call, base_path: str = "/sys/bus/pci/devices"):
+        self.call, self.base_path = call, base_path
+
+    def _read(self, addr, prop, link):
+        return _read_raw(os.path.join(os.fsencode(self.base_path), os.fsencode(addr), prop), link)
+
+    def __call__(self, device_name, requests, iommufd, egm_entries):
+        """requests: [(devices_ids, plan, lookup_error_at)] with GenericDevicePlugin._plan's plan; iommufd:
+        supports_iommufd; egm_entries: discover_egm_raw's entries (None or [] for none).  Returns the
+        AllocateResponse, or raises AllocateError / ReferencePanic with the reference's text."""
+        errors, packed = {}, []
+        for r, (ids, plan, lookup_error_at) in enumerate(requests):
+            visits = []
+            for _, group, members in plan:
+                visit = []
+                for dev in members:
+                    listing = NOT_READ
+                    if iommufd:
+                        listing, text = read_vfio_dev_raw(self.base_path, dev.addr)
+                        if text is not None:
+                            errors[(r, dev.addr)] = text
+                    visit.append((dev.addr, self._read(dev.addr, b"iommu_group", True),
+                                  self._read(dev.addr, b"vendor", False), group, listing))
+                visits.append(visit)
+            packed.append((ids, visits, lookup_error_at is not None))
+        egm = [(e.name, e.gpu_devices, e.stat) for e in (egm_entries or [])]
+        decided = self.call(*pack_alloc_response(packed, egm, iommufd))
+        responses = dpapi.AllocateResponse()
+        key = "%s_%s" % (GPU_PREFIX, device_name.upper())
+        for r, (error, at, paths, env) in enumerate(decided):
+            ids, plan, _ = requests[r]
+            addr = lambda p: [d.addr for _, _, members in plan for d in members][p]   # noqa: E731
+            if error == L.ARESP_UNKNOWN_ID:
+                raise AllocateError("invalid allocation request: unknown device: %s" % ids[at])
+            if error == L.ARESP_UNKNOWN_MEMBER:
+                raise AllocateError("invalid allocation request: unknown device: %s" % addr(at))
+            if error == L.ARESP_PANIC:
+                raise ReferencePanic("slice bounds out of range reading %s/vendor" % addr(at))
+            if error in (L.ARESP_VFIO_READ, L.ARESP_VFIO_NONE):
+                why = errors[(r, addr(at))] if error == L.ARESP_VFIO_READ else "no iommufd device found"
+                raise AllocateError("could not determine iommufd device for device %s: %s" % (addr(at), why))
+            specs = [dpapi.DeviceSpec(host_path=os.fsdecode(p), container_path=os.fsdecode(p), permissions="mrw")
+                     for p in paths]
+            envs = {key: os.fsdecode(env)} if env is not None else {}
+            responses.container_responses.append(dpapi.ContainerAllocateResponse(envs=envs, devices=specs))
+        return responses
+
+
 # ------------------------------------------------------------------------------------------------
 # the plugins
 # ------------------------------------------------------------------------------------------------
@@ -586,16 +657,18 @@ class GenericDevicePlugin(_PluginBase):
     returnBdfToIommuMap supply in the reference; `revalidate` is the Allocate-time re-check
     (GroupCheck, or BatchRevalidator over a scan function); `allocate_check` (AllocateCheck), when set, takes every
     Allocate decision of an AllocateRequest in one GPU call instead: the re-check and the EGM match of every container
-    request; `prefer` answers GetPreferredAllocation
+    request; `allocate_response` (AllocateResponder), when set, builds the whole AllocateResponse of an AllocateRequest
+    in one GPU call after the plan; `prefer` answers GetPreferredAllocation
     (NumaPacker: every container request in one GPU call; None: preferred_allocation per request on the CPU)."""
 
     def __init__(self, device_name, device_path, devs, maps: Maps, *, revalidate=None,
                  base_path="/sys/bus/pci/devices", root_path="/", discover_egm=None, prefer=None, allocate_check=None,
-                 **kw):
+                 allocate_response=None, **kw):
         super().__init__(device_name, devs, **kw)
         self.device_path, self.maps = device_path, maps
         self.base_path, self.root_path = base_path, root_path
         self.revalidate, self.prefer, self.allocate_check = revalidate, prefer, allocate_check
+        self.allocate_response = allocate_response
         self.discover_egm = discover_egm or (lambda: discover_egm_devices(self.root_path))
 
     def GetPreferredAllocation(self, request, context):
@@ -632,7 +705,7 @@ class GenericDevicePlugin(_PluginBase):
         of them all; each request is then replayed in the reference's order, so the first error of the first failing
         request wins.  Otherwise the per-device re-validation of each request is handed to `self.revalidate` as one
         batch, and the EGM match is the CPU rule."""
-        if self.revalidate is None and self.allocate_check is None:
+        if self.revalidate is None and self.allocate_check is None and self.allocate_response is None:
             raise AllocateError("no re-validation function configured (the scan context is required)")
         responses = dpapi.AllocateResponse()
         env_list = {}                       # declared OUTSIDE the request loop in the reference (:361)
@@ -642,6 +715,10 @@ class GenericDevicePlugin(_PluginBase):
         except Exception:                   # :366-370 a discovery failure only disables EGM mounts
             egm_devices = None
         reqs = list(request.container_requests)
+        if self.allocate_response is not None:
+            return self.allocate_response(self.device_name,
+                                          [(list(req.devices_ids),) + self._plan(req) for req in reqs], iommufd,
+                                          egm_devices)
         plans = decided = None
         if self.allocate_check is not None:
             plans = [self._plan(req) for req in reqs]
